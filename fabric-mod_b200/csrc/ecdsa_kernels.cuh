@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include "ecdsa_verify.cuh"
 #include "ecdsa_batchaffine.cuh"
+#include "fieldops.cuh"
 
 namespace fabgpu {
 
@@ -639,24 +640,13 @@ __global__ void table_entries_kernel(const aff* __restrict__ tab, int wbits, con
     if (i < n) out[i] = tab[(size_t)window[i] * ((1u << wbits) - 1u) + (digit[i] - 1u)];
 }
 
-// Unit-test hook: out[i] = op(a[i], b[i]) on the device primitives (tests/test_gpu_field.py).
+// Unit-test hook: out[i] = op(a[i], b[i]) on the device primitives, op from the table of fieldops.cuh (tests/test_gpu_field.py).
 __global__ void fieldop_kernel(int op, const uint8_t* a, const uint8_t* b, int n, uint8_t* out)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const u256 x = load_be32(a + 32 * (size_t)i), y = load_be32(b + 32 * (size_t)i);
-    u256 z;
-    switch (op) {
-        case 0: z = fe_mul(x, y); break;
-        case 1: z = fe_add(x, y); break;
-        case 2: z = fe_sub(x, y); break;
-        case 3: z = sc_mul(x, y); break;
-        case 4: z = fe_inv(x); break;
-        case 5: z = sc_inv_to_mont(x); break;
-        case 7: z = fe_sqr(x); break;
-        default: z = sc_inv_to_mont_safegcd(x); break;
-    }
-    u256_to_be(z, out + 32 * (size_t)i);
+    u256_to_be(fieldop(op, x, y), out + 32 * (size_t)i);
 }
 
 }  // namespace fabgpu

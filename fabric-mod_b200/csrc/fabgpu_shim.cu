@@ -2134,7 +2134,7 @@ int fabgpu_sha256_segments(fabgpu_ctx* ctx, const uint8_t* buf, size_t buf_len, 
 
 int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t* b, size_t n, uint8_t* out)
 {
-    if (!ctx || !a || !b || !out) return FABGPU_E_ARG;
+    if (!ctx || !a || !b || !out || op < 0 || op >= FOP_COUNT) return FABGPU_E_ARG;
     std::lock_guard<std::mutex> lk(ctx->mu);
     Device& dv = ctx->devs[0];
     CK(ctx, cudaSetDevice(dv.id));

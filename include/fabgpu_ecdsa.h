@@ -262,8 +262,8 @@ int fabgpu_block_timing(const fabgpu_ctx* ctx, double out_us[10]);
 int fabgpu_sha256_segments(fabgpu_ctx* ctx, const uint8_t* buf, size_t buf_len, const uint32_t* jobs, size_t n, uint8_t* digests);
 
 /* ---- test / bring-up hooks ------------------------------------------------------------------------------ */
-/* Device field primitives on arrays (op: 0 fe_mul, 1 fe_add, 2 fe_sub, 3 sc_mul, 4 fe_inv,
- * 5 sc_inv_to_mont by Fermat, 6 the same by division steps, 7 fe_sqr). */
+/* Device field primitives on arrays: out[i] = op(a[i], b[i]), 32 big-endian bytes each.  op is a code of the table in
+ * fabric-mod_b200/csrc/fieldops.cuh (0 fe_mul ... 16); FABGPU_E_ARG for any other value. */
 int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t* b, size_t n, uint8_t* out);
 /* Sampled entries of a device window table: out[i] (64 bytes: X then Y, Montgomery form, little-endian 32-bit limbs) =
  * entry (window[i], digit[i]) = digit * 2^(w * window) * P, digit in [1, 2^w).  key_slot < 0: the generator's table

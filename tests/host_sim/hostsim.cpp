@@ -9,6 +9,7 @@
 #include <utility>
 #include "../../fabric-mod_b200/csrc/ecdsa_verify.cuh"
 #include "../../fabric-mod_b200/csrc/ecdsa_batchaffine.cuh"
+#include "../../fabric-mod_b200/csrc/fieldops.cuh"
 
 using namespace fabgpu;
 
@@ -201,24 +202,13 @@ void hostsim_verify_batch_small(const uint8_t* qx, const uint8_t* qy, const uint
     }
 }
 
-// field / scalar unit hooks: op 0 fe_mul, 1 fe_add, 2 fe_sub, 3 sc_mul, 4 fe_inv, 5 sc_inv_to_mont (b ignored for 4,5)
-void hostsim_fieldop(int op, const uint8_t* a, const uint8_t* b, int n, uint8_t* out)
+// field / scalar unit hooks, the op table of fieldops.cuh (the device's fabgpu_test_fieldop); -1 for an unknown op
+int hostsim_fieldop(int op, const uint8_t* a, const uint8_t* b, int n, uint8_t* out)
 {
-    for (int i = 0; i < n; i++) {
-        u256 x = u256_from_be(a + 32 * (size_t)i), y = u256_from_be(b + 32 * (size_t)i), z;
-        switch (op) {
-            case 0: z = fe_mul(x, y); break;
-            case 1: z = fe_add(x, y); break;
-            case 2: z = fe_sub(x, y); break;
-            case 3: z = sc_mul(x, y); break;
-            case 4: z = fe_inv(x); break;
-            case 5: z = sc_inv_to_mont(x); break;
-            case 8: z = fe_inv_safegcd(x); break;
-        case 7: z = fe_sqr(x); break;
-        default: z = sc_inv_to_mont_safegcd(x); break;
-        }
-        u256_to_be(z, out + 32 * (size_t)i);
-    }
+    if (op < 0 || op >= FOP_COUNT) return -1;
+    for (int i = 0; i < n; i++)
+        u256_to_be(fieldop(op, u256_from_be(a + 32 * (size_t)i), u256_from_be(b + 32 * (size_t)i)), out + 32 * (size_t)i);
+    return 0;
 }
 
 // k*P for affine plain (x,y) and plain scalar k, via the same table + Booth routine the kernel uses; returns affine plain

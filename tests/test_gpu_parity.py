@@ -37,45 +37,8 @@ def _ints(arr):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# device limb primitives (PTX) vs Python integers
+# device tables vs the oracle's scalar multiplication (the field primitives: tests/test_gpu_field.py)
 # ---------------------------------------------------------------------------------------------------------
-def _operands(mod, rnd, n):
-    edge = [0, 1, 2, mod - 1, mod - 2, (1 << 255) % mod, (1 << 224) % mod, (1 << 32) - 1, ((1 << 256) - 1) % mod, (1 << 96) % mod]
-    a = [rnd.randrange(mod) for _ in range(n)] + [x for x in edge for _ in edge]
-    b = [rnd.randrange(mod) for _ in range(n)] + [y for _ in edge for y in edge]
-    return a, b
-
-
-def test_field_primitives(ctx):
-    rnd = random.Random(1)
-    P, N = p256.P, p256.N
-    a, b = _operands(P, rnd, 4000)
-    A = np.stack([be32(x) for x in a]); B = np.stack([be32(x) for x in b])
-    rinv = pow(R, -1, P)
-    assert _ints(ctx.test_fieldop(0, A, B)) == [x * y * rinv % P for x, y in zip(a, b)]
-    assert _ints(ctx.test_fieldop(1, A, B)) == [(x + y) % P for x, y in zip(a, b)]
-    assert _ints(ctx.test_fieldop(2, A, B)) == [(x - y) % P for x, y in zip(a, b)]
-    a, b = _operands(N, rnd, 4000)
-    A = np.stack([be32(x) for x in a]); B = np.stack([be32(x) for x in b])
-    rinvn = pow(R, -1, N)
-    assert _ints(ctx.test_fieldop(3, A, B)) == [x * y * rinvn % N for x, y in zip(a, b)]
-    a = [rnd.randrange(1, P) for _ in range(64)] + [1, P - 1]
-    A = np.stack([be32(x) for x in a])
-    assert _ints(ctx.test_fieldop(4, A, A)) == [pow(x * rinv % P, -1, P) * R % P for x in a]
-    a = [rnd.randrange(1, N) for _ in range(64)] + [1, N - 1, p256.HALF_N]
-    A = np.stack([be32(x) for x in a])
-    assert _ints(ctx.test_fieldop(5, A, A)) == [pow(x, -1, N) * R % N for x in a]
-    # division-step inversion (p256_modinv.cuh) on a wider sample, incl. small and structured values
-    a = [rnd.randrange(1, N) for _ in range(4000)] + [1, 2, 3, N - 1, N - 2, p256.HALF_N, 1 << 30, (1 << 30) - 1, 1 << 255] + \
-        [rnd.getrandbits(k) or 1 for k in range(1, 256)]
-    A = np.stack([be32(x) for x in a])
-    assert _ints(ctx.test_fieldop(6, A, A)) == [pow(x, -1, N) * R % N for x in a]
-    # dedicated squaring
-    a, _ = _operands(P, rnd, 4000)
-    A = np.stack([be32(x) for x in a])
-    assert _ints(ctx.test_fieldop(7, A, A)) == [x * x * rinv % P for x in a]
-
-
 def _table_picks(w, rnd):
     """(window, digit) samples that hit the corners of the two-level build: digits below 2^(w/2) (low table only), multiples of
     2^(w/2) (high table only), chunk boundaries (64 entries per thread), the last entry, the top window's largest useful digit."""
@@ -218,6 +181,37 @@ def test_constructed_edge_cases(csp):
     st = csp.VerifyBatch(keys, list(range(len(cases))), [c["digest"] for c in cases], [c["sig"] for c in cases])
     for c, got in zip(cases, st):
         assert int(got) == vectors.expected_status(c), c["name"]
+
+
+def _chain_cases(orders=vectors.CHAIN_ORDERS):
+    """vectors.chain_cases at the library's window widths."""
+    b = pkg().binding
+    return vectors.chain_cases(*b.build_info(), b.Context.small_table_info()[0], orders=orders)
+
+
+def _fill_soa(ctx, slot, soa, key_slots):
+    hb = ctx.host_buffers(slot)
+    for name, arr in zip(("qx", "qy", "e", "r", "s"), soa):
+        hb[name][: arr.shape[0]] = arr
+    ctx.host_key_slots(slot)[: len(key_slots)] = key_slots
+    return hb
+
+
+def _chain_mismatches(cases, mix, bits):
+    assert bits.shape == mix["valid"].shape
+    bad = [c["name"] for c, p in zip(cases, mix["pos"]) if bits[p] != mix["valid"][p]]
+    return bad + ["honest row %d" % i for i in np.flatnonzero(bits != mix["valid"]) if i not in set(mix["pos"].tolist())][:4]
+
+
+def test_chain_collisions_through_the_generic_kernel(ctx):
+    """ecdsa_verify_kernel (Booth u2 Q, then the G windows ascending): a doubling, a mid-chain infinity and a final infinity at every
+    G window (vectors.chain_cases), plus the other kernels' chain cases as further adversarial inputs, interleaved with honest
+    signatures at rows that are not warp aligned."""
+    cases = _chain_cases()
+    mix = vectors.mix_with_workload(cases)
+    mask, off = ctx.verify_p256_host(*mix["soa"])
+    bad = _chain_mismatches(cases, mix, mask_bits(mask, len(mix["valid"])).astype(bool))
+    assert not bad and not off.any(), bad[:8]
 
 
 def test_nil_key_empty_digest_statuses(csp):
@@ -478,6 +472,13 @@ def test_key_table_kernel_variants_are_bit_exact(variant):
     finally:
         del os.environ["FABGPU_CACHED_KERNEL"]
         del os.environ["FABGPU_KEY_MIN_USES"]
+    try:
+        _check_key_table_variant(c, variant)
+    finally:
+        c.close()                       # a failing variant must not leave its tables on the device for the next one
+
+
+def _check_key_table_variant(c, variant):
     w = workload.Workload(20000 + 7, 16, seed=workload.DEFAULT_SEED + 21)
     w.tamper_r(0.05)
     exp = fast.valid_mask(fast.verify_batch(w.keys_xy, w.key_idx, w.digest, w.dig_off(), w.sigs, w.sig_off, nthreads=os.cpu_count()))
@@ -494,7 +495,19 @@ def test_key_table_kernel_variants_are_bit_exact(variant):
     st = c.bccsp_verify_batch(keys, np.arange(len(cases), dtype=np.int32), np.frombuffer(b"".join(digs), np.uint8), doff, np.frombuffer(b"".join(sigs), np.uint8), soff)
     for cs, got in zip(cases, st):
         assert int(got) == vectors.expected_status(cs), (variant, cs["name"])
-    c.close()
+    # the chain-collision cases of this kernel's own addition order (a doubling or an infinity at every step that can collide, the
+    # lane combines and the batch-affine tail included) and of the Jacobian chain, interleaved with honest signatures so that every
+    # CTA mixes both, through the keyed leaf.  One window table per distinct key: all of them fit, nothing is evicted.
+    own = {"jac": ("jac",), "ba": ("ba", "jac"), "ba2": ("ba", "jac"), "l2": ("l2", "jac"), "l4": ("l4", "jac")}[variant]
+    cases = _chain_cases(own)
+    mix = vectors.mix_with_workload(cases)
+    handles = c.keys_register(mix["keys_xy"])
+    assert (handles >= 0).all() and mix["keys_xy"].shape[0] < c.key_slot_capacity()
+    n = len(mix["valid"])
+    hb = _fill_soa(c, 1, mix["soa"], handles[mix["kidx"]])
+    c.verify_p256_keyed(1, n)
+    bad = _chain_mismatches(cases, mix, mask_bits(hb["mask"], n).astype(bool))
+    assert not bad, (variant, bad[:8])
 
 
 def test_bccsp_batch_inplace_pinned_buffers_match_the_copying_form():

@@ -61,6 +61,52 @@ def test_small_tables_through_the_keyed_entry_points(ctx):
     assert (mask_bits(hb["mask"], 5001) == mask_bits(exp, 5001)).all()
 
 
+def _fill_soa(ctx, slot, soa, key_slots):
+    hb = ctx.host_buffers(slot)
+    for name, arr in zip(("qx", "qy", "e", "r", "s"), soa):
+        hb[name][: arr.shape[0]] = arr
+    ctx.host_key_slots(slot)[: len(key_slots)] = key_slots
+    return hb
+
+
+def _mismatches(cases, mix, hb):
+    bits = mask_bits(hb["mask"], len(mix["valid"])).astype(bool)
+    return [c["name"] for c, p in zip(cases, mix["pos"]) if bits[p] != mix["valid"][p]] + \
+        ["honest row %d" % i for i in np.flatnonzero(bits != mix["valid"]) if i not in mix["pos"]][:4]
+
+
+def test_chain_collisions_through_the_small_table_kernels(ctx):
+    """The small-table order's chain cases (vectors.chain_cases: a doubling or an infinity at every signed window of the key, at the
+    library's widths) interleaved with honest signatures: first with every handle small (ecdsa_verify_small_kernel over the whole
+    batch), then in one batch of window-table, small-table and no-table handles together with the key-table and generic orders'
+    cases (compact_classes_kernel, then ecdsa_verify_indexed_kernel and the indexed form of the small kernel)."""
+    b = pkg().binding
+    widths = b.build_info() + (b.Context.small_table_info()[0],)
+    cases = vectors.chain_cases(*widths, orders=("small",))
+    mix = vectors.mix_with_workload(cases, seed=0x5A11)
+    hs = ctx.keys_register_small(mix["keys_xy"])
+    assert (hs <= -2).all()
+    hb = _fill_soa(ctx, 0, mix["soa"], hs[mix["kidx"]])
+    ctx.verify_p256_keyed(0, len(mix["valid"]))
+    bad = _mismatches(cases, mix, hb)
+    assert not bad, bad[:8]
+    cases = vectors.chain_cases(*widths, orders=("small", "jac", "generic"))
+    mix = vectors.mix_with_workload(cases, seed=0x5A12)
+    big, small = ctx.keys_register(mix["keys_xy"]), ctx.keys_register_small(mix["keys_xy"])
+    assert (big >= 0).all() and (small <= -2).all()
+    kidx = mix["kidx"]
+    code = np.select([kidx % 3 == 0, kidx % 3 == 1], [small[kidx], big[kidx]], -1).astype(np.int32)
+    handles = {"small": small, "jac": big, "generic": None}             # each case through the kernel of its own order
+    for c, p in zip(cases, mix["pos"]):
+        h = handles[c["order"]]
+        code[p] = -1 if h is None else h[kidx[p]]
+    assert (code >= 0).sum() > 100 and (code == -1).sum() > 100 and (code <= -2).sum() > 100
+    hb = _fill_soa(ctx, 1, mix["soa"], code)
+    ctx.verify_p256_keyed(1, len(mix["valid"]))
+    bad = _mismatches(cases, mix, hb)
+    assert not bad, bad[:8]
+
+
 def test_small_tables_device_resident(ctx):
     import torch
     w = workload.Workload(8192, 40, seed=143)

@@ -7,10 +7,12 @@ import pytest
 from oracle import bccsp_sw as o
 from oracle import fast
 from tools import workload
-from util import be32, hash_to_e32, hostsim_verify, pkg
+from util import be32, from_be, hash_to_e32, hostsim_verify, pkg
 import vectors
 
 V_INVALID, V_VALID, V_OFFCURVE = 0, 1, 2
+HOST_WIDTHS = (8, 8, 8)         # FAB_WG, FAB_WQ, FAB_WS of the host build (util.hostsim)
+PRODUCT_WIDTHS = (22, 16, 8)    # the library's (binding.build_info, Context.small_table_info): the widths of the GPU tests' chain cases
 
 
 @pytest.mark.parametrize("cached", [False, True, "ba", "small"])
@@ -30,6 +32,65 @@ def test_constructed_edge_cases(cached):
                              np.frombuffer(r, np.uint8), np.frombuffer(s, np.uint8), cached=cached is True, ba=cached == "ba", small=cached == "small")[0]
         got = {V_VALID: o.VALID, V_INVALID: o.INVALID, V_OFFCURVE: o.ERR_OFF_CURVE}[int(out)]
         assert got == exp, c["name"]
+    # the chain-collision cases of every order at the host build's widths, in one batch: this path's own order takes its doubling and
+    # infinity branches at every reachable step, the other orders' cases are adversarial inputs all the same
+    cases = vectors.chain_cases(*HOST_WIDTHS)
+    exp = vectors.oracle_statuses(cases)
+    out = hostsim_verify(*vectors.chain_soa(cases), cached=cached is True, ba=cached == "ba", small=cached == "small")
+    bad = [c["name"] for c, e, g in zip(cases, exp, out) if g != (V_VALID if e == o.VALID else V_INVALID)]
+    assert not bad, "%d of %d chain cases disagree with the oracle, e.g. %s" % (len(bad), len(cases), bad[:8])
+
+
+_COVERAGE = [(HOST_WIDTHS, order) for order in vectors.CHAIN_ORDERS] + [(PRODUCT_WIDTHS, order) for order in vectors.CHAIN_ORDERS] + \
+            [((8, 8, ws), "small") for ws in (5, 6, 7)]
+
+
+def _chain_cases(widths):
+    return vectors.chain_cases(*widths) if widths[2] == 8 else vectors.chain_cases(*widths, orders=("small",))
+
+
+@pytest.mark.parametrize("widths,order", _COVERAGE, ids=["%d-%d-%d-%s" % (w + (order,)) for w, order in _COVERAGE])
+def test_chain_cases_reach_every_exceptional_step(widths, order):
+    """The chain-collision generator (vectors.chain_cases) against its scalar model (vectors.chain_events): every case takes exactly
+    its intended branch under its own kernel's order, the cases reach every (step, kind) that order can reach at these widths, none
+    collides inside the affine levels of the batch-affine kernels (where the per-signature fallback would run), and the oracle gives
+    VALID for the doublings and mid-chain infinities, INVALID for the final infinities."""
+    cases = [c for c in _chain_cases(widths) if c["order"] == order]
+    for c in cases:
+        assert vectors.chain_events(order, c["u1"], c["u2"], c["d"], widths) == [(c["step"], c["kind"])], c["name"]
+        assert not [ev for ev in vectors.chain_events("ba", c["u1"], c["u2"], c["d"], widths) if ev[0][0] == "L"], c["name"]
+    reached = {(c["step"], c["kind"]) for c in cases}
+    assert len(reached) == len(cases) and reached == vectors.chain_steps(order, widths)
+    assert {k for _, k in reached} == set(vectors.CHAIN_KINDS)
+    st = vectors.oracle_statuses(cases)
+    assert [int(s) for s in st] == [c["expect"] for c in cases]
+    for kind in vectors.CHAIN_KINDS:                 # and the Python oracle agrees with its C restatement on these inputs
+        c = next(c for c in cases if c["kind"] == kind)
+        assert vectors.expected_status(c) == c["expect"], c["name"]
+
+
+def test_chain_model_on_known_chains():
+    """chain_events on chains worked out by hand at 8/8: u1 = 5, u2 = 1 meets the key's first window at the same point (dbl) in
+    the key-table order and at the opposite point when the key is negated (final infinity); lanes and tail labels."""
+    w = HOST_WIDTHS
+    assert vectors.chain_events("jac", 5, 1, 5, w) == [("q0", "dbl")]
+    assert vectors.chain_events("jac", 5, 1, N_ - 5, w) == [("q0", "final_inf")]
+    assert vectors.chain_events("jac", 5, 1 + (1 << 8), N_ - 5, w) == [("q0", "opp")]       # window q1 follows: R = 256 Q
+    assert vectors.chain_events("generic", 5, 1, 5, w) == [("g0", "dbl")]
+    assert vectors.chain_events("small", 5, 1, 5, w) == [("q0", "dbl")]
+    assert vectors.chain_events("small", 0x81, 0xFF, 0x81, w) == [("q0", "opp")]           # 0xFF recodes to -1 + 256
+    # 8/8: windows 0..31 are G's, 32..63 the key's; lane 0 = g0 = 1, lane 1 = q1 (window 33) = 2^8 d = 1: the combine doubles
+    assert vectors.chain_events("l2", 1, 1 << 8, pow(1 << 8, -1, N_), w) == [("c0.0", "dbl")]
+    assert vectors.chain_events("ba", 3 << 24, 0, 1, w) == []                               # a G group never collides with its own windows
+    assert vectors.chain_events("ba", 1, (N_ - 1), 1, w) == [("t0", "final_inf")]
+
+
+N_ = vectors.N
+
+
+def test_product_widths_are_the_librarys():
+    b = pkg().binding
+    assert b.build_info() + (b.Context.small_table_info()[0],) == PRODUCT_WIDTHS
 
 
 def test_config1_1024_tuples():
@@ -138,3 +199,30 @@ def test_small_tables_at_other_window_widths(ws):
     out = np.zeros(w.n, np.uint8)
     hs.hostsim_verify_batch_small(*[a.ctypes.data_as(ctypes.c_void_p) for a in arrs], ctypes.c_int(w.n), out.ctypes.data_as(ctypes.c_void_p))
     assert ((out == V_VALID) == (exp == o.VALID)).all() and 30 < int((exp != o.VALID).sum()) < 100
+    # the small-table order's chain-collision cases at this width: a doubling or an infinity at every signed window
+    cases = vectors.chain_cases(8, 8, ws, orders=("small",))
+    exp = vectors.oracle_statuses(cases)
+    arrs = vectors.chain_soa(cases)
+    out = np.zeros(len(cases), np.uint8)
+    hs.hostsim_verify_batch_small(*[a.ctypes.data_as(ctypes.c_void_p) for a in arrs], ctypes.c_int(len(cases)), out.ctypes.data_as(ctypes.c_void_p))
+    bad = [c["name"] for c, e, g in zip(cases, exp, out) if g != (V_VALID if e == o.VALID else V_INVALID)]
+    assert not bad, (ws, bad[:8])
+
+
+def test_field_ops_match_python_integers():
+    """Every op of the shared test table (fieldops.cuh) in the host build, against Python integers: the same op codes and expectations
+    as tests/test_gpu_field.py, so the host and device hooks agree op for op."""
+    import ctypes
+    import random
+    from util import field_op_cases, hostsim
+    hs = hostsim()
+    for op, (a, b, exp) in field_op_cases(random.Random(5), 200).items():
+        A = np.stack([be32(x) for x in a]); B = np.stack([be32(x) for x in b])
+        out = np.zeros_like(A)
+        assert hs.hostsim_fieldop(ctypes.c_int(op), A.ctypes.data_as(ctypes.c_void_p), B.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(len(a)),
+                                  out.ctypes.data_as(ctypes.c_void_p)) == 0
+        assert [from_be(row) for row in out] == exp, op
+    z = np.zeros((1, 32), np.uint8)
+    for op in (-1, 17):
+        assert hs.hostsim_fieldop(ctypes.c_int(op), z.ctypes.data_as(ctypes.c_void_p), z.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(1),
+                                  z.ctypes.data_as(ctypes.c_void_p)) == -1
