@@ -32,6 +32,7 @@ enum : uint8_t {
 #define BD_MAX_SIGNERS 64       // distinct verified signers one policy evaluation handles (`used` is a 64-bit mask); more -> CPU validator
 #define BD_MAX_NS 4             // namespaces validated per transaction (the invoked chaincode + those it writes to); more -> CPU validator
 #define BD_MAX_NS_SEEN 8        // namespaces of one read/write set checked for duplicates; more -> CPU validator
+#define BD_MAX_POLICY_DEPTH 12  // deepest node of a policy tree eval_policy walks (root = 0); fabgpu_msp_configure refuses deeper trees
 #define BD_ENDS_HINT 16         // job-array sizing: expected endorsements per transaction (the capacity is a parameter, see JobArrays::J_cap)
 
 struct Seg { uint32_t off, len; };
@@ -120,25 +121,34 @@ BD_HD int32_t msp_find(const MspDev& m, const uint8_t* p, uint32_t n)
 }
 
 // ---- protobuf wire reader ------------------------------------------------------------------------------------------------
+// The only wire reader of the block path: the walk below and blockval.cpp's split_block both use it.
+#define BD_FIELD_TOO_LARGE 0xffffffffu   // reported for every field number >= 2^32-1: no message on the path has such a field
 struct Reader {
     const uint8_t* base; uint32_t pos, end; bool ok;
+    // At most 10 bytes, and the 10th may only carry bit 63 (0 or 1): any other value overflows 64 bits and is an error, as in
+    // golang/protobuf's decodeVarint (`if y < 2`), which proto.Unmarshal uses for tags, lengths and values.
     BD_HD bool varint(uint64_t& v)
     {
         v = 0;
-        for (int shift = 0; shift < 70; shift += 7) {
+        for (int shift = 0; shift < 63; shift += 7) {
             if (pos >= end) { ok = false; return false; }
             const uint8_t c = base[pos++];
             v |= (uint64_t)(c & 0x7f) << shift;
             if (!(c & 0x80)) return true;
         }
-        ok = false; return false;
+        if (pos >= end || base[pos] > 1) { ok = false; return false; }
+        v |= (uint64_t)base[pos++] << 63;
+        return true;
     }
     BD_HD bool next(uint32_t& field, uint32_t& wt, uint64_t& val, Seg& bytes)
     {
         if (pos >= end) return false;
         uint64_t key;
         if (!varint(key)) return false;
-        field = (uint32_t)(key >> 3); wt = (uint32_t)(key & 7);
+        // A field number that does not fit 32 bits is an unknown field, as in the reference's decoder.  Truncating it instead
+        // would read field 2^32 + 2 as field 2 (a second signature, a second Block.data).
+        const uint64_t fno = key >> 3;
+        field = fno < BD_FIELD_TOO_LARGE ? (uint32_t)fno : BD_FIELD_TOO_LARGE; wt = (uint32_t)(key & 7);
         if (field == 0) { ok = false; return false; }
         if (wt == 0) return varint(val);
         if (wt == 1) { if (end - pos < 8) { ok = false; return false; } pos += 8; return true; }
@@ -472,7 +482,17 @@ BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* chan
     }
     if (!tx.endorsements_parse_ok || n_jobs == 0) return;
     uint32_t j = alloc_end(n_jobs);
-    if (j + n_jobs > ja.J_cap || j + n_jobs < j) { tx.overflow = 1; return; }          // job arrays full: this transaction goes to the CPU validator
+    if (j + n_jobs > ja.J_cap || j + n_jobs < j) {                    // job arrays full: this transaction goes to the CPU validator
+        tx.overflow = 1;
+        // The later stages run over every slot up to J_cap once the counter passes it: the slots handed out here that still
+        // lie inside the arrays get dead records, not whatever the previous block (or cudaMalloc) left there.
+        ShaJobD z; for (int k = 0; k < 3; k++) { z.off[k] = 0; z.len[k] = 0; }
+        for (uint32_t q = j; q < ja.J_cap && q - j < n_jobs; q++) {
+            raw[q].ident.off = raw[q].ident.len = raw[q].sig.off = raw[q].sig.len = 0; raw[q].tx = 0xffffffffu; raw[q].k = -1;
+            ja.sha[q] = z;
+        }
+        return;
+    }
     tx.first_end_job = j; tx.n_end_jobs = n_jobs;
     {
         Reader r; r.base = base; r.pos = cap.s[1].off; r.end = cap.s[1].off + cap.s[1].len; r.ok = true;
@@ -527,7 +547,7 @@ struct PolicyDev {
 
 BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer_code, int n_signers, uint64_t& used, int depth)
 {
-    if (idx < 0 || idx >= pol.n_nodes || depth > 12) return false;
+    if (idx < 0 || idx >= pol.n_nodes || depth > BD_MAX_POLICY_DEPTH) return false;
     const int32_t type = pol.nodes[4 * idx], n = pol.nodes[4 * idx + 1], first = pol.nodes[4 * idx + 2], cnt = pol.nodes[4 * idx + 3];
     if (type == 0) {
         int verified = 0;

@@ -1,73 +1,34 @@
 // See blockval.hpp.
 #include "blockval.hpp"
+#include "blockdev.cuh"
 
 namespace fabgpu { namespace blockval {
 
-namespace {
-
-// protobuf wire reader: just enough for Block and BlockData
-struct Reader {
-    const uint8_t* base;
-    const uint8_t* p;
-    const uint8_t* end;
-    bool ok = true;
-
-    bool varint(uint64_t& v) {
-        v = 0;
-        for (int shift = 0; shift < 70; shift += 7) {
-            if (p >= end) return ok = false;
-            const uint8_t c = *p++;
-            v |= (uint64_t)(c & 0x7f) << shift;
-            if (!(c & 0x80)) return true;
-        }
-        return ok = false;
-    }
-    // next field: returns false at end of message or on error (check ok)
-    bool next(uint32_t& field, uint32_t& wt, Seg& bytes) {
-        if (p >= end) return false;
-        uint64_t key, v;
-        if (!varint(key)) return false;
-        field = (uint32_t)(key >> 3); wt = (uint32_t)(key & 7);
-        if (field == 0) return ok = false;
-        switch (wt) {
-            case 0: return varint(v);
-            case 1: if (end - p < 8) return ok = false; p += 8; return true;
-            case 5: if (end - p < 4) return ok = false; p += 4; return true;
-            case 2: {
-                uint64_t ln;
-                if (!varint(ln)) return false;
-                if ((uint64_t)(end - p) < ln) return ok = false;
-                bytes.off = (uint32_t)(p - base); bytes.len = (uint32_t)ln;
-                p += ln;
-                return true;
-            }
-            default: return ok = false;
-        }
-    }
-};
-
-}  // namespace
-
+// The envelopes are read with the device walk's wire reader (bdev::Reader), so that every level of the block path takes the
+// same decision on every tag.
 bool split_block(const uint8_t* block, size_t len, std::vector<Seg>& envs)
 {
     envs.clear();
-    Seg data; bool has_data = false;
+    if (len >= (1ull << 32)) return false;                               // offsets are 32-bit
+    auto reader = [&](uint32_t off, uint32_t n) { bdev::Reader r; r.base = block; r.pos = off; r.end = off + n; r.ok = true; return r; };
+    bdev::Seg data; data.off = data.len = 0; bool has_data = false;
     {
-        Reader r{block, block, block + len};
-        uint32_t f, wt; Seg b;
-        while (r.next(f, wt, b)) {
+        bdev::Reader r = reader(0, (uint32_t)len);
+        uint32_t f, wt; uint64_t v; bdev::Seg b;
+        while (r.next(f, wt, v, b)) {
             if (f == 1 || f == 3) { if (wt != 2) return false; }         // header, metadata: known fields, must be length-delimited
             if (f == 2) { if (wt != 2) return false; data = b; has_data = true; }
         }
         if (!r.ok) return false;
     }
     if (!has_data) return true;
-    Reader r{block, block + data.off, block + data.off + data.len};
-    uint32_t f, wt; Seg b;
-    while (r.next(f, wt, b)) {
+    bdev::Reader r = reader(data.off, data.len);
+    uint32_t f, wt; uint64_t v; bdev::Seg b;
+    while (r.next(f, wt, v, b)) {
         if (f != 1) continue;
         if (wt != 2) return false;
-        envs.push_back(b);
+        Seg e; e.off = b.off; e.len = b.len;
+        envs.push_back(e);
     }
     return r.ok;
 }

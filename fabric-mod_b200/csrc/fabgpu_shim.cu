@@ -1742,6 +1742,39 @@ static int msp_small_tier(fabgpu_ctx* ctx, const uint8_t* keys_xy, int n_ids)
     return FABGPU_OK;
 }
 
+// Height of node i's tree (a leaf is 0), or -1 when it is deeper than BD_MAX_POLICY_DEPTH or runs into a cycle (a cycle makes the
+// path longer than any bound).  height: memo, -1 = not known yet.  The path length bounds the recursion.
+static int policy_height(const std::vector<blockval::PolicyNode>& nodes, int i, int path, std::vector<int>& height)
+{
+    if (path > BD_MAX_POLICY_DEPTH) return -1;
+    if (height[i] >= 0) return height[i];
+    int h = 0;
+    if (nodes[i].type == 0)
+        for (int c = nodes[i].first_child; c < nodes[i].first_child + nodes[i].n_children; c++) {
+            const int hc = policy_height(nodes, c, path + 1, height);
+            if (hc < 0 || hc + 1 > BD_MAX_POLICY_DEPTH) return -1;
+            h = std::max(h, hc + 1);
+        }
+    return height[i] = h;
+}
+
+// What eval_policy can evaluate exactly: children inside the array, SignedBy indices inside the principals, and from every node a
+// tree at most BD_MAX_POLICY_DEPTH deep without cycles.  Past that depth the device would report ENDORSEMENT_POLICY_FAILURE where
+// the reference, which has no depth limit, may accept: such a policy is refused, and the caller validates on the CPU.
+static const char* check_policy(const std::vector<blockval::PolicyNode>& nodes, int n_principals)
+{
+    const int64_t n_nodes = (int64_t)nodes.size();
+    for (const auto& nd : nodes) {
+        if (nd.type == 0 && (nd.first_child < 0 || nd.n_children < 0 || (int64_t)nd.first_child + nd.n_children > n_nodes))
+            return "policy node children out of range";
+        if (nd.type != 0 && (nd.n < 0 || nd.n >= n_principals)) return "SignedBy principal index out of range";
+    }
+    std::vector<int> height(nodes.size(), -1);
+    for (int i = 0; i < (int)n_nodes; i++)
+        if (policy_height(nodes, i, 0, height) < 0) return "policy tree deeper than the device evaluates, or cyclic";
+    return nullptr;
+}
+
 int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* mspid_blob,
                          const uint32_t* mspid_off, const uint8_t* keys_xy, const uint8_t* valid, int n_ids,
                          const int32_t* policy_nodes, int n_nodes, const uint8_t* principal_blob, const uint32_t* principal_off,
@@ -1749,6 +1782,13 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
 {
     if (!ctx || n_ids < 0 || n_nodes < 0 || n_principals < 0 || !channel_id) return FABGPU_E_ARG;
     if (n_ids && (!id_blob || !id_off || !mspid_blob || !mspid_off || !keys_xy || !valid)) return FABGPU_E_ARG;
+    if (n_nodes && !policy_nodes) return FABGPU_E_ARG;
+    {
+        std::vector<blockval::PolicyNode> nodes;
+        for (int i = 0; i < n_nodes; i++)
+            nodes.push_back({policy_nodes[4 * i], policy_nodes[4 * i + 1], policy_nodes[4 * i + 2], policy_nodes[4 * i + 3]});
+        if (const char* err = check_policy(nodes, n_principals)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    }
     {
         std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
         ctx->msp = blockval::MspTable();
@@ -1761,10 +1801,6 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
         ctx->policy.clear();
         for (int i = 0; i < n_nodes; i++)
             ctx->policy.push_back({policy_nodes[4 * i], policy_nodes[4 * i + 1], policy_nodes[4 * i + 2], policy_nodes[4 * i + 3]});
-        for (const auto& nd : ctx->policy)
-            if (nd.type == 0 && (nd.first_child < 0 || nd.n_children < 0 || nd.first_child + nd.n_children > n_nodes)) {
-                ctx->last_error = "policy node children out of range"; return FABGPU_E_ARG;
-            }
         ctx->principals.clear();
         for (int i = 0; i < n_principals; i++)
             ctx->principals.emplace_back((const char*)principal_blob + principal_off[i], principal_off[i + 1] - principal_off[i]);

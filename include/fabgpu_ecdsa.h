@@ -219,7 +219,10 @@ int fabgpu_gate_signature(const uint8_t* sig, size_t sig_len, uint8_t r_out[32],
  * [first_child, first_child + n_children), type 1 = SignedBy(principal n); node 0 is the root.  Principals are MSP ids
  * (ROLE member).  Every identity's key gets a window table when the MSP fits the window-table pool (n_ids <= fabgpu_key_slot_capacity);
  * a larger MSP -- thousands of client certificates -- goes to the small tier instead, except the identities whose key already owns a
- * window table: register the few busy keys (the endorsing peers) with fabgpu_keys_register BEFORE this call and they keep it. */
+ * window table: register the few busy keys (the endorsing peers) with fabgpu_keys_register BEFORE this call and they keep it.
+ * FABGPU_E_ARG, with nothing installed, for a policy array the device cannot evaluate exactly: children outside the array, a
+ * SignedBy index outside the principals, a cycle, or a tree deeper than 12 levels below any node (BD_MAX_POLICY_DEPTH).
+ * The caller then validates that channel's blocks on the CPU. */
 int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* mspid_blob,
                          const uint32_t* mspid_off, const uint8_t* keys_xy, const uint8_t* valid, int n_ids,
                          const int32_t* policy_nodes, int n_nodes, const uint8_t* principal_blob, const uint32_t* principal_off,

@@ -64,6 +64,13 @@ S_COLLHASHED = {1: ("collection_name", "bytes"), 2: ("hashed_rwset", "bytes"), 3
 S_HASHEDRWSET = {1: ("hashed_reads", "rep_bytes"), 2: ("hashed_writes", "rep_bytes"), 3: ("metadata_writes", "rep_bytes")}
 
 
+def int32_field(v: int) -> int:
+    """A proto3 int32 / enum field as Go decodes it: the varint's low 32 bits, two's complement (ChannelHeader.type = 3 + 2^32
+    is 3; -1 sent as a 10-byte varint is -1)."""
+    v &= 0xFFFFFFFF
+    return v - (1 << 32) if v >= 1 << 31 else v
+
+
 def identity_id(serialized: bytes, mspid: str):
     """The IdentityIdentifier the reference de-duplicates on (common/policies/policy.go:380-386: Mspid + Id, with
     Id = hex(SHA-256(certificate DER)), msp/identities.go:55-76): two byte-different serializations of ONE certificate (PEM line
@@ -195,7 +202,8 @@ def validate_tx(env_bytes, msp: Msp, channel: str, nodes, principals, verify=_ve
         hdr = pb.parse(payload["header"], S_HEADER)
         chdr = pb.parse(hdr["channel_header"] or b"", S_CHDR_EXT)
         shdr = pb.parse(hdr["signature_header"] or b"", S_SHDR)
-        if (chdr["type"] or 0) not in (1, 2, 3):
+        chdr["type"] = int32_field(chdr["type"] or 0)
+        if chdr["type"] not in (1, 2, 3):
             raise pb.PbError("invalid header type")
         if (chdr["epoch"] or 0) != 0:
             raise pb.PbError("invalid epoch")

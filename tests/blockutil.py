@@ -46,17 +46,35 @@ def bd_lib():
     if _BD is None:
         d = os.path.join(ROOT, "tests", "host_sim")
         so, src = os.path.join(d, "libblockdev_host.so"), os.path.join(d, "blockdev_host.cpp")
-        deps = [src, os.path.join(ROOT, "fabric-mod_b200", "csrc", "blockdev.cuh")]
+        csrc = os.path.join(ROOT, "fabric-mod_b200", "csrc")
+        deps = [src] + [os.path.join(csrc, f) for f in ("blockdev.cuh", "blockval.cpp", "blockval.hpp")]
         if not os.path.exists(so) or any(os.path.getmtime(so) < os.path.getmtime(f) for f in deps):
-            subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-o", so, src])
+            subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-o", so, src, os.path.join(csrc, "blockval.cpp")])
         _BD = ctypes.CDLL(so)
         _BD.bd_new.restype = ctypes.c_void_p
+        _BD.bd_split_block.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int]
     return _BD
+
+
+def split_block(blk: bytes):
+    """The library's split_block (blockval.cpp) on a serialized Block: the envelopes, or None when the Block does not parse."""
+    L = bd_lib()
+    buf = np.frombuffer(blk or b"\x00", np.uint8)
+    cap = len(blk) + 1
+    out = np.zeros(2 * cap, np.uint32)
+    n = L.bd_split_block(_p(buf), len(blk), _p(out), cap)
+    return None if n < 0 else [blk[out[2 * i]: out[2 * i] + out[2 * i + 1]] for i in range(n)]
 
 
 def device_logic_flags(env_blob, env_off, identities, channel, nodes, principals, policies=None):
     """The device-side block logic (blockdev.cuh) executed on the host, driven by oracle verdicts and hashlib digests.
     policies: {namespace: root node} (None: one policy for every namespace)."""
+    return device_logic_run(env_blob, env_off, identities, channel, nodes, principals, policies)[0]
+
+
+def device_logic_run(env_blob, env_off, identities, channel, nodes, principals, policies=None, ends_hint=16, poison=False):
+    """device_logic_flags with the job arrays sized T (1 + ends_hint) and, with poison, filled with garbage instead of dead records
+    before the walk.  -> (flags, number of job slots the later stages would read that the walk left unwritten)."""
     from oracle import goasn1
     from util import pkg
     L = bd_lib()
@@ -78,7 +96,8 @@ def device_logic_flags(env_blob, env_off, identities, channel, nodes, principals
     blob = np.frombuffer(env_blob, np.uint8) if len(env_blob) else np.zeros(1, np.uint8)
     env_off = np.ascontiguousarray(env_off, np.uint32)
     T = env_off.shape[0] - 1
-    n_end = L.bd_plan(h, _p(blob), _p(env_off), T)
+    n_end = L.bd_plan_ex(h, _p(blob), _p(env_off), T, ends_hint, 1 if poison else 0)
+    stale = L.bd_stale(h)
     J = T + n_end
     ident, gok = ctypes.c_int(0), ctypes.c_int(0)
     r = (ctypes.c_uint8 * 32)(); s = (ctypes.c_uint8 * 32)(); segs = (ctypes.c_uint32 * 12)()
@@ -108,7 +127,7 @@ def device_logic_flags(env_blob, env_off, identities, channel, nodes, principals
     flags = np.full(max(T, 1), 254, np.uint8)
     L.bd_decide(h, _p(sig_ok), _p(chk), _p(flags))
     L.bd_free(h)
-    return flags[:T]
+    return flags[:T], stale
 
 
 def device_gate(sig: bytes):
@@ -119,3 +138,20 @@ def device_gate(sig: bytes):
     ok = L.bd_gate(buf, ctypes.c_uint32(len(sig)), r, s)
     st = L.bd_gate_status(buf, ctypes.c_uint32(len(sig)), r, s)
     return bool(ok), bytes(r), bytes(s), int(st)
+
+
+def capacity_edge_cases():
+    """Capacity edges of the device logic: BD_MAX_NS_SEEN (8 / 9 namespaces), BD_MAX_NS (4 / 5 written namespaces), BD_MAX_SIGNERS
+    (64 / 65 distinct verified signers).  [(name, network, n_tx, nodes, policies, build_block shape, index of the transaction at the
+    limit, index of the one past it)]."""
+    cc = blockgen.CHAINCODE
+    net = blockgen.Network()
+    nodes = net.policy_n_of(2)
+    seen = lambda t: [(cc, 1, 1)] + [("read%d" % i, 1, 0) for i in range(7 + (t == 1))]            # 8 / 9 namespaces
+    wrote = lambda t: [(cc, 1, 1)] + [("write%d" % i, 0, 1) for i in range(3 + (t == 1))]          # 4 / 5 written namespaces
+    pol = {cc: 0, **{"write%d" % i: 0 for i in range(4)}}
+    many = blockgen.Network(n_orgs=4, n_clients=70, seed=0x5167)
+    signers = lambda t: many.clients[: 64 + (t == 1)] if t < 2 else [many.peers[(t + k) % 4] for k in range(3)]   # 64 / 65 signers
+    return [("namespaces_seen", net, 4, nodes, {cc: 0}, dict(namespaces=seen), 0, 1),
+            ("namespaces_written", net, 4, nodes, pol, dict(namespaces=wrote), 0, 1),
+            ("signers", many, 12, many.policy_n_of(3), None, dict(endorsers=signers), 0, 1)]

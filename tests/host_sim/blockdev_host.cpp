@@ -1,12 +1,15 @@
 // TEST HELPER (not product code): runs the device-side block logic (fabric-mod_b200/csrc/blockdev.cuh: plan_tx, gate_signature,
 // decide_tx -- the very functions the CUDA kernels call) on the host, one transaction at a time, so tests can compare it with
 // the oracle on the CPU-only box.  Signature verdicts and SHA-256 digests are supplied by the test (oracle, hashlib).
+// Built together with the library's blockval.cpp (split_block).
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <map>
 #include <string>
 #include <vector>
 #include "../../fabric-mod_b200/csrc/blockdev.cuh"
+#include "../../fabric-mod_b200/csrc/blockval.hpp"
 
 using namespace fabgpu::bdev;
 
@@ -16,7 +19,7 @@ struct H {
     std::vector<int32_t> group, ns_root; std::vector<uint8_t> ns_blob; std::vector<uint32_t> ns_off;
     std::vector<uint8_t> block; std::vector<uint32_t> env_off;
     std::vector<TxDev> txs; std::vector<RawJob> raw; std::vector<ShaJobD> sha; std::vector<uint8_t> r, s, gate_ok; std::vector<int32_t> jks, jid;
-    uint32_t T = 0, J_cap = 0, n_end = 0;
+    uint32_t T = 0, J_cap = 0, n_end = 0, stale = 0;
     MspDev msp() const {
         MspDev m; m.id_blob = id_blob.data(); m.id_off = id_off.data(); m.key_slot = key_slot.data(); m.valid = valid.data(); m.msp_code = msp_code.data();
         m.group = group.empty() ? nullptr : group.data();
@@ -58,14 +61,21 @@ void bd_namespaces(void* p, const uint8_t* ns_blob, const uint32_t* ns_off, cons
     if (h->ns_blob.empty()) h->ns_blob.push_back(0);
 }
 
-// plans every transaction; returns the number of endorsement jobs; J = T + n_end signature jobs, 2T check digests after J_cap
-int bd_plan(void* p, const uint8_t* blob, const uint32_t* env_off, int n_env)
+// Plans every transaction; returns the number of endorsement jobs inside the arrays; J = T + n_end signature jobs, 2T check digests
+// after J_cap.  ends_hint sizes the job arrays as the library does (J_cap = T (1 + ends_hint)).  poison = 1: the job arrays start
+// filled with the byte 0xA5 instead of dead records, as device memory holds whatever the previous block left; every slot the later
+// stages would read must then have been written by the walk.  bd_stale tells how many were not (those are not resolved here).
+int bd_plan_ex(void* p, const uint8_t* blob, const uint32_t* env_off, int n_env, int ends_hint, int poison)
 {
     H* h = (H*)p;
     h->block.assign(blob, blob + env_off[n_env]); h->env_off.assign(env_off, env_off + n_env + 1);
-    h->T = (uint32_t)n_env; h->J_cap = h->T * (1 + BD_ENDS_HINT); h->n_end = 0;
+    h->T = (uint32_t)n_env; h->J_cap = h->T * (1 + (uint32_t)ends_hint); h->n_end = 0;
     h->txs.assign(h->T, TxDev()); h->sha.assign(h->J_cap + 2 * h->T, ShaJobD());
     { RawJob dead; dead.ident.off = dead.ident.len = dead.sig.off = dead.sig.len = 0; dead.tx = 0xffffffffu; dead.k = -1; h->raw.assign(h->J_cap, dead); }
+    if (poison) {
+        memset(h->raw.data(), 0xA5, sizeof(RawJob) * h->raw.size());
+        memset(h->sha.data(), 0xA5, sizeof(ShaJobD) * h->sha.size());
+    }
     h->r.assign(32 * (size_t)h->J_cap, 0); h->s.assign(32 * (size_t)h->J_cap, 0); h->gate_ok.assign(h->J_cap, 0); h->jks.assign(h->J_cap, -1); h->jid.assign(h->J_cap, -1);
     JobArrays ja; ja.sha = h->sha.data(); ja.r = h->r.data(); ja.s = h->s.data(); ja.key_slot = h->jks.data(); ja.identity = h->jid.data();
     ja.qx = nullptr; ja.qy = nullptr; ja.gate_ok = h->gate_ok.data(); ja.J_cap = h->J_cap; ja.T = h->T;
@@ -75,8 +85,24 @@ int bd_plan(void* p, const uint8_t* blob, const uint32_t* env_off, int n_env)
         walk_tx(h->block.data(), env, t, (const uint8_t*)h->channel.data(), (uint32_t)h->channel.size(), h->txs[t], h->raw.data(), ja,
                 [&](uint32_t n) { uint32_t b = h->T + h->n_end; h->n_end += n; return b; });
     }
-    for (uint32_t j = 0; j < h->T + h->n_end; j++) resolve_job(h->block.data(), j, h->raw.data(), m, ja, h->txs.data());
-    return (int)h->n_end;
+    // the device's later stages stop at min(J_cap, T + n_end): the walk may hand out more slots than there are
+    const uint32_t J = std::min<uint64_t>(h->J_cap, (uint64_t)h->T + h->n_end);
+    h->stale = 0;
+    for (uint32_t j = 0; j < J; j++) {
+        if (h->raw[j].tx == 0xA5A5A5A5u || h->sha[j].len[0] == 0xA5A5A5A5u) { h->stale++; continue; }
+        resolve_job(h->block.data(), j, h->raw.data(), m, ja, h->txs.data());
+    }
+    return (int)(J - h->T);
+}
+int bd_plan(void* p, const uint8_t* blob, const uint32_t* env_off, int n_env) { return bd_plan_ex(p, blob, env_off, n_env, BD_ENDS_HINT, 0); }
+int bd_stale(void* p) { return (int)((H*)p)->stale; }
+// fabgpu_validate_block's split of a serialized common.Block: the envelopes' (offset, length) pairs, or -1 when the Block does not parse
+int bd_split_block(const uint8_t* block, size_t len, uint32_t* out, int cap)
+{
+    std::vector<fabgpu::blockval::Seg> envs;
+    if (!fabgpu::blockval::split_block(block, len, envs)) return -1;
+    for (size_t i = 0; i < envs.size() && (int)i < cap; i++) { out[2 * i] = envs[i].off; out[2 * i + 1] = envs[i].len; }
+    return (int)envs.size();
 }
 // job j (0 <= j < T + n_end): identity (-1 unused), gate_ok, r, s, message segments (6 uint32)
 void bd_job(void* p, int j, int* identity, int* gate_ok, uint8_t* r, uint8_t* s, uint32_t* segs)
@@ -96,7 +122,7 @@ void bd_decide(void* p, const uint8_t* sig_ok, const uint8_t* check_digests, uin
 {
     H* h = (H*)p;
     std::vector<uint8_t> dig(32 * (size_t)(h->J_cap + 2 * h->T), 0);
-    memcpy(&dig[32 * (size_t)h->J_cap], check_digests, 64 * (size_t)h->T);
+    if (h->T) memcpy(dig.data() + 32 * (size_t)h->J_cap, check_digests, 64 * (size_t)h->T);
     PolicyDev pol; pol.nodes = h->nodes.data(); pol.n_nodes = (int32_t)h->nodes.size() / 4; pol.principal_code = h->principal_code.data(); pol.n_principals = (int32_t)h->principal_code.size();
     pol.ns_blob = h->ns_blob.data(); pol.ns_off = h->ns_off.data(); pol.ns_root = h->ns_root.data(); pol.n_ns = (int32_t)h->ns_root.size();
     const MspDev m = h->msp();

@@ -1,12 +1,18 @@
 """The device-side block logic (fabric-mod_b200/csrc/blockdev.cuh: walk, dispatcher checks, gates, decisions), compiled for the host,
 against the oracle's restatement of the reference's validator (oracle/blockval.py), on the CPU: every fault class of
 tools/blockgen.py, per-chaincode policies, policy-evaluator semantics, de-duplication, duplicates, structural corner cases."""
+import functools
+import os
+import random
+
 import numpy as np
+import pytest
 
 from oracle import blockval as ob
 from tools import blockgen
 from tools import fabricpb as pb
 import blockutil
+import wiremut
 
 
 # ---- the device-side implementation of the same logic (blockdev.cuh), executed on the host ---------------------------------
@@ -184,3 +190,235 @@ def test_device_logic_with_hundreds_of_client_identities():
         return x or 1
     hashes = {h(i[0]) for i in ids}
     assert len(hashes) == len(ids)                      # head + tail alone gave one value per MSP id
+
+
+# ---- wire-level fuzzing of the block parser (tests/wiremut.py) -----------------------------------------------------------------
+def test_wire_mutation_corpus_matches_oracle():
+    """Every mutation kind at every message level of a transaction: the device logic's flag equals the oracle's for every transaction,
+    and every kind changes some verdict (no kind passes without reaching a check)."""
+    net, ids, nodes, pol, blocks = wiremut.corpus()
+    seen, changed = set(), set()
+    for blk, info, labels, exp in blocks:
+        got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, nodes, net.principals, policies=pol)
+        bad = [(t, labels[t], int(exp[t]), int(got[t])) for t in range(len(exp)) if got[t] != exp[t]]
+        assert not bad, bad[:10]
+        for t, lab in enumerate(labels):
+            if lab is None:
+                assert exp[t] == ob.VALID
+                continue
+            seen.add(lab)
+            if exp[t] != ob.VALID:
+                changed.add(lab[1])
+    assert sum(lab is not None for b in blocks for lab in b[2]) >= 3000          # mutated transactions
+    assert seen == {(p, k) for p in wiremut.TX_PARTS for k in wiremut.KINDS if k != "chdr_int" or p == "ChannelHeader"}
+    assert changed == set(wiremut.KINDS)
+
+
+def _one_tx():
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    blk, _ = blockgen.build_block(net, 1, 3, {}, seed=5, nthreads=2)
+    env = pb.parse(pb.parse(blk, ob.S_BLOCK)["data"], ob.S_BLOCKDATA)["data"][0]
+    e = pb.parse(env, ob.S_ENVELOPE)
+    return net, ids, env, e["payload"], e["signature"]
+
+
+def _flags_both(net, ids, envs):
+    blk = pb.block(1, envs)
+    exp = ob.validate_block(blk, ids, net.channel, net.policy_n_of(3), net.principals, known=_known(ids))
+    blob, off = _envs(blk)
+    return exp.tolist(), blockutil.device_logic_flags(blob, off, ids, net.channel, net.policy_n_of(3), net.principals).tolist()
+
+
+def test_field_number_2_pow_32_plus_2_is_an_unknown_field():
+    net, ids, env, _, _ = _one_tx()
+    assert _flags_both(net, ids, [env + pb.f_bytes((1 << 32) + 2, b"xyz")]) == ([ob.VALID], [ob.VALID])
+
+
+def test_aliased_signature_field_does_not_replace_the_signature():
+    net, ids, _, payload, sig = _one_tx()
+    env = pb.f_bytes(1, payload) + pb.f_bytes(2, b"\x30\x06\x02\x01\x01\x02\x01\x01") + pb.f_bytes((1 << 32) + 2, sig)
+    assert _flags_both(net, ids, [env]) == ([ob.BAD_CREATOR_SIGNATURE], [ob.BAD_CREATOR_SIGNATURE])
+
+
+def test_field_number_2_pow_29_plus_2_is_an_unknown_field():
+    net, ids, env, payload, sig = _one_tx()
+    assert _flags_both(net, ids, [env + pb.f_bytes((1 << 29) + 2, b"xyz")]) == ([ob.VALID], [ob.VALID])
+    env2 = pb.f_bytes(1, payload) + pb.f_bytes(2, b"\x30\x06\x02\x01\x01\x02\x01\x01") + pb.f_bytes((1 << 29) + 2, sig)
+    assert _flags_both(net, ids, [env2]) == ([ob.BAD_CREATOR_SIGNATURE], [ob.BAD_CREATOR_SIGNATURE])
+
+
+@pytest.mark.parametrize("value,code", [(3 + (1 << 32), ob.VALID), (3 + (1 << 63), ob.VALID), ((1 << 64) - 1, ob.BAD_COMMON_HEADER),
+                                        ((1 << 32) - 3, ob.BAD_COMMON_HEADER), (2 + (1 << 32), ob.UNSUPPORTED_TX_PAYLOAD)])
+def test_channel_header_type_is_an_int32(value, code):
+    """ChannelHeader.type is an int32: the decoder keeps the varint's low 32 bits (3 + 2^32 is an endorser transaction, -1 sent
+    as a 10-byte varint is -1)."""
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+
+    def mut(t, part, b):
+        if part != "ChannelHeader":
+            return b
+        return b"".join(wiremut.enc(*f) for f in wiremut.split(b) if f[0] != 1) + pb.f_uint(1, value)
+    blk, info = blockgen.build_block(net, 2, 3, {}, seed=5, nthreads=2, mutate=mut)
+    exp = ob.validate_block(blk, ids, net.channel, net.policy_n_of(3), net.principals, known=_known(ids))
+    got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, net.policy_n_of(3), net.principals)
+    assert exp.tolist() == [code, code] and got.tolist() == exp.tolist()
+
+
+def test_epoch_2_pow_64_minus_1_is_a_bad_header():
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    mut = lambda t, part, b: b + pb.f_uint(6, (1 << 64) - 1) if part == "ChannelHeader" else b
+    blk, info = blockgen.build_block(net, 1, 3, {}, seed=5, nthreads=2, mutate=mut)
+    exp = ob.validate_block(blk, ids, net.channel, net.policy_n_of(3), net.principals, known=_known(ids))
+    got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, net.policy_n_of(3), net.principals)
+    assert exp.tolist() == got.tolist() == [ob.BAD_COMMON_HEADER]
+
+
+def _oracle_split(blk):
+    try:
+        return pb.parse(pb.parse(blk, ob.S_BLOCK)["data"] or b"", ob.S_BLOCKDATA)["data"]
+    except pb.PbError:
+        return None
+
+
+def test_split_block_matches_oracle_fuzz():
+    """split_block (blockval.cpp) finds the same envelopes as the oracle's Block / BlockData parse, or fails where it fails, under every
+    mutation kind of the Block and of its BlockData."""
+    mutants = wiremut.block_mutants()
+    failed = 0
+    for i, (kind, m) in enumerate(mutants):
+        exp = _oracle_split(m)
+        assert blockutil.split_block(m) == exp, (kind, i, m.hex())
+        failed += exp is None
+    assert len(mutants) >= 900 and 0 < failed < len(mutants)
+
+
+def test_split_block_aliased_data_field():
+    """A Block field numbered 2^32 + 2 is not Block.data: the envelopes are those of the real data field."""
+    net = blockgen.Network()
+    blk, _ = blockgen.build_block(net, 3, 3, {}, seed=5, nthreads=2)
+    other, _ = blockgen.build_block(net, 2, 3, {}, seed=6, nthreads=2)
+    other_data = pb.parse(other, ob.S_BLOCK)["data"]
+    for forged in (blk + pb.f_bytes((1 << 32) + 2, other_data), pb.f_bytes((1 << 32) + 2, other_data) + blk):
+        assert blockutil.split_block(forged) == _oracle_split(forged) == _oracle_split(blk)
+        assert len(_oracle_split(forged)) == 3
+
+
+def test_job_overflow_writes_dead_records():
+    """More than BD_ENDS_HINT endorsements per transaction on average: the endorsement-job arrays fill up and the transactions that do not
+    fit go to the CPU validator (NOT_VALIDATED).  The arrays start out as garbage (what the previous block or cudaMalloc left), so every
+    slot the walk hands out must get a record: a live job or a dead one.  Transactions that fit are exact."""
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    n = 12
+    faults = {t: "many_endorsements" for t in range(n) if t % 4 != 1}       # 21 endorsements each, 3 for every fourth transaction
+    blk, info = blockgen.build_block(net, n, 3, faults, seed=9, nthreads=2)
+    exp = ob.validate_block(blk, ids, net.channel, net.policy_n_of(3), net.principals, known=_known(ids))
+    assert (exp == ob.VALID).all()
+    for hint in (16, 8, 3):
+        got, stale = blockutil.device_logic_run(info["env_blob"], info["env_off"], ids, net.channel, net.policy_n_of(3), net.principals,
+                                                ends_hint=hint, poison=True)
+        assert stale == 0, hint
+        e_cap, used, fits = n * hint, 0, []
+        for t in range(n):                                   # the host build hands out job slots in transaction order
+            k = 21 if t in faults else 3
+            fits.append(used + k <= e_cap)
+            used += k
+        assert not all(fits) and any(fits)
+        for t in range(n):
+            assert got[t] == (exp[t] if fits[t] else ob.NOT_VALIDATED), (hint, t)
+
+
+def _edge_flags(net, n_tx, nodes, policies, **shape):
+    ids = blockutil.identities_of(net)
+    blk, info = blockgen.build_block(net, n_tx, 3, {}, seed=19, nthreads=2, **shape)
+    exp = ob.validate_block(blk, ids, net.channel, nodes, net.principals, policies=policies, known=_known(ids))
+    got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, nodes, net.principals, policies=policies)
+    return exp.tolist(), got.tolist()
+
+
+@pytest.mark.parametrize("case", blockutil.capacity_edge_cases(), ids=lambda c: c[0])
+def test_capacity_edges(case):
+    """BD_MAX_NS_SEEN, BD_MAX_NS and BD_MAX_SIGNERS: exact at the limit, NOT_VALIDATED one past it (the CPU validator decides)."""
+    name, net, n_tx, nodes, pol, shape, at, past = case
+    exp, got = _edge_flags(net, n_tx, nodes, pol, **shape)
+    assert exp[at] == exp[past] == ob.VALID
+    assert got[at] == ob.VALID and got[past] == ob.NOT_VALIDATED
+    assert [g for i, g in enumerate(got) if i != past] == [e for i, e in enumerate(exp) if i != past]
+
+
+def _chain(depth):
+    """NOutOf(1) nested `depth` times over SignedBy(Org1MSP): the SignedBy node sits at depth `depth`."""
+    return np.array([(0, 1, i + 1, 1) for i in range(depth)] + [(1, 0, 0, 0)], np.int32)
+
+
+def test_policy_depth_limit():
+    """eval_policy evaluates trees BD_MAX_POLICY_DEPTH (12) deep exactly; one level deeper it would fail where the reference accepts,
+    which is why fabgpu_msp_configure refuses such trees (tests/test_gpu_block.py)."""
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    blk, info = blockgen.build_block(net, 8, 3, {}, seed=5, nthreads=2)
+    for depth, device_exact in ((0, True), (12, True), (13, False)):
+        exp = ob.validate_block(blk, ids, net.channel, _chain(depth), net.principals, known=_known(ids))
+        got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, _chain(depth), net.principals)
+        assert (exp == ob.VALID).sum() >= 6
+        assert (got.tolist() == exp.tolist()) == device_exact, depth
+
+
+def test_block_parser_memory_safety_under_sanitizers(tmp_path):
+    """split_block, walk_tx, resolve_job and decide_tx built with -fsanitize=address,undefined and run as a separate process over the
+    mutation corpus, the Block-level mutants, the capacity edges and job-array overflow (small job arrays): no sanitizer report."""
+    import struct
+    import subprocess
+    from util import ROOT
+    d = os.path.join(ROOT, "tests", "host_sim")
+    exe = str(tmp_path / "blockdev_asan")
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer",
+                           "-o", exe, os.path.join(d, "blockdev_asan.cpp"), os.path.join(ROOT, "fabric-mod_b200", "csrc", "blockval.cpp")])
+    net, ids, _, _, blocks = wiremut.corpus()
+    u32 = lambda v: struct.pack("<I", v)
+    lb = lambda b: u32(len(b)) + bytes(b)
+    nodes = np.ascontiguousarray(net.policy_n_of(2), np.int32)
+    head = u32(len(ids)) + b"".join(lb(i[0]) + lb(i[1].encode()) + bytes([1 if i[3] else 0]) for i in ids)
+    head += u32(nodes.shape[0]) + nodes.tobytes() + u32(len(net.principals)) + b"".join(lb(p.encode()) for p in net.principals) + lb(net.channel.encode())
+    items = [(16, b[0]) for b in blocks] + [(1, b[0]) for b in blocks[:2]] + [(16, m) for _, m in wiremut.block_mutants()]
+    for case in blockutil.capacity_edge_cases():
+        items.append((16, blockgen.build_block(case[1], case[2], 3, {}, seed=19, nthreads=2, **case[5])[0]))
+    overflow, _ = blockgen.build_block(net, 12, 3, {t: "many_endorsements" for t in range(12) if t % 4 != 1}, seed=9, nthreads=2)
+    items += [(16, overflow), (3, overflow)]
+    corpus = tmp_path / "corpus.bin"
+    corpus.write_bytes(head + u32(len(items)) + b"".join(u32(h) + lb(b) for h, b in items))
+    env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:halt_on_error=1", UBSAN_OPTIONS="halt_on_error=1:print_stacktrace=1")
+    run = subprocess.run([exe, str(corpus)], capture_output=True, text=True, env=env, timeout=600)
+    assert run.returncode == 0 and "runtime error" not in run.stderr and "Sanitizer" not in run.stderr, run.stderr[-4000:]
+    parsed = sum(_oracle_split(b) is not None for _, b in items)
+    assert run.stdout.split()[:4] == ["blocks", str(len(items)), "parsed", str(parsed)], run.stdout
+    assert int(run.stdout.split()[5]) > 3000
+
+
+@pytest.mark.parametrize("field,v,last,code", wiremut.TEN_BYTE_CASES)
+def test_ten_byte_varint_last_byte(field, v, last, code):
+    """golang/protobuf's decodeVarint takes a 10th byte only when it is 0 or 1; a larger one overflows and the ChannelHeader does not
+    unmarshal.  epoch = 0 with a 10th byte of 2 is a bad header, not epoch 0."""
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    blk, info = wiremut.ten_byte_block(net, field, v, last)
+    exp = ob.validate_block(blk, ids, net.channel, net.policy_n_of(3), net.principals, known=_known(ids))
+    got = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, net.policy_n_of(3), net.principals)
+    assert exp.tolist() == [code, code] and got.tolist() == exp.tolist()
+
+
+@pytest.mark.parametrize("last", [0, 1, 2, 0x7F])
+def test_ten_byte_varint_in_block_and_envelope(last):
+    """The same rule for the lengths and values split_block and the envelope walk read: an unknown varint field whose 10th byte is
+    0 or 1 is skipped; a larger 10th byte makes the Block (split_block) or the Envelope (INVALID_OTHER_REASON) fail to parse."""
+    net, ids, env, _, _ = _one_tx()
+    extra = wiremut.uvarint(9 << 3) + wiremut.ten_byte_varint(5, last)
+    exp_code = ob.VALID if last < 2 else ob.INVALID_OTHER_REASON
+    assert _flags_both(net, ids, [env + extra]) == ([exp_code], [exp_code])
+    blk = pb.block(1, [env]) + extra
+    assert blockutil.split_block(blk) == _oracle_split(blk) == (None if last >= 2 else [env])
+    blk = pb.block(1, [env]) + wiremut.uvarint(9 << 3 | 2) + wiremut.ten_byte_varint(8, last) + b"x" * 8          # a length in 10 bytes
+    assert blockutil.split_block(blk) == _oracle_split(blk) == (None if last else [env])          # 1: bit 63 of the length

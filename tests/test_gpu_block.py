@@ -7,6 +7,7 @@ import pytest
 
 from oracle import blockval as ob
 from tools import blockgen
+from tools import fabricpb as pb
 from util import pkg
 import blockutil
 
@@ -175,3 +176,125 @@ def test_two_blocks_in_flight(ctx):
     assert ctx.validate_envelopes(blocks[1][1], blocks[1][2]).tolist() == blocks[1][3].tolist()
     assert ctx.validate_envelopes_async(1, np.zeros(1, np.uint8), np.zeros(1, np.uint32)) == 0
     assert ctx.validate_wait(1, 1).shape[0] == 0
+
+
+# ---- wire-level fuzzing: the host-side tests/test_blockval_host.py corpus on the device -----------------------------------------
+def test_wire_mutation_corpus_all_entry_points(ctx):
+    """Every block of the mutation corpus (3 080 mutated transactions, every mutation kind at every message level) through the envelope form,
+    the serialized-Block form (split_block), a pinned buffer and the two async slots: the flags equal the oracle's and the host
+    build's, byte for byte."""
+    import wiremut
+    net, ids, nodes, pol, blocks = wiremut.corpus()
+    ctx.msp_configure(ids, nodes, net.principals, net.channel, policies=pol)
+    for k, (blk, info, labels, exp) in enumerate(blocks):
+        host = blockutil.device_logic_flags(info["env_blob"], info["env_off"], ids, net.channel, nodes, net.principals, policies=pol)
+        assert host.tolist() == exp.tolist()
+        assert ctx.validate_envelopes(info["env_blob"], info["env_off"]).tolist() == exp.tolist(), k
+        assert ctx.validate_block(blk).tolist() == exp.tolist(), k
+        if k % 2 == 0:
+            pinned = ctx.block_buffer(len(blk))
+            pinned[:] = np.frombuffer(blk, np.uint8)
+            assert ctx.validate_block(pinned).tolist() == exp.tolist(), k
+    for (b0, i0, _, e0), (b1, i1, _, e1) in zip(blocks[0::2], blocks[1::2]):
+        n0 = ctx.validate_envelopes_async(0, i0["env_blob"], i0["env_off"])
+        n1 = ctx.validate_block_async(1, b1)
+        assert ctx.validate_wait(1, n1).tolist() == e1.tolist()
+        assert ctx.validate_wait(0, n0).tolist() == e0.tolist()
+
+
+def test_block_with_aliased_data_field(ctx):
+    """A Block field numbered 2^32 + 2 carrying other envelopes is an unknown field, not Block.data."""
+    net = blockgen.Network()
+    blk, _ = blockgen.build_block(net, 30, 3, {}, seed=41)
+    other, _ = blockgen.build_block(net, 5, 3, {2: "bad_creator_sig"}, seed=42)
+    forged = blk + pb.f_bytes((1 << 32) + 2, pb.parse(other, ob.S_BLOCK)["data"])
+    exp = _oracle(forged, net, net.policy_n_of(3))
+    assert exp.tolist() == _oracle(blk, net, net.policy_n_of(3)).tolist() and len(exp) == 30
+    _configure(ctx, net, 3)
+    assert ctx.validate_block(forged).tolist() == exp.tolist()
+
+
+def test_job_overflow_after_a_larger_block():
+    """A block that needs more endorsement jobs than the job arrays hold, first on fresh device memory, then on a slot whose arrays
+    hold a larger block's jobs: every flag is the oracle's or NOT_VALIDATED, only the few transactions that do not fit get the latter,
+    and the slot validates the larger block exactly afterwards.  The flags cannot show whether the walk wrote dead records into the
+    slots it gave up (a stale record belongs to no transaction of this block); test_job_overflow_writes_dead_records in
+    tests/test_blockval_host.py checks that on the host build, with the job arrays filled with garbage."""
+    c = pkg().binding.Context(max_batch=8192)
+    try:
+        net = blockgen.Network()
+        n = 12
+        small, _ = blockgen.build_block(net, n, 3, {t: "many_endorsements" for t in range(n) if t % 4 != 1}, seed=9)   # 198 jobs, room for 192
+        exp = _oracle(small, net, net.policy_n_of(3))
+        assert (exp == ob.VALID).all()
+        big, _ = blockgen.build_block(net, 3000, 3, blockutil.fault_map(3000), seed=43)
+        exp_big = _oracle(big, net, net.policy_n_of(3))
+        _configure(c, net, 3)
+
+        def check(got):
+            assert all(g in (e, ob.NOT_VALIDATED) for g, e in zip(got.tolist(), exp.tolist())), got
+            assert 1 <= int((got == ob.NOT_VALIDATED).sum()) <= 2
+        for slot in (0, 1):
+            check(c.validate_wait(slot, c.validate_block_async(slot, small)))
+            assert c.validate_wait(slot, c.validate_block_async(slot, big)).tolist() == exp_big.tolist()
+            check(c.validate_wait(slot, c.validate_block_async(slot, small)))
+        assert c.validate_block(big).tolist() == exp_big.tolist()           # and nothing stale is left behind
+    finally:
+        c.close()
+
+
+@pytest.mark.parametrize("case", blockutil.capacity_edge_cases(), ids=lambda c: c[0])
+def test_capacity_edges(ctx, case):
+    """BD_MAX_NS_SEEN, BD_MAX_NS, BD_MAX_SIGNERS on the device: exact at the limit, NOT_VALIDATED one past it."""
+    name, net, n_tx, nodes, pol, shape, at, past = case
+    blk, _ = blockgen.build_block(net, n_tx, 3, {}, seed=19, **shape)
+    exp = _oracle(blk, net, nodes, pol)
+    ctx.msp_configure(blockutil.identities_of(net), nodes, net.principals, net.channel, policies=pol)
+    got = ctx.validate_block(blk).tolist()
+    assert exp[at] == exp[past] == ob.VALID and got[past] == ob.NOT_VALIDATED
+    assert [g for i, g in enumerate(got) if i != past] == [e for i, e in enumerate(exp.tolist()) if i != past]
+
+
+def _chain(depth):
+    return np.array([(0, 1, i + 1, 1) for i in range(depth)] + [(1, 0, 0, 0)], np.int32)
+
+
+def test_msp_configure_refuses_policies_it_cannot_evaluate(ctx):
+    """Deeper than BD_MAX_POLICY_DEPTH, cyclic, or a SignedBy principal out of range: FABGPU_E_ARG (the caller validates on the CPU),
+    also when the tree is one of several namespace policies.  At the depth limit the flags are exact."""
+    binding = pkg().binding
+    net = blockgen.Network()
+    ids = blockutil.identities_of(net)
+    a = net.policy_n_of(3)
+    refused = [_chain(13), np.array([(0, 1, 1, 1), (0, 1, 0, 1)], np.int32), np.array([(0, 1, 1, 1), (0, 1, 1, 1)], np.int32),
+               np.array([(0, 1, 1, 1), (1, 4, 0, 0)], np.int32), np.array([(1, -1, 0, 0)], np.int32)]
+    for nodes in refused:
+        with pytest.raises(binding.FabGpuError) as e:
+            ctx.msp_configure(ids, nodes, net.principals, net.channel)
+        assert e.value.code == binding.E_ARG
+    deep = _chain(13).copy(); deep[:-1, 2] += a.shape[0]
+    with pytest.raises(binding.FabGpuError) as e:
+        ctx.msp_configure(ids, np.concatenate([a, deep]), net.principals, net.channel, policies={blockgen.CHAINCODE: 0, "deepcc": int(a.shape[0])})
+    assert e.value.code == binding.E_ARG
+    blk, _ = blockgen.build_block(net, 20, 3, blockutil.fault_map(20), seed=44)
+    ctx.msp_configure(ids, _chain(12), net.principals, net.channel)
+    exp = _oracle(blk, net, _chain(12))
+    assert ctx.validate_block(blk).tolist() == exp.tolist() and (exp == ob.VALID).sum() >= 10
+
+
+def test_ten_byte_varint_last_byte(ctx):
+    """A varint's 10th byte may only be 0 or 1 (golang/protobuf's decodeVarint): ChannelHeader.type and epoch written in 10 bytes,
+    and an unknown Block field whose 10-byte varint overflows (the Block does not parse)."""
+    import wiremut
+    net = blockgen.Network()
+    _configure(ctx, net, 3)
+    for field, v, last, code in wiremut.TEN_BYTE_CASES:
+        blk, _ = wiremut.ten_byte_block(net, field, v, last)
+        exp = _oracle(blk, net, net.policy_n_of(3))
+        assert exp.tolist() == [code, code] and ctx.validate_block(blk).tolist() == exp.tolist(), (field, last)
+    blk, _ = blockgen.build_block(net, 3, 3, {}, seed=5)
+    for last in (0, 1):
+        assert ctx.validate_block(blk + wiremut.uvarint(9 << 3) + wiremut.ten_byte_varint(5, last)).tolist() == _oracle(blk, net, net.policy_n_of(3)).tolist()
+    with pytest.raises(pkg().binding.FabGpuError) as e:
+        ctx.validate_block(blk + wiremut.uvarint(9 << 3) + wiremut.ten_byte_varint(5, 2))
+    assert e.value.code == pkg().binding.E_ARG

@@ -33,6 +33,18 @@ def chaincode_id(name: str, version: str = "") -> bytes:
     return pb.f_bytes(2, name.encode()) + (pb.f_bytes(3, version.encode()) if version else b"")
 
 
+# The message levels build_block's `mutate` hook sees, innermost first.  "ChaincodeID" is both the header extension's and the
+# chaincode action's; the read/write-set levels occur once per namespace.
+PARTS = ("ChaincodeID", "ChaincodeHeaderExtension", "ChannelHeader", "SignatureHeader", "ChaincodeProposalPayload", "KVRWSet", "HashedRWSet",
+         "CollectionHashedReadWriteSet", "NsReadWriteSet", "TxReadWriteSet", "ChaincodeEvent", "ChaincodeAction", "ProposalResponsePayload",
+         "Endorsement", "ChaincodeEndorsedAction", "ChaincodeActionPayload", "TransactionAction", "Transaction", "Header", "Payload", "Envelope",
+         "Block")
+
+
+def _same(part, b):
+    return b
+
+
 def kv_rwset(n_reads=1, n_writes=1, tag=b"k") -> bytes:
     """kvrwset.KVRWSet{reads=1, writes=3}: KVRead{key=1}, KVWrite{key=1, value=3}."""
     out = b""
@@ -43,9 +55,26 @@ def kv_rwset(n_reads=1, n_writes=1, tag=b"k") -> bytes:
     return out
 
 
-def tx_rwset(namespaces) -> bytes:
-    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes)."""
-    return b"".join(pb.f_bytes(2, pb.f_bytes(1, name.encode()) + pb.f_bytes(2, kv_rwset(nr, nw, name.encode()))) for name, nr, nw in namespaces)
+def hashed_rwset(n_writes, tag=b"k") -> bytes:
+    """kvrwset.HashedRWSet{hashed_reads=1, hashed_writes=2}: KVReadHash{key_hash=1}, KVWriteHash{key_hash=1, value_hash=3}."""
+    h = lambda s: hashlib.sha256(s).digest()
+    return pb.f_bytes(1, pb.f_bytes(1, h(tag + b"-hr"))) + b"".join(pb.f_bytes(2, pb.f_bytes(1, h(tag + b"-hw%d" % i)) + pb.f_bytes(3, h(b"v%d" % i)))
+                                                                  for i in range(n_writes))
+
+
+def tx_rwset(namespaces, mut=_same) -> bytes:
+    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes[, n_hashed_writes]).  A fourth
+    entry adds one private-data collection, NsReadWriteSet.collection_hashed_rwset = CollectionHashedReadWriteSet{collection_name=1,
+    hashed_rwset=2} with that many hashed writes.  mut(part, bytes): see build_block."""
+    out = b""
+    for ns in namespaces:
+        name, nr, nw = ns[:3]
+        body = pb.f_bytes(1, name.encode()) + pb.f_bytes(2, mut("KVRWSet", kv_rwset(nr, nw, name.encode())))
+        if len(ns) > 3:
+            coll = pb.f_bytes(1, b"collection") + pb.f_bytes(2, mut("HashedRWSet", hashed_rwset(ns[3], name.encode())))
+            body += pb.f_bytes(3, mut("CollectionHashedReadWriteSet", coll))
+        out += pb.f_bytes(2, mut("NsReadWriteSet", body))
+    return mut("TxReadWriteSet", out)
 
 
 class Identity:
@@ -107,17 +136,24 @@ class Network:
         return np.array(nodes, np.int32)
 
 
-def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, seed=7, number=1, nthreads=None):
-    """faults: {tx_index: fault_name}.  Returns (block_bytes, info) where info['expected_hint'][i] is the validation code the
-    construction aims at (the oracle decides the truth)."""
+def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, seed=7, number=1, nthreads=None, mutate=None, namespaces=None,
+                endorsers=None, events=None):
+    """faults: {tx_index: fault_name}.  Returns (block_bytes, info); the oracle decides the validation codes.
+    mutate(t, part, data) -> bytes rewrites the serialized message `part` (one of PARTS; t = None for the Block) of transaction t as
+    it is assembled: the tx id, the proposal hash, the endorsement and creator signatures and every enclosing length prefix are
+    then computed from the returned bytes, as a client and its endorsers would.  namespaces(t) -> the read/write set's namespaces
+    (see tx_rwset); endorsers(t) -> the Identity list that endorses t; events(t) -> True: the chaincode action carries a
+    ChaincodeEvent of the invoked chaincode.  Without these arguments the output does not depend on them."""
     import ctypes
     faults = faults or {}
     rng = np.random.default_rng(seed)
     L = workload.lib()
+    hook = mutate or (lambda t, part, b: b)
     # ---- phase 1: build every message that must be signed ------------------------------------------------------
     txs = []
     sign_msgs, sign_keys = [], []
     for t in range(n_tx):
+        mut = lambda part, b, t=t: hook(t, part, b)
         f = faults.get(t)
         client = net.clients[t % len(net.clients)]
         if f == "unknown_creator":
@@ -129,21 +165,30 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
             nonce = txs[t - 1]["nonce"]
             client = txs[t - 1]["client"]
         creator = client.serialized
-        txid = hashlib.sha256(nonce + creator).hexdigest()
+        shdr0 = pb.signature_header(creator, b"" if f == "empty_nonce" else nonce)
+        shdr = mut("SignatureHeader", shdr0)
+        id_src = nonce + creator
+        if shdr != shdr0:                                                  # the tx id of the nonce and creator a decoder reads
+            try:
+                sh = pb.parse(shdr, {1: ("creator", "bytes"), 2: ("nonce", "bytes")})
+                id_src = (sh["nonce"] or b"") + (sh["creator"] or b"")
+            except pb.PbError:
+                pass
+        txid = hashlib.sha256(id_src).hexdigest()
         if f == "bad_txid":
             txid = hashlib.sha256(b"x" + nonce + creator).hexdigest()
         channel = net.channel if f != "wrong_channel" else "other-channel"
         htype = pb.HEADER_TYPE_ENDORSER_TRANSACTION if f != "config_update_type" else pb.HEADER_TYPE_CONFIG_UPDATE
-        hext = pb.f_bytes(2, chaincode_id(CHAINCODE))                      # peer.ChaincodeHeaderExtension{chaincode_id = 2}
+        hext = pb.f_bytes(2, mut("ChaincodeID", chaincode_id(CHAINCODE)))  # peer.ChaincodeHeaderExtension{chaincode_id = 2}
         if f == "bad_header_extension":
             hext = b"\x12\x7fshort"                                         # length prefix runs past the end
-        chdr = pb.channel_header(htype, channel, txid, epoch=(5 if f == "nonzero_epoch" else 0), extension=hext)
-        shdr = pb.signature_header(creator, b"" if f == "empty_nonce" else nonce)
-        cpp = pb.f_bytes(1, b"invoke-args-" + bytes(rng.integers(0, 256, 40, dtype=np.uint8)))     # ChaincodeProposalPayload
+        hext = mut("ChaincodeHeaderExtension", hext)
+        chdr = mut("ChannelHeader", pb.channel_header(htype, channel, txid, epoch=(5 if f == "nonzero_epoch" else 0), extension=hext))
+        cpp = mut("ChaincodeProposalPayload", pb.f_bytes(1, b"invoke-args-" + bytes(rng.integers(0, 256, 40, dtype=np.uint8))))
         phash = hashlib.sha256(chdr + shdr + cpp).digest()
         if f == "bad_proposal_hash":
             phash = bytes(32)
-        nss = [(CHAINCODE, 2, 2)]
+        nss = list(namespaces(t)) if namespaces else [(CHAINCODE, 2, 2)]
         if f == "writes_strict_namespace":
             nss.append((STRICT_NAMESPACE, 0, 1))                            # cc-to-cc call that WRITES there: that policy applies too
         if f == "reads_strict_namespace":
@@ -152,18 +197,22 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
             nss.append((UNKNOWN_NAMESPACE, 0, 1))
         if f == "dup_namespace":
             nss.append((CHAINCODE, 1, 0))
-        rwset = tx_rwset(nss)
+        rwset = tx_rwset(nss, mut)
         if f == "bad_rwset":
             rwset = pb.f_bytes(2, b"\x0a\x7fnamespace-length-runs-past-the-end")
-        ccact = pb.f_bytes(1, rwset) + pb.f_bytes(4, chaincode_id("othercc" if f == "cc_name_mismatch" else CHAINCODE, "" if f == "empty_cc_version" else "1.0"))
+        ccact = pb.f_bytes(1, rwset) + pb.f_bytes(4, mut("ChaincodeID", chaincode_id("othercc" if f == "cc_name_mismatch" else CHAINCODE,
+                                                                                     "" if f == "empty_cc_version" else "1.0")))
         if f == "event_wrong_cc":
-            ccact += pb.f_bytes(2, pb.f_bytes(1, b"othercc") + pb.f_bytes(3, b"evt"))
-        prp = pb.proposal_response_payload(phash, ccact)
+            ccact += pb.f_bytes(2, mut("ChaincodeEvent", pb.f_bytes(1, b"othercc") + pb.f_bytes(3, b"evt")))
+        elif events and events(t):                                         # ChaincodeEvent{chaincode_id=1, event_name=3, payload=4}
+            ccact += pb.f_bytes(2, mut("ChaincodeEvent", pb.f_bytes(1, CHAINCODE.encode()) + pb.f_bytes(3, b"evt") + pb.f_bytes(4, b"event-payload")))
+        prp = pb.proposal_response_payload(phash, mut("ChaincodeAction", ccact))
         if f == "no_prp_extension":
             prp = pb.f_bytes(1, phash)
+        prp = mut("ProposalResponsePayload", prp)
         # endorsers: the first n_endorsements orgs, rotated per tx
         order = [(t + k) % net.n_orgs for k in range(n_endorsements)]
-        ends = [net.peers[o] for o in order]
+        ends = list(endorsers(t)) if endorsers else [net.peers[o] for o in order]
         if f == "dup_endorser":
             ends[-1] = ends[0]
         if f == "unknown_endorser":
@@ -202,10 +251,12 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
             i0 = tx["first_end_sig"]
             rr = int.from_bytes(bytes(end_r[i0]), "big"); ss = N_ORDER - int.from_bytes(bytes(end_s[i0]), "big")
             sigs[0] = _der_sig(rr, ss)
-        action = pb.chaincode_endorsed_action(tx["prp"], [pb.endorsement(e.serialized, sg) for e, sg in zip(tx["ends"], sigs)])
-        cap = pb.chaincode_action_payload(tx["cpp"], action)
-        data = pb.transaction([pb.transaction_action(tx["shdr"], cap)])
-        pl = pb.payload(pb.header(tx["chdr"], tx["shdr"]), data)
+        mut = lambda part, b, t=t: hook(t, part, b)
+        action = mut("ChaincodeEndorsedAction", pb.chaincode_endorsed_action(
+            tx["prp"], [mut("Endorsement", pb.endorsement(e.serialized, sg)) for e, sg in zip(tx["ends"], sigs)]))
+        cap = mut("ChaincodeActionPayload", pb.chaincode_action_payload(tx["cpp"], action))
+        data = mut("Transaction", pb.transaction([mut("TransactionAction", pb.transaction_action(tx["shdr"], cap))]))
+        pl = mut("Payload", pb.payload(mut("Header", pb.header(tx["chdr"], tx["shdr"])), data))
         payloads.append(pl); payload_keys.append(tx["client"].priv_index)
     pay_sigs, _, _ = sign_all(payloads, payload_keys)
     envs = []
@@ -219,8 +270,8 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
         env = pb.envelope(payloads[t], sg)
         if f == "bad_payload":
             env = pb.f_bytes(1, b"\xff\xff\xff\xff garbage that is not a Payload") + pb.f_bytes(2, sg)
-        envs.append(env)
+        envs.append(hook(t, "Envelope", env))
     env_off = np.zeros(len(envs) + 1, np.uint32)
     env_off[1:] = np.cumsum([len(e) for e in envs])
-    return pb.block(number, envs), dict(n_tx=n_tx, faults=dict(faults), n_sigs=n_tx + sum(len(tx["ends"]) for tx in txs),
+    return hook(None, "Block", pb.block(number, envs)), dict(n_tx=n_tx, faults=dict(faults), n_sigs=n_tx + sum(len(tx["ends"]) for tx in txs),
                                         env_blob=b"".join(envs), env_off=env_off)   # Block.Data.Data as the Go validator holds it

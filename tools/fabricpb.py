@@ -111,6 +111,7 @@ class PbError(Exception):
 
 
 def read_varint(b, off):
+    """golang/protobuf's decodeVarint: at most 10 bytes, and the 10th may only be 0 or 1 (bit 63); anything else overflows."""
     v = 0
     shift = 0
     while True:
@@ -118,12 +119,12 @@ def read_varint(b, off):
             raise PbError("truncated varint")
         c = b[off]
         off += 1
+        if shift == 63 and c > 1:
+            raise PbError("varint overflow")
         v |= (c & 0x7F) << shift
         if not c & 0x80:
-            return v & ((1 << 64) - 1), off
+            return v, off
         shift += 7
-        if shift >= 70:
-            raise PbError("varint overflow")
 
 
 def fields(b):
@@ -157,7 +158,8 @@ def fields(b):
 
 def parse(b, spec):
     """spec: {field_no: (name, kind)} with kind in 'bytes' | 'uint' | 'rep_bytes'.  Unknown fields are skipped; a known
-    field with the wrong wire type is an error (as in Go's proto.Unmarshal); later singular occurrences win."""
+    field with the wrong wire type is an error (as in Go's proto.Unmarshal -- not verified against golang/protobuf v1.3.3, see
+    DESIGN.md section 2); later singular occurrences win."""
     out = {name: ([] if kind == "rep_bytes" else None) for name, kind in spec.values()}
     for fno, wt, v in fields(b):
         if fno not in spec:
