@@ -303,8 +303,8 @@ FAB_HD bool ba_range_ok(const u256& r, const u256& s)
 // Stage between the exchanges, per signature: w = s^-1 R mod n  ->  u1 = e w, u2 = r w  ->  leaf indices.
 FAB_HD void ba_scalars(const u256& e, const u256& r, const u256& w, uint32_t* dig, int stride)
 {
-    const u256 u1 = sc_mul(sc_reduce_once(e), w);
-    const u256 u2 = sc_mul(r, w);
+    u256 u1, u2;
+    ecdsa_u1u2(e, r, w, u1, u2);
     ba_digits(u1, u2, dig, stride);
 }
 

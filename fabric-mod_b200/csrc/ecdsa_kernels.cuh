@@ -229,6 +229,63 @@ __global__ void peer_scatter_kernel(const uint32_t* __restrict__ local_words, ui
     peer_publish(po);
 }
 
+// ---- scalars of the key-table kernel, one shared inversion per CTA ---------------------------------------------------------------
+// ecdsa_prep_kernel runs before ecdsa_verify_cached_kernel on the same stream, one thread per signature: the range gate r, s in
+// [1, n-1], w = s^-1 by Montgomery's trick over the CTA (ba_inverse_lane, mod n: one warp of division-step inversions serves
+// FAB_PREP_THREADS signatures), then u1 = e w and u2 = r w.  A signature that fails the gate contributes 1 to the product and gets
+// u2 = 0, which no signature that passes it can have (r, w in [1, n-1] and n is prime): the chain kernel reads that as INVALID.
+// Signatures without a window table (key_slot < 0: mixed batches) contribute 1 too and get nothing written; the chain kernel skips them.
+// Scalars: 64 bytes per signature as four rows of uint4 -- [u1 limbs 0..3], [u1 4..7], [u2 0..3], [u2 4..7] -- each row `stride`
+// entries long (the launch bound n), so that every load and store of a warp is one contiguous 512-byte span.
+// The kernel needs few registers: several CTAs stay resident per SM, and while one CTA's warps wait for its inverter warp the others'
+// products and loads run.  (The `ba` kernels shared their inversions inside the 128-register chain kernel: one CTA per SM, seven of
+// eight warps idle at each exchange.)
+#ifndef FAB_PREP_THREADS
+#define FAB_PREP_THREADS 128           // signatures per shared inversion (DESIGN.md section 4.1: 64 / 128 / 256 measured)
+#endif
+#ifndef FAB_PREP_MINBLOCKS
+#define FAB_PREP_MINBLOCKS 6           // 128 threads x 80 registers (no spills): six CTAs per SM
+#endif
+__global__ void __launch_bounds__(FAB_PREP_THREADS, FAB_PREP_MINBLOCKS)
+ecdsa_prep_kernel(const int32_t* __restrict__ key_slot, const uint8_t* __restrict__ e, const uint8_t* __restrict__ r, const uint8_t* __restrict__ s,
+                  uint32_t n, uint4* __restrict__ scal, const uint32_t* __restrict__ n_dev, uint32_t n_base)
+{
+    constexpr int T = FAB_PREP_THREADS;
+    __shared__ uint32_t exa[8 * T], exb[8 * T];                // [limb][thread], as ba_cta_inverse
+    const uint32_t stride = n;
+    if (n_dev) n = min(n, n_base + *n_dev);
+    if (blockIdx.x * T >= n) return;                            // whole CTA past the device-side batch size (block path)
+    const int tid = threadIdx.x;
+    const uint32_t idx = blockIdx.x * T + tid;
+    const size_t o = (size_t)idx * 32;
+    const bool mine = idx < n && key_slot[idx] >= 0;           // signatures without a window table are not the chain kernel's
+    bool ok = false;
+    u256 rv = u256_zero(), v = u256_const(1, 0, 0, 0, 0, 0, 0, 0);
+    if (mine) {
+        rv = load_be32(r + o);
+        const u256 sv = load_be32(s + o);
+        ok = ba_range_ok(rv, sv);
+        if (ok) v = sv;
+    }
+#pragma unroll
+    for (int l = 0; l < 8; l++) exa[l * T + tid] = v.v[l];
+    __syncthreads();
+    if (tid < 32) ba_inverse_lane(true, exa + tid, exb + tid, T / 32, 32, T);     // inverter lane l: values l, l + 32, l + 64, ...
+    __syncthreads();
+    if (!mine) return;
+    u256 u1 = u256_zero(), u2 = u256_zero();
+    if (ok) {
+        u256 w;
+#pragma unroll
+        for (int l = 0; l < 8; l++) w.v[l] = exa[l * T + tid];
+        ecdsa_u1u2(load_be32(e + o), rv, w, u1, u2);
+    }
+    scal[idx] = make_uint4(u1.v[0], u1.v[1], u1.v[2], u1.v[3]);
+    scal[stride + idx] = make_uint4(u1.v[4], u1.v[5], u1.v[6], u1.v[7]);
+    scal[2 * (size_t)stride + idx] = make_uint4(u2.v[0], u2.v[1], u2.v[2], u2.v[3]);
+    scal[3 * (size_t)stride + idx] = make_uint4(u2.v[4], u2.v[5], u2.v[6], u2.v[7]);
+}
+
 #ifndef FAB_CACHED_THREADS
 #define FAB_CACHED_THREADS 512        // largest CTA the kernel may be launched with (launch_verify picks 128 / 256 / 512)
 #endif
@@ -236,22 +293,25 @@ __global__ void peer_scatter_kernel(const uint32_t* __restrict__ local_words, ui
 #define FAB_CACHED_MINBLOCKS 1        // 512 threads x 128 registers = one CTA per SM; four CTAs of 128 threads fit as well
 #endif
 // Signatures whose public key has a precomputed window table: both scalar multiplications are fixed-base
-// (FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions gathered from HBM-resident tables, no doublings).  Slot < 0 -> bit 0, left to
-// ecdsa_verify_kernel.  qtab: key_slot_capacity tables of FAB_Q_WINDOWS*FAB_Q_ENTRIES affine points.
+// (FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions gathered from HBM-resident tables, no doublings), on the scalars ecdsa_prep_kernel
+// wrote (same n, n_dev, n_base).  Slot < 0 -> bit 0, left to ecdsa_verify_kernel.  qtab: key_slot_capacity tables of
+// FAB_Q_WINDOWS*FAB_Q_ENTRIES affine points.
 __global__ void __launch_bounds__(FAB_CACHED_THREADS, FAB_CACHED_MINBLOCKS)
-ecdsa_verify_cached_kernel(const int32_t* __restrict__ key_slot, const uint8_t* __restrict__ e, const uint8_t* __restrict__ r,
-                           const uint8_t* __restrict__ s, uint32_t n, const aff* __restrict__ gtab, const aff* __restrict__ qtab,
+ecdsa_verify_cached_kernel(const int32_t* __restrict__ key_slot, const uint4* __restrict__ scal, const uint8_t* __restrict__ r,
+                           uint32_t n, const aff* __restrict__ gtab, const aff* __restrict__ qtab,
                            uint32_t* __restrict__ mask, uint32_t* __restrict__ offcurve, const uint32_t* __restrict__ n_dev, uint32_t n_base, PeerOut po)
 {
+    const uint32_t stride = n;
     if (n_dev) n = min(n, n_base + *n_dev);
     const uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t res = V_INVALID;
     if (idx < n) {
         const int32_t slot = key_slot[idx];
         if (slot >= 0) {
-            const size_t o = (size_t)idx * 32;
-            res = ecdsa_verify_one_cached(qtab + (size_t)slot * (FAB_Q_WINDOWS * FAB_Q_ENTRIES), load_be32(e + o), load_be32(r + o),
-                                          load_be32(s + o), gtab);
+            const uint4 a = scal[idx], b = scal[stride + idx], c = scal[2 * (size_t)stride + idx], d = scal[3 * (size_t)stride + idx];
+            const u256 u1 = u256_const(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w), u2 = u256_const(c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w);
+            if (!u256_is_zero(u2))                                  // u2 = 0: r or s outside [1, n-1]
+                res = ecdsa_chain_cached(qtab + (size_t)slot * (FAB_Q_WINDOWS * FAB_Q_ENTRIES), u1, u2, load_be32(r + (size_t)idx * 32), gtab);
         }
     }
     const uint32_t vmask = __ballot_sync(0xffffffffu, res == V_VALID);

@@ -166,20 +166,20 @@ FAB_HD uint32_t ecdsa_verify_one(const u256& qx, const u256& qy, const u256& e, 
     return final_check(acc, r);
 }
 
-// Same verification when the public key has a precomputed window table (fabgpu_keys_register): u2*Q becomes
-// fixed-base too -- FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions in total, no doublings, no per-signature table.  The key was
-// checked to be a curve point when its table was built.
-FAB_HD uint32_t ecdsa_verify_one_cached(const aff* qtab, const u256& e, const u256& r, const u256& s, const aff* gtab)
+// u1 = e*w mod n, u2 = r*w mod n (plain) from w = s^-1 * 2^256 mod n.  For r, s in [1, n-1] u2 is never 0 (n is prime).
+FAB_HD void ecdsa_u1u2(const u256& e, const u256& r, const u256& w, u256& u1, u256& u2)
 {
-    const u256 n = sc_n();
-    if (u256_is_zero(r) || u256_is_zero(s) || !u256_lt(r, n) || !u256_lt(s, n)) return V_INVALID;
-#if FAB_SAFEGCD
-    const u256 w = sc_inv_to_mont_safegcd(s);
-#else
-    const u256 w = sc_inv_to_mont(s);
-#endif
-    const u256 u1 = sc_mul(sc_reduce_once(e), w);
-    const u256 u2 = sc_mul(r, w);
+    u1 = sc_mul(sc_reduce_once(e), w);
+    u2 = sc_mul(r, w);
+}
+
+// The second half of a verification when the public key has a precomputed window table (fabgpu_keys_register): from the
+// scalars u1, u2, R = u1*G + u2*Q with u2*Q fixed-base too -- FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions in total, no
+// doublings, no per-signature table -- and the final check against r.  The key was checked to be a curve point when its table
+// was built.  ecdsa_verify_cached_kernel runs this on the scalars ecdsa_prep_kernel computed; ecdsa_verify_one_cached below is
+// the whole verification for one signature.
+FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& u2, const u256& r, const aff* gtab)
+{
     // One loop over both tables -- 12 windows of u1 in the generator's table, then 16 windows of u2 in the key's table -- so that
     // the kernel holds a single copy of the point addition (expanded in place when FAB_CACHED_INLINE).
     jac acc = jac_infinity();
@@ -230,6 +230,21 @@ FAB_HD uint32_t ecdsa_verify_one_cached(const aff* qtab, const u256& e, const u2
         }
     }
     return final_check(acc, r);
+}
+
+// One signature through a key's window table, scalars included (one inversion of its own).
+FAB_HD uint32_t ecdsa_verify_one_cached(const aff* qtab, const u256& e, const u256& r, const u256& s, const aff* gtab)
+{
+    const u256 n = sc_n();
+    if (u256_is_zero(r) || u256_is_zero(s) || !u256_lt(r, n) || !u256_lt(s, n)) return V_INVALID;
+#if FAB_SAFEGCD
+    const u256 w = sc_inv_to_mont_safegcd(s);
+#else
+    const u256 w = sc_inv_to_mont(s);
+#endif
+    u256 u1, u2;
+    ecdsa_u1u2(e, r, w, u1, u2);
+    return ecdsa_chain_cached(qtab, u1, u2, r, gtab);
 }
 
 // ---- small key tables: the tier between "never seen" and a 64 MiB window table --------------------------------------------------

@@ -43,6 +43,7 @@ struct DevSlot {
     uint32_t* d_off = nullptr;
     int32_t* d_key_slot = nullptr;
     uint32_t* d_idx = nullptr;      // dev_cap + 2 words: compaction scratch of mixed batches
+    uint4* d_scal = nullptr;        // 4 x dev_cap: scalars u1, u2 of the key-table kernel (ecdsa_prep_kernel)
 };
 
 struct Device {
@@ -57,6 +58,11 @@ struct Device {
     aff* s_bases = nullptr; uint8_t* s_keys = nullptr; int32_t* s_slots = nullptr; size_t s_cap = 0;
     cudaStream_t s_stream = nullptr; cudaEvent_t s_ev = nullptr; bool s_ev_set = false;
     DevSlot slot[FABGPU_SLOTS];
+    // Stream-ordered scratch for launches on a caller's stream (fabgpu_verify_p256_device_keyed*), which own no slot: allocated and
+    // freed in the launch's stream order, so concurrent callers on different streams never share a buffer and never wait for
+    // each other.  The pool keeps what it was given (release threshold: no limit) and reuses a block on another stream only when
+    // its free has already completed (no dependencies inserted between streams).
+    cudaMemPool_t scal_pool = nullptr;
     // bitmask exchange over peer memory (fabgpu_peer_mask_*): this rank's receive buffer, the peers' mapped ones
     struct Peer {
         uint32_t* local = nullptr; uint32_t* mapped[FAB_PEER_MAX] = {nullptr}; bool opened[FAB_PEER_MAX] = {false};
@@ -214,7 +220,7 @@ struct fabgpu_ctx {
         int32_t *h_kidx = nullptr, *h_slot_of = nullptr;
         uint8_t *d_sigs = nullptr, *d_digs = nullptr, *d_keys = nullptr, *d_status = nullptr, *d_pre = nullptr, *d_r = nullptr, *d_s = nullptr, *d_e = nullptr,
         *d_qx = nullptr, *d_qy = nullptr; uint32_t *d_sig_off = nullptr, *d_dig_off = nullptr, *d_mask = nullptr, *d_off = nullptr;
-        int32_t *d_kidx = nullptr, *d_slot_of = nullptr, *d_ks = nullptr; uint32_t* d_idx = nullptr;
+        int32_t *d_kidx = nullptr, *d_slot_of = nullptr, *d_ks = nullptr; uint32_t* d_idx = nullptr; uint4* d_scal = nullptr;
         // fabgpu_bccsp_verify_batch_async .. _wait: what is in flight on this slot
         bool busy = false; bool on_device = false; size_t n = 0;
         std::vector<uint8_t> done_status;       // statuses of a batch that could not take the device-gate path (finished at submit time)
@@ -225,7 +231,7 @@ struct fabgpu_ctx {
         size_t tx_cap = 0, j_cap = 0;
         uint32_t* d_env_off = nullptr; bdev::TxDev* d_txs = nullptr; bdev::RawJob* d_raw = nullptr; bdev::ShaJobD* d_sha = nullptr; uint8_t *d_r = nullptr, *d_s = nullptr, *d_qx = nullptr,
         *d_qy = nullptr, *d_gate = nullptr, *d_dig = nullptr, *d_flags = nullptr; int32_t *d_ks = nullptr, *d_ident = nullptr; uint32_t *d_mask = nullptr,
-        *d_off = nullptr, *d_counter = nullptr, *d_idx = nullptr; uint64_t* d_hash = nullptr; bdev::Seg* d_seg = nullptr;
+        *d_off = nullptr, *d_counter = nullptr, *d_idx = nullptr; uint64_t* d_hash = nullptr; bdev::Seg* d_seg = nullptr; uint4* d_scal = nullptr;
         uint8_t* h_flags = nullptr; uint64_t* h_hash = nullptr; bdev::Seg* h_seg = nullptr; uint32_t* h_counter = nullptr; uint32_t* h_env_off = nullptr;
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
         bool busy = false, on_device = false, use_ev = false; size_t T = 0; const uint8_t* block = nullptr;
@@ -321,7 +327,7 @@ enum { CLASS_SMALL = 1, CLASS_GENERIC = 2 };
 int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* key_slot, const uint8_t* qx, const uint8_t* qy,
                   const uint8_t* e, const uint8_t* r, const uint8_t* s, size_t n, uint32_t* mask, uint32_t* off, cudaStream_t st,
                   const uint32_t* n_dev = nullptr, uint32_t n_base = 0, const PeerOut* peer = nullptr, uint32_t* scratch_idx = nullptr,
-                  int classes = CLASS_SMALL | CLASS_GENERIC)
+                  int classes = CLASS_SMALL | CLASS_GENERIC, uint4* scal = nullptr)
 {
     PeerOut po; memset(&po, 0, sizeof po);
     const bool fused_peer = peer && mode == MODE_CACHED && (ctx->cached_kernel == 0 || ctx->cached_kernel == 1 || ctx->cached_kernel == 3) && n > 0 && !n_dev;
@@ -359,11 +365,18 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
             const unsigned blocks = (unsigned)((n + FAB_BA_THREADS - 1) / FAB_BA_THREADS);
             ecdsa_verify_ba_kernel<<<blocks, FAB_BA_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.qtab, mask, off, n_dev, n_base, po);
         } else {
+        // the scalars (ecdsa_prep_kernel), then the chain.  scal: 64 bytes per signature from the caller's slot, or stream-ordered from
+        // the device's pool when the launch has no slot
+        const bool own = scal == nullptr;
+        if (own) CK(ctx, cudaMallocFromPoolAsync((void**)&scal, 64 * n, dv.scal_pool, st));
+        ecdsa_prep_kernel<<<(unsigned)((n + FAB_PREP_THREADS - 1) / FAB_PREP_THREADS), FAB_PREP_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, scal, n_dev, n_base);
+        ctx->launches++;
         unsigned threads = 128;
         const size_t sms = (size_t)dv.sms;
         if (!n_dev && n > sms * 384) threads = (n <= sms * FAB_CACHED_THREADS) ? FAB_CACHED_THREADS : 256;
         const unsigned blocks = (unsigned)((n + threads - 1) / threads);
-        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.qtab, mask, off, n_dev, n_base, po);
+        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, scal, r, (uint32_t)n, dv.gtab, dv.qtab, mask, off, n_dev, n_base, po);
+        if (own) CK(ctx, cudaFreeAsync(scal, st));
         }
         ctx->launches++;
         CK(ctx, cudaGetLastError());
@@ -463,7 +476,7 @@ int enqueue_slot(fabgpu_ctx* ctx, int slot, size_t n, bool keyed)
         if (mode != MODE_GENERIC)
             CK(ctx, cudaMemcpyAsync(ds.d_key_slot, hs.h_key_slot + begin, 4 * cnt, cudaMemcpyHostToDevice, ds.stream));
         int rc = launch_verify(ctx, dv, mode, ds.d_key_slot, ds.d_in[0], ds.d_in[1], ds.d_in[2], ds.d_in[3], ds.d_in[4], cnt, ds.d_mask,
-                               ds.d_off, ds.stream, nullptr, 0, nullptr, ds.d_idx, classes);
+                               ds.d_off, ds.stream, nullptr, 0, nullptr, ds.d_idx, classes, ds.d_scal);
         if (rc) return rc;
         const size_t words = (cnt + 31) / 32;
         CK(ctx, cudaMemcpyAsync(hs.h_mask + begin / 32, ds.d_mask, 4 * words, cudaMemcpyDeviceToHost, ds.stream));
@@ -497,7 +510,7 @@ void free_all(fabgpu_ctx* ctx)
         for (void* p : dev2) if (p) cudaFree(p);
         for (auto& db : ctx->dbs) {
             void* dev4[] = {db.d_env_off, db.d_txs, db.d_raw, db.d_sha, db.d_r, db.d_s, db.d_qx, db.d_qy, db.d_gate, db.d_dig, db.d_flags, db.d_ks, db.d_ident, db.d_mask, db.d_off,
-                            db.d_counter, db.d_hash, db.d_seg, db.d_idx};
+                            db.d_counter, db.d_hash, db.d_seg, db.d_idx, db.d_scal};
             for (void* p : dev4) if (p) cudaFree(p);
             void* host2[] = {db.h_flags, db.h_hash, db.h_seg, db.h_counter, db.h_env_off};
             for (void* p : host2) if (p) cudaFreeHost(p);
@@ -505,7 +518,7 @@ void free_all(fabgpu_ctx* ctx)
         }
         for (auto& gb : ctx->gb) {
         void* dev3[] = {gb.d_sigs, gb.d_digs, gb.d_keys, gb.d_status, gb.d_pre, gb.d_r, gb.d_s, gb.d_e, gb.d_qx, gb.d_qy, gb.d_sig_off, gb.d_dig_off, gb.d_mask, gb.d_off,
-                        gb.d_kidx, gb.d_slot_of, gb.d_ks, gb.d_idx};
+                        gb.d_kidx, gb.d_slot_of, gb.d_ks, gb.d_idx, gb.d_scal};
         for (void* p : dev3) if (p) cudaFree(p);
         void* host3[] = {gb.h_sigs, gb.h_digs, gb.h_keys, gb.h_status, gb.h_sig_off, gb.h_dig_off, gb.h_kidx, gb.h_slot_of};
         for (void* p : host3) if (p) cudaFreeHost(p);
@@ -527,9 +540,11 @@ void free_all(fabgpu_ctx* ctx)
         for (void* q : sm) if (q) cudaFree(q);
         if (dv.s_ev) cudaEventDestroy(dv.s_ev);
         if (dv.s_stream) cudaStreamDestroy(dv.s_stream);
+        if (dv.scal_pool) cudaMemPoolDestroy(dv.scal_pool);      // frees still in flight complete on their own
         for (auto& ds : dv.slot) {
             if (ds.d_key_slot) cudaFree(ds.d_key_slot);
             if (ds.d_idx) cudaFree(ds.d_idx);
+            if (ds.d_scal) cudaFree(ds.d_scal);
             for (auto& p : ds.d_in) if (p) cudaFree(p);
             if (ds.d_mask) cudaFree(ds.d_mask);
             if (ds.d_off) cudaFree(ds.d_off);
@@ -650,6 +665,18 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             CK(ctx, cudaMalloc(&ds.d_off, 4 * words));
             CK(ctx, cudaMalloc(&ds.d_key_slot, 4 * ctx->dev_cap));
             CK(ctx, cudaMalloc(&ds.d_idx, 4 * (ctx->dev_cap + 2)));
+            CK(ctx, cudaMalloc(&ds.d_scal, 64 * ctx->dev_cap));
+        }
+        {
+            cudaMemPoolProps pp; memset(&pp, 0, sizeof pp);
+            pp.allocType = cudaMemAllocationTypePinned;
+            pp.location.type = cudaMemLocationTypeDevice;
+            pp.location.id = dv.id;
+            CK(ctx, cudaMemPoolCreate(&dv.scal_pool, &pp));
+            uint64_t keep = UINT64_MAX;
+            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool, cudaMemPoolAttrReleaseThreshold, &keep));
+            int no = 0;
+            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool, cudaMemPoolReuseAllowInternalDependencies, &no));
         }
 #if FAB_G_TWO_LEVEL
         {
@@ -1195,6 +1222,7 @@ static int gate_bufs_reserve(fabgpu_ctx* ctx, int slot, size_t n, size_t sig_byt
         rc |= grow_dev(ctx, gb.d_status, c); rc |= grow_dev(ctx, gb.d_pre, c); rc |= grow_dev(ctx, gb.d_r, 32 * c); rc |= grow_dev(ctx, gb.d_s, 32 * c);
         rc |= grow_dev(ctx, gb.d_e, 32 * c); rc |= grow_dev(ctx, gb.d_qx, 32 * c); rc |= grow_dev(ctx, gb.d_qy, 32 * c); rc |= grow_dev(ctx, gb.d_ks, 4 * c);
         rc |= grow_dev(ctx, gb.d_mask, c / 8 + 8); rc |= grow_dev(ctx, gb.d_off, c / 8 + 8); rc |= grow_dev(ctx, gb.d_idx, 4 * (c + 2));
+        rc |= grow_dev(ctx, gb.d_scal, 64 * c);
         if (rc) return FABGPU_E_CUDA;
         gb.n_cap = c;
     }
@@ -1270,7 +1298,7 @@ static int bccsp_device_submit(fabgpu_ctx* ctx, int slot, const uint8_t* keys_xy
     ctx->launches++;
     CK(ctx, cudaGetLastError());
     rc = launch_verify(ctx, dv, all_slots ? MODE_CACHED : MODE_MIXED, gb.d_ks, gb.d_qx, gb.d_qy, gb.d_e, gb.d_r, gb.d_s, n, gb.d_mask, gb.d_off, st, nullptr, 0, nullptr,
-                       gb.d_idx, classes ? classes : CLASS_GENERIC);
+                       gb.d_idx, classes ? classes : CLASS_GENERIC, gb.d_scal);
     if (rc) return rc;
     bdev::bccsp_status_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(gb.d_pre, gb.d_mask, gb.d_off, (uint32_t)n, gb.d_status);
     ctx->launches++;
@@ -1958,6 +1986,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
         rc |= grow_dev(ctx, db.d_r, 32 * jc); rc |= grow_dev(ctx, db.d_s, 32 * jc); rc |= grow_dev(ctx, db.d_qx, 32 * jc); rc |= grow_dev(ctx, db.d_qy, 32 * jc);
         rc |= grow_dev(ctx, db.d_gate, jc); rc |= grow_dev(ctx, db.d_ks, 4 * jc); rc |= grow_dev(ctx, db.d_ident, 4 * jc);
         rc |= grow_dev(ctx, db.d_mask, jc / 8 + 8); rc |= grow_dev(ctx, db.d_off, jc / 8 + 8); rc |= grow_dev(ctx, db.d_counter, 16); rc |= grow_dev(ctx, db.d_idx, 4 * (jc + 2));
+        rc |= grow_dev(ctx, db.d_scal, 64 * jc);
         rc |= grow_dev(ctx, db.d_flags, tc); rc |= grow_dev(ctx, db.d_hash, 8 * tc); rc |= grow_dev(ctx, db.d_seg, 8 * tc);
         rc |= grow_host(ctx, db.h_flags, tc); rc |= grow_host(ctx, db.h_hash, 8 * tc); rc |= grow_host(ctx, db.h_seg, 8 * tc);
         rc |= grow_host(ctx, db.h_counter, 16); rc |= grow_host(ctx, db.h_env_off, 8 * (tc + 1));
@@ -2000,7 +2029,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     CK(ctx, cudaGetLastError());
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[3], st));
     int rc = launch_verify(ctx, dv, dm.all_slots ? MODE_CACHED : MODE_MIXED, db.d_ks, db.d_qx, db.d_qy, db.d_dig, db.d_r, db.d_s, J_cap, db.d_mask, db.d_off, st,
-                           db.d_counter, cnt, nullptr, db.d_idx, dm.classes ? dm.classes : CLASS_GENERIC);
+                           db.d_counter, cnt, nullptr, db.d_idx, dm.classes ? dm.classes : CLASS_GENERIC, db.d_scal);
     if (rc) return rc;
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4], st));
     bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block, db.d_txs, cnt, m, pol, db.d_mask, db.d_gate, db.d_ident, db.d_dig, (uint32_t)J_cap, db.d_flags,

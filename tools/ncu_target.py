@@ -1,5 +1,6 @@
 """Small profiling target (development tool): a few launches of each hot kernel on a 64k batch, for
-   ncu --set full -k regex:<kernel> -s <skip> -c 1 python tools/ncu_target.py"""
+   ncu --set full -k regex:<kernel> -s <skip> -c 1 python tools/ncu_target.py
+   Each keyed call below is two kernels: ecdsa_prep_kernel (the scalars), then ecdsa_verify_cached_kernel (the chain)."""
 import importlib, os, sys
 import numpy as np
 import torch
