@@ -24,7 +24,7 @@ EXPORTS = [
     "fabgpu_verify_p256_keyed_async", "fabgpu_verify_p256_device_keyed", "fabgpu_last_timing", "fabgpu_build_info",
     "fabgpu_msp_configure", "fabgpu_validate_block", "fabgpu_validate_envelopes", "fabgpu_block_buffer", "fabgpu_block_timing", "fabgpu_sha256_segments",
     "fabgpu_bccsp_verify_batch_async", "fabgpu_bccsp_verify_batch_wait", "fabgpu_bccsp_batch_buffers", "fabgpu_bccsp_verify_batch_inplace_async",
-    "fabgpu_msp_identity_groups", "fabgpu_namespace_policies",
+    "fabgpu_msp_identity_groups", "fabgpu_namespace_policies", "fabgpu_msp_principal_bits",
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
@@ -111,6 +111,20 @@ def identity_groups(identities):
             pass
         groups[i] = keys.setdefault(k, len(keys))
     return groups
+
+
+def pack_principal_bits(bits):
+    """bool [n_ids, n_principals] -> uint32 [n_ids, ceil(n_principals / 32)], the layout fabgpu_msp_principal_bits reads: bit p % 32
+    of word p // 32 of row i is bits[i, p]."""
+    b = np.asarray(bits, dtype=bool)
+    if b.ndim != 2:
+        raise ValueError("principal bits must be a 2-D [n_ids, n_principals] array")
+    n_ids, n_pr = b.shape
+    W = (n_pr + 31) // 32
+    padded = np.zeros((n_ids, 32 * W), np.uint64)
+    padded[:, :n_pr] = b
+    words = (padded.reshape(n_ids, W, 32) << np.arange(32, dtype=np.uint64)).sum(axis=2)
+    return words.astype(np.uint32)
 
 
 def build_info():
@@ -387,6 +401,15 @@ class Context:
         nb, no = blob([n.encode() for n in names])
         roots = np.array([policies[n] for n in names] or [0], np.int32)
         self._ck(lib().fabgpu_namespace_policies(self._h, _p(nb), _p(no), _p(roots), ctypes.c_int(len(names))))
+
+    def msp_principal_bits(self, bits):
+        """bits: bool [n_ids, n_principals], bits[i, p] = identity i satisfies principal p (msp Identity.SatisfiesPrincipal), for the
+        identities and principals of the last msp_configure, in that order.  SignedBy(p) then matches by these bits instead of by
+        MSP id.  None, or no rows, removes them."""
+        b = np.zeros((0, 0), bool) if bits is None else np.asarray(bits, dtype=bool)
+        words = np.ascontiguousarray(pack_principal_bits(b)).reshape(-1)
+        words = words if words.size else np.zeros(1, np.uint32)
+        self._ck(lib().fabgpu_msp_principal_bits(self._h, _p(words), ctypes.c_int(b.shape[0]), ctypes.c_int(b.shape[1])))
 
     def block_buffer(self, nbytes, slot=0):
         """Pinned staging buffer (numpy view) for block bytes; one per slot."""

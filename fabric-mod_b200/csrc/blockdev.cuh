@@ -540,12 +540,17 @@ BD_HD void resolve_job(const uint8_t* base, uint32_t j, const RawJob* raw, const
 
 // ---- policy evaluator: cauthdsl.go:24-92, `used` as a bit mask over at most BD_MAX_SIGNERS signers ------------------------
 // Several policies share one node array (one tree per chaincode namespace); ns_* name the root of each.
+// Node types: 0 = NOutOf(n), 1 = SignedBy(principal n), 2 = ImplicitMeta with threshold n (implicitmeta.go:69-103).
+// principal_bits (fabgpu_msp_principal_bits): bits_words words per identity, bit p set = identity.SatisfiesPrincipal(p) == nil.
+// Null: principals are MSP ids matched as ROLE MEMBER (msp_code equality of a valid identity).
 struct PolicyDev {
     const int32_t* nodes; int32_t n_nodes; const int32_t* principal_code; int32_t n_principals;
     const uint8_t* ns_blob; const uint32_t* ns_off; const int32_t* ns_root; int32_t n_ns;     // n_ns = 0: one policy (root 0) for every namespace
+    const uint32_t* principal_bits = nullptr; int32_t bits_words = 0;          // a PolicyDev built field by field has no bits
 };
 
-BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer_code, int n_signers, uint64_t& used, int depth)
+// signer[i]: with principal bits, the identity index of verified signer i; without, its MSP-id code, -1 when Validate() failed.
+BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer, int n_signers, uint64_t& used, int depth)
 {
     if (idx < 0 || idx >= pol.n_nodes || depth > BD_MAX_POLICY_DEPTH) return false;
     const int32_t type = pol.nodes[4 * idx], n = pol.nodes[4 * idx + 1], first = pol.nodes[4 * idx + 2], cnt = pol.nodes[4 * idx + 3];
@@ -553,15 +558,35 @@ BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer_code
         int verified = 0;
         for (int c = first; c < first + cnt; c++) {
             uint64_t scratch = used;
-            if (eval_policy(pol, c, signer_code, n_signers, scratch, depth + 1)) { verified++; used = scratch; }
+            if (eval_policy(pol, c, signer, n_signers, scratch, depth + 1)) { verified++; used = scratch; }
         }
         return verified >= n;
     }
-    if (n < 0 || n >= pol.n_principals) return false;
+    if (type == 2) {
+        // Every sub-policy is a policy of its own (its own SignatureSetToValidIdentities and cauthdsl `used`): one signer may satisfy
+        // several of them, and the caller's `used` is not touched.
+        int satisfied = 0;
+        for (int c = first; c < first + cnt && satisfied < n; c++) {
+            uint64_t fresh = 0;
+            if (eval_policy(pol, c, signer, n_signers, fresh, depth + 1)) satisfied++;
+        }
+        return satisfied >= n;
+    }
+    if (type != 1 || n < 0 || n >= pol.n_principals) return false;
+    if (pol.principal_bits) {
+        const uint32_t word = (uint32_t)n >> 5, bit = 1u << (n & 31);
+        for (int i = 0; i < n_signers; i++) {
+            if (used & (1ull << i)) continue;
+            if (!(pol.principal_bits[(size_t)signer[i] * pol.bits_words + word] & bit)) continue;
+            used |= 1ull << i;
+            return true;
+        }
+        return false;
+    }
     const int32_t want = pol.principal_code[n];
     for (int i = 0; i < n_signers; i++) {
         if (used & (1ull << i)) continue;
-        if (signer_code[i] < 0 || signer_code[i] != want) continue;
+        if (signer[i] < 0 || signer[i] != want) continue;
         used |= 1ull << i;
         return true;
     }
@@ -619,7 +644,10 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
     }
     // SignatureSetToValidIdentities (policy.go:365-402): in order; de-duplicated by Mspid + Id against the identities that already
     // VERIFIED; a failed signature drops that entry only.  One set per transaction, shared by every namespace's evaluation.
-    int32_t signer_code[BD_MAX_SIGNERS]; int n_signers = 0;
+    // With principal bits a signer is its identity index: the caller's SatisfiesPrincipal answers already include Validate() where
+    // the reference checks it (an admin-listed identity satisfies ADMIN without it, mspimpl.go:506-513).  Without, it is its MSP-id
+    // code, -1 when Validate() failed (ROLE MEMBER, mspimpl.go:501-505).
+    int32_t signer[BD_MAX_SIGNERS]; int n_signers = 0;
     for (uint32_t i = 0; i < tx.n_end_jobs; i++) {
         const uint32_t j = tx.first_end_job + i;
         const int32_t idn = job_identity[j];
@@ -634,11 +662,11 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
         if (dup) continue;
         if (!sig_ok(j)) continue;
         if (n_signers >= BD_MAX_SIGNERS) return TXC_NOT_VALIDATED;
-        signer_code[n_signers++] = msp.valid[idn] ? msp.msp_code[idn] : -1;
+        signer[n_signers++] = pol.principal_bits ? idn : msp.valid[idn] ? msp.msp_code[idn] : -1;
     }
     for (int i = 0; i < tx.n_ns; i++) {
         uint64_t used = 0;
-        if (!eval_policy(pol, roots[i], signer_code, n_signers, used, 0)) return TXC_ENDORSEMENT_POLICY_FAILURE;
+        if (!eval_policy(pol, roots[i], signer, n_signers, used, 0)) return TXC_ENDORSEMENT_POLICY_FAILURE;
     }
     uint64_t hsh = 1469598103934665603ull;
     for (uint32_t k = 0; k < tx.txid_ascii.len; k++) hsh = (hsh ^ base[tx.txid_ascii.off + k]) * 1099511628211ull;

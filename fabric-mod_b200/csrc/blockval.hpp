@@ -29,7 +29,7 @@ struct MspTable {
     void add(const uint8_t* p, size_t n) { serialized.emplace_back((const char*)p, n); }
 };
 
-struct PolicyNode { int32_t type, n, first_child, n_children; };   // type 0: NOutOf(n) over children; 1: SignedBy(principal n)
+struct PolicyNode { int32_t type, n, first_child, n_children; };   // type 0: NOutOf(n) over children; 1: SignedBy(principal n); 2: ImplicitMeta(threshold n)
 
 // Block{header = 1, data = 2, metadata = 3}, BlockData{repeated bytes data = 1} -> the envelopes' byte ranges.  false when the outer
 // messages do not parse (Go: proto.Unmarshal of the Block fails).

@@ -413,7 +413,9 @@ ecdsa_verify_lanes_kernel(const int32_t* __restrict__ key_slot, const uint8_t* _
     for (int k = 0; k < 32 / LANES; k++) packed |= ((b >> (k * LANES)) & 1u) << k;
     if ((threadIdx.x & 31u) == 0) {
         const uint32_t first = blockIdx.x * SIGS + (threadIdx.x / LANES);     // first signature of this warp
-        if (first < n) {
+        // Every warp whose slice lies in a mask word of the batch writes it, also when all its signatures are past n: a warp covers
+        // only 32 / LANES signatures, and the rest of the batch's last word would otherwise keep whatever the buffer held.
+        if ((first >> 5) <= ((n - 1) >> 5)) {
             if (LANES == 2) { reinterpret_cast<uint16_t*>(mask)[first >> 4] = (uint16_t)packed; if (offcurve) reinterpret_cast<uint16_t*>(offcurve)[first >> 4] = 0; }
             else if (LANES == 4) { reinterpret_cast<uint8_t*>(mask)[first >> 3] = (uint8_t)packed; if (offcurve) reinterpret_cast<uint8_t*>(offcurve)[first >> 3] = 0; }
             else { mask[first >> 5] = packed; if (offcurve) offcurve[first >> 5] = 0; }

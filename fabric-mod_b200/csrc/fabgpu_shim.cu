@@ -211,6 +211,7 @@ struct fabgpu_ctx {
         uint32_t* id_off = nullptr; int32_t *key_slot = nullptr, *msp_code = nullptr, *ht_idx = nullptr, *nodes = nullptr, *principal_code = nullptr;
         int32_t* group = nullptr;                                     // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
         uint8_t* ns_blob = nullptr; uint32_t* ns_off = nullptr; int32_t* ns_root = nullptr; int32_t n_ns = 0;    // fabgpu_namespace_policies
+        uint32_t* pbits = nullptr; int32_t pbits_words = 0;           // fabgpu_msp_principal_bits, null = MSP-id member matching
         uint64_t* ht_hash = nullptr; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
         bool all_slots = true; int classes = 0;                    // which non-big classes the identities' keys fall in (CLASS_*)
     } dm;
@@ -506,7 +507,7 @@ void free_all(fabgpu_ctx* ctx)
         }
         auto& dm = ctx->dm;
         void* dev2[] = {dm.id_blob, dm.valid, dm.keys_xy, dm.channel, dm.id_off, dm.key_slot, dm.msp_code, dm.ht_idx, dm.nodes, dm.principal_code, dm.ht_hash,
-                        dm.group, dm.ns_blob, dm.ns_off, dm.ns_root};
+                        dm.group, dm.ns_blob, dm.ns_off, dm.ns_root, dm.pbits};
         for (void* p : dev2) if (p) cudaFree(p);
         for (auto& db : ctx->dbs) {
             void* dev4[] = {db.d_env_off, db.d_txs, db.d_raw, db.d_sha, db.d_r, db.d_s, db.d_qx, db.d_qy, db.d_gate, db.d_dig, db.d_flags, db.d_ks, db.d_ident, db.d_mask, db.d_off,
@@ -1700,7 +1701,7 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
     // blocks already enqueued on a slot were launched with the OLD tables (passed by value): let them finish before those go away
     for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream));
     void* old[] = {dm.id_blob, dm.valid, dm.keys_xy, dm.channel, dm.id_off, dm.key_slot, dm.msp_code, dm.ht_idx, dm.nodes, dm.principal_code, dm.ht_hash,
-                   dm.group, dm.ns_blob, dm.ns_off, dm.ns_root};
+                   dm.group, dm.ns_blob, dm.ns_off, dm.ns_root, dm.pbits};
     for (void* p : old) if (p) cudaFree(p);
     dm = fabgpu_ctx::DevMsp();
     // MSP-id codes: equal strings <=> equal codes, shared between identities and policy principals
@@ -1777,7 +1778,7 @@ static int policy_height(const std::vector<blockval::PolicyNode>& nodes, int i, 
     if (path > BD_MAX_POLICY_DEPTH) return -1;
     if (height[i] >= 0) return height[i];
     int h = 0;
-    if (nodes[i].type == 0)
+    if (nodes[i].type == 0 || nodes[i].type == 2)
         for (int c = nodes[i].first_child; c < nodes[i].first_child + nodes[i].n_children; c++) {
             const int hc = policy_height(nodes, c, path + 1, height);
             if (hc < 0 || hc + 1 > BD_MAX_POLICY_DEPTH) return -1;
@@ -1786,17 +1787,27 @@ static int policy_height(const std::vector<blockval::PolicyNode>& nodes, int i, 
     return height[i] = h;
 }
 
-// What eval_policy can evaluate exactly: children inside the array, SignedBy indices inside the principals, and from every node a
-// tree at most BD_MAX_POLICY_DEPTH deep without cycles.  Past that depth the device would report ENDORSEMENT_POLICY_FAILURE where
-// the reference, which has no depth limit, may accept: such a policy is refused, and the caller validates on the CPU.
+// What eval_policy can evaluate exactly: node types 0 (NOutOf), 1 (SignedBy) and 2 (ImplicitMeta), children inside the array,
+// SignedBy indices inside the principals, and from every node a tree at most BD_MAX_POLICY_DEPTH deep without cycles.  Past that
+// depth the device would report ENDORSEMENT_POLICY_FAILURE where the reference, which has no depth limit, may accept: such a
+// policy is refused, and the caller validates on the CPU.  ImplicitMeta nodes must be what NewImplicitMetaPolicy builds
+// (implicitmeta.go:44-58): a threshold in [1, n_children], or 0 over no children; and never a child of an NOutOf node, since a
+// signature policy compiles only NOutOf and SignedBy (cauthdsl.go:24-92).
 static const char* check_policy(const std::vector<blockval::PolicyNode>& nodes, int n_principals)
 {
     const int64_t n_nodes = (int64_t)nodes.size();
     for (const auto& nd : nodes) {
-        if (nd.type == 0 && (nd.first_child < 0 || nd.n_children < 0 || (int64_t)nd.first_child + nd.n_children > n_nodes))
+        if (nd.type < 0 || nd.type > 2) return "policy node type is not NOutOf (0), SignedBy (1) or ImplicitMeta (2)";
+        if (nd.type != 1 && (nd.first_child < 0 || nd.n_children < 0 || (int64_t)nd.first_child + nd.n_children > n_nodes))
             return "policy node children out of range";
-        if (nd.type != 0 && (nd.n < 0 || nd.n >= n_principals)) return "SignedBy principal index out of range";
+        if (nd.type == 1 && (nd.n < 0 || nd.n >= n_principals)) return "SignedBy principal index out of range";
+        if (nd.type == 2 && !(nd.n >= 1 ? nd.n <= nd.n_children : nd.n == 0 && nd.n_children == 0))
+            return "ImplicitMeta threshold outside [1, n_children] (or 0 with no children)";
     }
+    for (const auto& nd : nodes)
+        if (nd.type == 0)
+            for (int c = nd.first_child; c < nd.first_child + nd.n_children; c++)
+                if (nodes[c].type == 2) return "ImplicitMeta node below an NOutOf node";
     std::vector<int> height(nodes.size(), -1);
     for (int i = 0; i < (int)n_nodes; i++)
         if (policy_height(nodes, i, 0, height) < 0) return "policy tree deeper than the device evaluates, or cyclic";
@@ -1866,6 +1877,27 @@ int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids)
     if (n_ids == 0) return FABGPU_OK;
     CK(ctx, cudaMalloc(&dm.group, 4 * (size_t)n_ids));
     CK(ctx, cudaMemcpy(dm.group, group, 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
+    return FABGPU_OK;
+}
+
+int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, int n_principals)
+{
+    if (!ctx || n_ids < 0 || n_principals < 0 || (n_ids && !bits)) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm;
+    if (n_ids && (n_ids != dm.n_ids || n_principals != dm.n_principals)) {
+        ctx->last_error = "principal bits do not match the identities and principals given to fabgpu_msp_configure";
+        return FABGPU_E_ARG;
+    }
+    int rc = drain_block_streams(ctx); if (rc) return rc;
+    if (dm.pbits) { cudaFree(dm.pbits); dm.pbits = nullptr; }
+    dm.pbits_words = 0;
+    if (n_ids == 0) return FABGPU_OK;
+    const int W = (n_principals + 31) / 32;
+    const size_t bytes = 4 * (size_t)n_ids * W;
+    CK(ctx, cudaMalloc(&dm.pbits, bytes + 8));                 // non-null even with no principals: it selects the bit test
+    if (bytes) CK(ctx, cudaMemcpy(dm.pbits, bits, bytes, cudaMemcpyHostToDevice));
+    dm.pbits_words = W;
     return FABGPU_OK;
 }
 
@@ -2005,6 +2037,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     m.keys_xy = dm.keys_xy; m.ht_hash = dm.ht_hash; m.ht_idx = dm.ht_idx; m.ht_size = dm.ht_size; m.n_ids = dm.n_ids;
     bdev::PolicyDev pol; pol.nodes = dm.nodes; pol.n_nodes = dm.n_nodes; pol.principal_code = dm.principal_code; pol.n_principals = dm.n_principals;
     pol.ns_blob = dm.ns_blob; pol.ns_off = dm.ns_off; pol.ns_root = dm.ns_root; pol.n_ns = dm.n_ns;
+    pol.principal_bits = dm.pbits; pol.bits_words = dm.pbits_words;
     const bool need_q = (dm.classes & CLASS_GENERIC) != 0;   // only the generic arithmetic reads the key itself
     bdev::JobArrays ja; ja.sha = db.d_sha; ja.r = db.d_r; ja.s = db.d_s; ja.key_slot = db.d_ks; ja.identity = db.d_ident; ja.qx = need_q ? db.d_qx : nullptr;
     ja.qy = need_q ? db.d_qy : nullptr; ja.gate_ok = db.d_gate; ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T;

@@ -216,18 +216,25 @@ int fabgpu_gate_signature(const uint8_t* sig, size_t sig_len, uint8_t r_out[32],
  * identities: n_ids serialized msp.SerializedIdentity byte strings (id_blob + (n_ids+1) offsets) exactly as they appear in
  * SignatureHeader.creator / Endorsement.endorser, their MSP ids, P-256 keys (X||Y) and the outcome of identity.Validate().
  * policy_nodes: n_nodes x 4 int32 (type, n, first_child, n_children); type 0 = NOutOf(n) over children
- * [first_child, first_child + n_children), type 1 = SignedBy(principal n); node 0 is the root.  Principals are MSP ids
- * (ROLE member).  Every identity's key gets a window table when the MSP fits the window-table pool (n_ids <= fabgpu_key_slot_capacity);
+ * [first_child, first_child + n_children), type 1 = SignedBy(principal n), type 2 = ImplicitMeta with threshold n over the
+ * children (common/policies/implicitmeta.go:44-103: satisfied iff at least n children are, each child evaluated as a policy of
+ * its own, so one signer may satisfy several); node 0 is the root.  Principals are named by strings.  By default a principal
+ * is an MSP id matched as ROLE MEMBER: a signer satisfies it iff its MSP id is that string and its Validate() passed.
+ * fabgpu_msp_principal_bits replaces that match by the caller's own SatisfiesPrincipal answers (roles, identities, OUs).
+ * Every identity's key gets a window table when the MSP fits the window-table pool (n_ids <= fabgpu_key_slot_capacity);
  * a larger MSP -- thousands of client certificates -- goes to the small tier instead, except the identities whose key already owns a
  * window table: register the few busy keys (the endorsing peers) with fabgpu_keys_register BEFORE this call and they keep it.
- * FABGPU_E_ARG, with nothing installed, for a policy array the device cannot evaluate exactly: children outside the array, a
- * SignedBy index outside the principals, a cycle, or a tree deeper than 12 levels below any node (BD_MAX_POLICY_DEPTH).
- * The caller then validates that channel's blocks on the CPU. */
+ * FABGPU_E_ARG, with nothing installed, for a policy array the device cannot evaluate exactly: a node type other than 0, 1
+ * or 2, children outside the array, a SignedBy index outside the principals, an ImplicitMeta node below an NOutOf node or
+ * with a threshold outside [1, n_children] (0 is accepted only with no children), a cycle, or a tree deeper than 12 levels
+ * below any node (BD_MAX_POLICY_DEPTH; ImplicitMeta nodes count as levels).  The caller then validates that channel's blocks
+ * on the CPU. */
 int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* mspid_blob,
                          const uint32_t* mspid_off, const uint8_t* keys_xy, const uint8_t* valid, int n_ids,
                          const int32_t* policy_nodes, int n_nodes, const uint8_t* principal_blob, const uint32_t* principal_off,
                          int n_principals, const char* channel_id);
-/* Two optional refinements of the table fabgpu_msp_configure installed (call them after it; each drains the block slots first):
+/* Optional refinements of the table fabgpu_msp_configure installed (call them after it; each drains the block slots first;
+ * fabgpu_msp_configure clears all three):
  *   _identity_groups: group[i] = de-duplication id of identity i.  The reference de-duplicates a transaction's signers on
  *       Mspid + certificate digest (common/policies/policy.go:380-386), so two byte-different serializations of ONE certificate
  *       must share a group; without this call every table entry is its own group.
@@ -235,8 +242,17 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
  *       transaction writes to, core/committer/txvalidator/v20/plugindispatcher/dispatcher.go:166-221,265-277): ns_root[i] is the
  *       root node -- an index into the node array given to fabgpu_msp_configure, which may hold several trees -- of namespace i's
  *       policy.  n_ns = 0 restores "node 0 is the policy of every namespace".  A transaction that needs a namespace without an
- *       entry is flagged 254 (NOT_VALIDATED): the CPU validator reads the chaincode definition from the ledger. */
+ *       entry is flagged 254 (NOT_VALIDATED): the CPU validator reads the chaincode definition from the ledger.
+ *   _principal_bits: which identity satisfies which principal, W = ceil(n_principals / 32) words per identity: bit p % 32 of
+ *       bits[i * W + p / 32] set iff identity i satisfies principal p -- the caller's msp Identity.SatisfiesPrincipal(principal)
+ *       == nil, so MSP version, NodeOUs, admin lists, IDENTITY and ORGANIZATION_UNIT principals are answered where the
+ *       reference answers them (msp/mspimpl.go); the device never parses certificates.  While bits are installed, SignedBy(p)
+ *       matches a verified, de-duplicated signer iff its bit p is set, whatever its Validate() outcome (an admin-listed
+ *       identity satisfies ADMIN without it, mspimpl.go:506-513); the creator's Validate() is still checked.  n_ids and
+ *       n_principals must equal fabgpu_msp_configure's, else FABGPU_E_ARG and nothing changes; n_ids = 0 removes the bits
+ *       and restores MSP-id member matching. */
 int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids);
+int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, int n_principals);
 int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const int32_t* ns_root, int n_ns);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
