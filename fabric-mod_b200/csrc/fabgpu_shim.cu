@@ -22,6 +22,7 @@
 #include "../../include/fabgpu_ecdsa.h"
 #include "bccsp_host.hpp"
 #include "blockval.hpp"
+#include "cuda_owned.hpp"
 #include "sha256.cuh"
 #include "blockdev_kernels.cuh"
 #include "ecdsa_kernels.cuh"
@@ -37,45 +38,50 @@ namespace {
 std::string g_init_error = "";
 
 struct DevSlot {
-    cudaStream_t stream = nullptr;
-    uint8_t* d_in[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // qx qy e r s
-    uint32_t* d_mask = nullptr;
-    uint32_t* d_off = nullptr;
-    int32_t* d_key_slot = nullptr;
-    uint32_t* d_idx = nullptr;      // dev_cap + 2 words: compaction scratch of mixed batches
-    uint4* d_scal = nullptr;        // 4 x dev_cap: scalars u1, u2 of the key-table kernel (ecdsa_prep_kernel)
+    Stream stream;
+    DevArray<uint8_t> d_in[5];      // qx qy e r s
+    DevArray<uint32_t> d_mask;
+    DevArray<uint32_t> d_off;
+    DevArray<int32_t> d_key_slot;
+    DevArray<uint32_t> d_idx;       // dev_cap + 2 words: compaction scratch of mixed batches
+    DevArray<uint4> d_scal;         // 4 x dev_cap: scalars u1, u2 of the key-table kernel (ecdsa_prep_kernel)
 };
 
+// Members go in reverse order of declaration, with this device current (~Device).
 struct Device {
     int id = 0;
-    aff* gtab = nullptr;
+    DevArray<aff> gtab;
     int sms = 132;            // multiprocessors (launch shapes; read from the device at fabgpu_init)
-    aff* qtab = nullptr;      // key_slots tables of FAB_G_WINDOWS * FAB_G_ENTRIES points (per-key fixed-base tables)
+    DevArray<aff> qtab;       // key_slots tables of FAB_G_WINDOWS * FAB_G_ENTRIES points (per-key fixed-base tables)
     // small key tables (FAB_S_POINTS points each): the pool, the build scratch (grown on demand) and the build stream.  Every
     // enqueue that may read a small table first makes its stream wait for s_ev (the last build): builds are ordered among
-    // themselves by s_stream, so one event covers all earlier ones.
-    aff* stab = nullptr;
-    aff* s_bases = nullptr; uint8_t* s_keys = nullptr; int32_t* s_slots = nullptr; size_t s_cap = 0;
-    cudaStream_t s_stream = nullptr; cudaEvent_t s_ev = nullptr; bool s_ev_set = false;
+    // themselves by s_stream, so one event covers all earlier ones.  The scratch holds s_cap() keys; s_bases is grown last.
+    DevArray<aff> stab;
+    DevArray<uint8_t> s_keys; DevArray<int32_t> s_slots; DevArray<aff> s_bases;
+    size_t s_cap() const { return s_bases.bytes() / (FAB_S_WINDOWS * sizeof(aff)); }
+    Stream s_stream; Event s_ev; bool s_ev_set = false;
     DevSlot slot[FABGPU_SLOTS];
     // Stream-ordered scratch for launches on a caller's stream (fabgpu_verify_p256_device_keyed*), which own no slot: allocated and
     // freed in the launch's stream order, so concurrent callers on different streams never share a buffer and never wait for
     // each other.  The pool keeps what it was given (release threshold: no limit) and reuses a block on another stream only when
     // its free has already completed (no dependencies inserted between streams).
-    cudaMemPool_t scal_pool = nullptr;
-    // bitmask exchange over peer memory (fabgpu_peer_mask_*): this rank's receive buffer, the peers' mapped ones
+    MemPool scal_pool;
+    // bitmask exchange over peer memory (fabgpu_peer_mask_*): this rank's receive buffer, the peers' mapped ones (none for this rank:
+    // its segment is `local`).  `mapped` comes last so that the mappings are closed before `local` is freed.
     struct Peer {
-        uint32_t* local = nullptr; uint32_t* mapped[FAB_PEER_MAX] = {nullptr}; bool opened[FAB_PEER_MAX] = {false};
-        uint32_t* done = nullptr; uint32_t* timeout = nullptr; uint32_t* h_timeout = nullptr;
+        DevArray<uint32_t> local; DevArray<uint32_t> done; uint32_t* timeout = nullptr; HostArray<uint32_t> h_timeout;
         int world = 0, rank = 0; size_t words_per_rank = 0; bool ready = false;
+        IpcMapping<uint32_t> mapped[FAB_PEER_MAX];
+        uint32_t* buf(int p) const { return p == rank ? local.get() : mapped[p].get(); }
     } peer;
+    ~Device() { cudaSetDevice(id); }
 };
 
 struct HostSlot {
-    uint8_t* h_in[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    uint32_t* h_mask = nullptr;
-    uint32_t* h_off = nullptr;
-    int32_t* h_key_slot = nullptr;
+    HostArray<uint8_t> h_in[5];
+    HostArray<uint32_t> h_mask;
+    HostArray<uint32_t> h_off;
+    HostArray<int32_t> h_key_slot;
 };
 
 }  // namespace
@@ -193,35 +199,30 @@ struct fabgpu_ctx {
     std::string channel;
     std::vector<int32_t> identity_slot;
     struct BlockBufs {
-        uint8_t* d_block = nullptr; size_t block_cap = 0;
-        uint8_t* h_block = nullptr; size_t h_block_cap = 0;       // optional pinned staging the caller may fill directly
-        size_t job_cap = 0;                                       // signature jobs
-        size_t sha_cap = 0;                                       // all digests (signature jobs + 2 per transaction)
-        ShaJob* d_sha = nullptr; ShaJob* h_sha = nullptr;
-        uint8_t* d_dig = nullptr; uint8_t* h_dig = nullptr;       // h_dig: check digests only
-        uint8_t *d_r = nullptr, *d_s = nullptr, *d_qx = nullptr, *d_qy = nullptr;
-        uint8_t *h_r = nullptr, *h_s = nullptr, *h_qx = nullptr, *h_qy = nullptr;
-        int32_t *d_ks = nullptr, *h_ks = nullptr;
-        uint32_t *d_mask = nullptr, *d_off = nullptr, *h_mask = nullptr;
-    } bbs[FABGPU_SLOTS];          // [0] also serves the host-thread path (FABGPU_BLOCK_HOST=1)
+        DevArray<uint8_t> d_block;
+        HostArray<uint8_t> h_block;                               // optional pinned staging the caller may fill directly
+    } bbs[FABGPU_SLOTS];
     double block_timing[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // host phases [0..4] (see fabgpu_block_timing), device stages [5..9]
     // device-side copy of the MSP view / policy (block_plan_kernel, block_decide_kernel)
     struct DevMsp {
-        uint8_t *id_blob = nullptr, *valid = nullptr, *keys_xy = nullptr, *channel = nullptr;
-        uint32_t* id_off = nullptr; int32_t *key_slot = nullptr, *msp_code = nullptr, *ht_idx = nullptr, *nodes = nullptr, *principal_code = nullptr;
-        int32_t* group = nullptr;                                     // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
-        uint8_t* ns_blob = nullptr; uint32_t* ns_off = nullptr; int32_t* ns_root = nullptr; int32_t n_ns = 0;    // fabgpu_namespace_policies
-        uint32_t* pbits = nullptr; int32_t pbits_words = 0;           // fabgpu_msp_principal_bits, null = MSP-id member matching
-        uint64_t* ht_hash = nullptr; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
+        DevArray<uint8_t> id_blob, valid, keys_xy, channel;
+        DevArray<uint32_t> id_off; DevArray<int32_t> key_slot, msp_code, ht_idx, nodes, principal_code;
+        DevArray<int32_t> group;                                      // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
+        DevArray<uint8_t> ns_blob; DevArray<uint32_t> ns_off; DevArray<int32_t> ns_root; int32_t n_ns = 0;    // fabgpu_namespace_policies
+        DevArray<uint32_t> pbits; int32_t pbits_words = 0;            // fabgpu_msp_principal_bits, null = MSP-id member matching
+        DevArray<uint64_t> ht_hash; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
         bool all_slots = true; int classes = 0;                    // which non-big classes the identities' keys fall in (CLASS_*)
     } dm;
     struct GateBufs {                          // fabgpu_bccsp_verify_batch with device-side gates
-        size_t n_cap = 0, sig_cap = 0, dig_cap = 0, k_cap = 0;
-        uint8_t *h_sigs = nullptr, *h_digs = nullptr, *h_keys = nullptr, *h_status = nullptr; uint32_t *h_sig_off = nullptr, *h_dig_off = nullptr;
-        int32_t *h_kidx = nullptr, *h_slot_of = nullptr;
-        uint8_t *d_sigs = nullptr, *d_digs = nullptr, *d_keys = nullptr, *d_status = nullptr, *d_pre = nullptr, *d_r = nullptr, *d_s = nullptr, *d_e = nullptr,
-        *d_qx = nullptr, *d_qy = nullptr; uint32_t *d_sig_off = nullptr, *d_dig_off = nullptr, *d_mask = nullptr, *d_off = nullptr;
-        int32_t *d_kidx = nullptr, *d_slot_of = nullptr, *d_ks = nullptr; uint32_t* d_idx = nullptr; uint4* d_scal = nullptr;
+        // Four groups, each grown together (gate_bufs_reserve).  A group's capacity is read from the array it grows last: signatures
+        // (n_cap), signature and digest bytes, keys.
+        HostArray<uint8_t> h_sigs, h_digs, h_keys, h_status; HostArray<uint32_t> h_sig_off, h_dig_off; HostArray<int32_t> h_kidx, h_slot_of;
+        DevArray<uint8_t> d_sigs, d_digs, d_keys, d_status, d_pre, d_r, d_s, d_e, d_qx, d_qy; DevArray<uint32_t> d_sig_off, d_dig_off, d_mask, d_off;
+        DevArray<int32_t> d_kidx, d_slot_of, d_ks; DevArray<uint32_t> d_idx; DevArray<uint4> d_scal;
+        size_t n_cap() const { return d_scal.bytes() / 64; }
+        size_t sig_cap() const { return d_sigs.bytes(); }
+        size_t dig_cap() const { return d_digs.bytes(); }
+        size_t k_cap() const { return d_slot_of.bytes() / 4; }
         // fabgpu_bccsp_verify_batch_async .. _wait: what is in flight on this slot
         bool busy = false; bool on_device = false; size_t n = 0;
         std::vector<uint8_t> done_status;       // statuses of a batch that could not take the device-gate path (finished at submit time)
@@ -229,19 +230,21 @@ struct fabgpu_ctx {
     } gb[FABGPU_SLOTS];
     std::mutex gb_mu[FABGPU_SLOTS];
     struct DevBlock {
-        size_t tx_cap = 0, j_cap = 0;
-        uint32_t* d_env_off = nullptr; bdev::TxDev* d_txs = nullptr; bdev::RawJob* d_raw = nullptr; bdev::ShaJobD* d_sha = nullptr; uint8_t *d_r = nullptr, *d_s = nullptr, *d_qx = nullptr,
-        *d_qy = nullptr, *d_gate = nullptr, *d_dig = nullptr, *d_flags = nullptr; int32_t *d_ks = nullptr, *d_ident = nullptr; uint32_t *d_mask = nullptr,
-        *d_off = nullptr, *d_counter = nullptr, *d_idx = nullptr; uint64_t* d_hash = nullptr; bdev::Seg* d_seg = nullptr; uint4* d_scal = nullptr;
-        uint8_t* h_flags = nullptr; uint64_t* h_hash = nullptr; bdev::Seg* h_seg = nullptr; uint32_t* h_counter = nullptr; uint32_t* h_env_off = nullptr;
+        // grown together in block_submit; the capacity in transactions is read from h_flags, which is grown last
+        DevArray<uint32_t> d_env_off; DevArray<bdev::TxDev> d_txs; DevArray<bdev::RawJob> d_raw; DevArray<bdev::ShaJobD> d_sha; DevArray<uint8_t> d_r, d_s, d_qx,
+        d_qy, d_gate, d_dig, d_flags; DevArray<int32_t> d_ks, d_ident; DevArray<uint32_t> d_mask, d_off, d_counter, d_idx; DevArray<uint64_t> d_hash;
+        DevArray<bdev::Seg> d_seg; DevArray<uint4> d_scal;
+        HostArray<uint64_t> h_hash; HostArray<bdev::Seg> h_seg; HostArray<uint32_t> h_counter, h_env_off; HostArray<uint8_t> h_flags;
+        size_t tx_cap() const { return h_flags.bytes(); }
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
         bool busy = false, on_device = false, use_ev = false; size_t T = 0; const uint8_t* block = nullptr;
-        std::vector<uint8_t> done_flags;         // host-thread path: finished at submit time
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
-        cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+        Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
     } dbs[FABGPU_SLOTS];
     std::mutex blk_mu[FABGPU_SLOTS];
+    // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
+    ~fabgpu_ctx() { if (!devs.empty()) cudaSetDevice(devs[0].id); }
 };
 
 namespace {
@@ -256,6 +259,14 @@ namespace {
             return FABGPU_E_CUDA;                                                                           \
         }                                                                                                   \
     } while (0)
+
+// Reserves arrays in order (CudaArray::reserve) until one fails; the arrays after that one are freed instead.  A group whose capacity is
+// read from the array it grows last therefore reads as empty after a failed grow, and the next call grows the whole group again.
+struct Grow {
+    fabgpu_ctx* ctx;
+    int rc = FABGPU_OK;
+    template <typename A> void operator()(A& a, size_t bytes) { if (rc == FABGPU_OK) rc = a.reserve(ctx, bytes); else a = A(); }
+};
 
 bool fault_injected()
 {
@@ -337,11 +348,11 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         if (n_dev) { ctx->last_error = "peer exchange needs a host-known batch size"; return FABGPU_E_ARG; }
     }
     if (n == 0 && !peer) return FABGPU_OK;
-    if ((mode == MODE_MIXED || mode == MODE_SMALL) && dv.s_ev_set) CK(ctx, cudaStreamWaitEvent(st, dv.s_ev, 0));   // small tables still being built
+    if ((mode == MODE_MIXED || mode == MODE_SMALL) && dv.s_ev_set) CK(ctx, cudaStreamWaitEvent(st, dv.s_ev.get(), 0));   // small tables still being built
     if (mode == MODE_SMALL && n > 0) {
         const unsigned sthreads = small_threads(ctx, dv, n, false);
         ecdsa_verify_small_kernel<<<(unsigned)((n + sthreads - 1) / sthreads), sthreads, 0, st>>>(
-            nullptr, nullptr, 0u, key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.stab, mask, off);
+            nullptr, nullptr, 0u, key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.stab.get(), mask, off);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -355,28 +366,28 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
             const unsigned sigs = FAB_LANES_THREADS / (unsigned)ctx->cached_kernel, blocks = (unsigned)((n + sigs - 1) / sigs);
             uint32_t nn = (uint32_t)n;
             if (n_dev) { ctx->last_error = "the lane-split kernel has no device-side batch size"; return FABGPU_E_ARG; }
-            if (ctx->cached_kernel == 2) ecdsa_verify_lanes_kernel<2><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab, dv.qtab, mask, off);
-            else ecdsa_verify_lanes_kernel<4><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab, dv.qtab, mask, off);
+            if (ctx->cached_kernel == 2) ecdsa_verify_lanes_kernel<2><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab.get(), dv.qtab.get(), mask, off);
+            else ecdsa_verify_lanes_kernel<4><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab.get(), dv.qtab.get(), mask, off);
         } else if (ctx->cached_kernel == 3 && !n_dev && !fused_peer) {
             // batch-affine, two signatures per thread, no CTA exchange
             const unsigned per = 2 * FAB_BA2_THREADS, blocks = (unsigned)((n + per - 1) / per);
-            ecdsa_verify_ba2_kernel<<<blocks, FAB_BA2_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.qtab, mask, off);
+            ecdsa_verify_ba2_kernel<<<blocks, FAB_BA2_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off);
         } else if (ctx->cached_kernel == 1 || ctx->cached_kernel == 3) {
             // batch-affine accumulation with CTA-shared inversions (ecdsa_batchaffine.cuh): fixed CTA width
             const unsigned blocks = (unsigned)((n + FAB_BA_THREADS - 1) / FAB_BA_THREADS);
-            ecdsa_verify_ba_kernel<<<blocks, FAB_BA_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.qtab, mask, off, n_dev, n_base, po);
+            ecdsa_verify_ba_kernel<<<blocks, FAB_BA_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off, n_dev, n_base, po);
         } else {
         // the scalars (ecdsa_prep_kernel), then the chain.  scal: 64 bytes per signature from the caller's slot, or stream-ordered from
         // the device's pool when the launch has no slot
         const bool own = scal == nullptr;
-        if (own) CK(ctx, cudaMallocFromPoolAsync((void**)&scal, 64 * n, dv.scal_pool, st));
+        if (own) CK(ctx, cudaMallocFromPoolAsync((void**)&scal, 64 * n, dv.scal_pool.get(), st));
         ecdsa_prep_kernel<<<(unsigned)((n + FAB_PREP_THREADS - 1) / FAB_PREP_THREADS), FAB_PREP_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, scal, n_dev, n_base);
         ctx->launches++;
         unsigned threads = 128;
         const size_t sms = (size_t)dv.sms;
         if (!n_dev && n > sms * 384) threads = (n <= sms * FAB_CACHED_THREADS) ? FAB_CACHED_THREADS : 256;
         const unsigned blocks = (unsigned)((n + threads - 1) / threads);
-        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, scal, r, (uint32_t)n, dv.gtab, dv.qtab, mask, off, n_dev, n_base, po);
+        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, scal, r, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off, n_dev, n_base, po);
         if (own) CK(ctx, cudaFreeAsync(scal, st));
         }
         ctx->launches++;
@@ -390,17 +401,17 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         if (classes & CLASS_SMALL) {
             const unsigned sthreads = small_threads(ctx, dv, n, true);
             ecdsa_verify_small_kernel<<<(unsigned)((n + sthreads - 1) / sthreads), sthreads, 0, st>>>(
-                scratch_idx, scratch_idx + n + 1, (uint32_t)n, key_slot, e, r, s, (uint32_t)n, dv.gtab, dv.stab, mask, off);
+                scratch_idx, scratch_idx + n + 1, (uint32_t)n, key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.stab.get(), mask, off);
         }
         if (classes & CLASS_GENERIC)
             ecdsa_verify_indexed_kernel<<<(unsigned)((n + FAB_INDEXED_THREADS - 1) / FAB_INDEXED_THREADS), FAB_INDEXED_THREADS, 0, st>>>(
-                scratch_idx, scratch_idx + n, qx, qy, e, r, s, dv.gtab, mask, off);
+                scratch_idx, scratch_idx + n, qx, qy, e, r, s, dv.gtab.get(), mask, off);
         ctx->launches += 1 + ((classes & CLASS_SMALL) ? 1 : 0) + ((classes & CLASS_GENERIC) ? 1 : 0);
         CK(ctx, cudaGetLastError());
     } else if (mode == MODE_MIXED && n > 0) {
         // no scratch (launches on a caller's stream): the generic kernel filters on key_slot itself
         const unsigned gthreads = 128, blocks = (unsigned)((n + gthreads - 1) / gthreads);
-        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(key_slot, qx, qy, e, r, s, (uint32_t)n, dv.gtab, mask, off, n_dev, n_base);
+        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(key_slot, qx, qy, e, r, s, (uint32_t)n, dv.gtab.get(), mask, off, n_dev, n_base);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -410,7 +421,7 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         unsigned gthreads = 64;
         if (!n_dev && n > (size_t)dv.sms * 192) gthreads = (n <= (size_t)dv.sms * FAB_VERIFY_THREADS) ? FAB_VERIFY_THREADS : 256;
         const unsigned blocks = (unsigned)((n + gthreads - 1) / gthreads);
-        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(nullptr, qx, qy, e, r, s, (uint32_t)n, dv.gtab, mask, off, n_dev, n_base);
+        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(nullptr, qx, qy, e, r, s, (uint32_t)n, dv.gtab.get(), mask, off, n_dev, n_base);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -469,19 +480,19 @@ int enqueue_slot(fabgpu_ctx* ctx, int slot, size_t n, bool keyed)
         DevSlot& ds = dv.slot[slot];
         HostSlot& hs = ctx->hslot[slot];
         CK(ctx, cudaSetDevice(dv.id));
-        if (keyed) for (size_t i = begin; i < end; i++) hs.h_key_slot[i] = handle_to_slot(ctx, hs.h_key_slot[i]);   // handles -> live slots
+        if (keyed) for (size_t i = begin; i < end; i++) hs.h_key_slot.get()[i] = handle_to_slot(ctx, hs.h_key_slot.get()[i]);   // handles -> live slots
         int classes = CLASS_GENERIC;
-        const int mode = keyed ? slots_mode(hs.h_key_slot + begin, cnt, &classes) : MODE_GENERIC;
+        const int mode = keyed ? slots_mode(hs.h_key_slot.get() + begin, cnt, &classes) : MODE_GENERIC;
         for (int a = ((mode == MODE_CACHED || mode == MODE_SMALL) ? 2 : 0); a < 5; a++)     // a range where every key has a table needs no Qx/Qy on the device
-            CK(ctx, cudaMemcpyAsync(ds.d_in[a], hs.h_in[a] + 32 * begin, 32 * cnt, cudaMemcpyHostToDevice, ds.stream));
+            CK(ctx, cudaMemcpyAsync(ds.d_in[a].get(), hs.h_in[a].get() + 32 * begin, 32 * cnt, cudaMemcpyHostToDevice, ds.stream.get()));
         if (mode != MODE_GENERIC)
-            CK(ctx, cudaMemcpyAsync(ds.d_key_slot, hs.h_key_slot + begin, 4 * cnt, cudaMemcpyHostToDevice, ds.stream));
-        int rc = launch_verify(ctx, dv, mode, ds.d_key_slot, ds.d_in[0], ds.d_in[1], ds.d_in[2], ds.d_in[3], ds.d_in[4], cnt, ds.d_mask,
-                               ds.d_off, ds.stream, nullptr, 0, nullptr, ds.d_idx, classes, ds.d_scal);
+            CK(ctx, cudaMemcpyAsync(ds.d_key_slot.get(), hs.h_key_slot.get() + begin, 4 * cnt, cudaMemcpyHostToDevice, ds.stream.get()));
+        int rc = launch_verify(ctx, dv, mode, ds.d_key_slot.get(), ds.d_in[0].get(), ds.d_in[1].get(), ds.d_in[2].get(), ds.d_in[3].get(), ds.d_in[4].get(), cnt, ds.d_mask.get(),
+                               ds.d_off.get(), ds.stream.get(), nullptr, 0, nullptr, ds.d_idx.get(), classes, ds.d_scal.get());
         if (rc) return rc;
         const size_t words = (cnt + 31) / 32;
-        CK(ctx, cudaMemcpyAsync(hs.h_mask + begin / 32, ds.d_mask, 4 * words, cudaMemcpyDeviceToHost, ds.stream));
-        CK(ctx, cudaMemcpyAsync(hs.h_off + begin / 32, ds.d_off, 4 * words, cudaMemcpyDeviceToHost, ds.stream));
+        CK(ctx, cudaMemcpyAsync(hs.h_mask.get() + begin / 32, ds.d_mask.get(), 4 * words, cudaMemcpyDeviceToHost, ds.stream.get()));
+        CK(ctx, cudaMemcpyAsync(hs.h_off.get() + begin / 32, ds.d_off.get(), 4 * words, cudaMemcpyDeviceToHost, ds.stream.get()));
     }
     return FABGPU_OK;
 }
@@ -490,74 +501,9 @@ int wait_slot(fabgpu_ctx* ctx, int slot)
 {
     for (auto& dv : ctx->devs) {
         CK(ctx, cudaSetDevice(dv.id));
-        CK(ctx, cudaStreamSynchronize(dv.slot[slot].stream));
+        CK(ctx, cudaStreamSynchronize(dv.slot[slot].stream.get()));
     }
     return FABGPU_OK;
-}
-
-void free_all(fabgpu_ctx* ctx)
-{
-    {
-        if (!ctx->devs.empty()) cudaSetDevice(ctx->devs[0].id);
-        for (auto& bb : ctx->bbs) {
-            void* dev_ptrs[] = {bb.d_block, bb.d_sha, bb.d_dig, bb.d_r, bb.d_s, bb.d_qx, bb.d_qy, bb.d_ks, bb.d_mask, bb.d_off};
-            for (void* p : dev_ptrs) if (p) cudaFree(p);
-            void* host_ptrs[] = {bb.h_block, bb.h_sha, bb.h_dig, bb.h_r, bb.h_s, bb.h_qx, bb.h_qy, bb.h_ks, bb.h_mask};
-            for (void* p : host_ptrs) if (p) cudaFreeHost(p);
-        }
-        auto& dm = ctx->dm;
-        void* dev2[] = {dm.id_blob, dm.valid, dm.keys_xy, dm.channel, dm.id_off, dm.key_slot, dm.msp_code, dm.ht_idx, dm.nodes, dm.principal_code, dm.ht_hash,
-                        dm.group, dm.ns_blob, dm.ns_off, dm.ns_root, dm.pbits};
-        for (void* p : dev2) if (p) cudaFree(p);
-        for (auto& db : ctx->dbs) {
-            void* dev4[] = {db.d_env_off, db.d_txs, db.d_raw, db.d_sha, db.d_r, db.d_s, db.d_qx, db.d_qy, db.d_gate, db.d_dig, db.d_flags, db.d_ks, db.d_ident, db.d_mask, db.d_off,
-                            db.d_counter, db.d_hash, db.d_seg, db.d_idx, db.d_scal};
-            for (void* p : dev4) if (p) cudaFree(p);
-            void* host2[] = {db.h_flags, db.h_hash, db.h_seg, db.h_counter, db.h_env_off};
-            for (void* p : host2) if (p) cudaFreeHost(p);
-            for (auto& e : db.ev) if (e) cudaEventDestroy(e);
-        }
-        for (auto& gb : ctx->gb) {
-        void* dev3[] = {gb.d_sigs, gb.d_digs, gb.d_keys, gb.d_status, gb.d_pre, gb.d_r, gb.d_s, gb.d_e, gb.d_qx, gb.d_qy, gb.d_sig_off, gb.d_dig_off, gb.d_mask, gb.d_off,
-                        gb.d_kidx, gb.d_slot_of, gb.d_ks, gb.d_idx, gb.d_scal};
-        for (void* p : dev3) if (p) cudaFree(p);
-        void* host3[] = {gb.h_sigs, gb.h_digs, gb.h_keys, gb.h_status, gb.h_sig_off, gb.h_dig_off, gb.h_kidx, gb.h_slot_of};
-        for (void* p : host3) if (p) cudaFreeHost(p);
-        }
-    }
-    for (auto& dv : ctx->devs) {
-        cudaSetDevice(dv.id);
-        {   // peer-memory bitmask exchange (fabgpu_peer_mask_*)
-            auto& pr = dv.peer;
-            for (int p = 0; p < FAB_PEER_MAX; p++) if (pr.opened[p]) cudaIpcCloseMemHandle(pr.mapped[p]);
-            if (pr.local) cudaFree(pr.local);
-            if (pr.done) cudaFree(pr.done);
-            if (pr.h_timeout) cudaFreeHost(pr.h_timeout);
-            pr = Device::Peer();
-        }
-        if (dv.gtab) cudaFree(dv.gtab);
-        if (dv.qtab) cudaFree(dv.qtab);
-        void* sm[] = {dv.stab, dv.s_bases, dv.s_keys, dv.s_slots};
-        for (void* q : sm) if (q) cudaFree(q);
-        if (dv.s_ev) cudaEventDestroy(dv.s_ev);
-        if (dv.s_stream) cudaStreamDestroy(dv.s_stream);
-        if (dv.scal_pool) cudaMemPoolDestroy(dv.scal_pool);      // frees still in flight complete on their own
-        for (auto& ds : dv.slot) {
-            if (ds.d_key_slot) cudaFree(ds.d_key_slot);
-            if (ds.d_idx) cudaFree(ds.d_idx);
-            if (ds.d_scal) cudaFree(ds.d_scal);
-            for (auto& p : ds.d_in) if (p) cudaFree(p);
-            if (ds.d_mask) cudaFree(ds.d_mask);
-            if (ds.d_off) cudaFree(ds.d_off);
-            if (ds.stream) cudaStreamDestroy(ds.stream);
-        }
-    }
-    for (auto& hs : ctx->hslot) {
-        for (auto& p : hs.h_in) if (p) cudaFreeHost(p);
-        if (hs.h_mask) cudaFreeHost(hs.h_mask);
-        if (hs.h_off) cudaFreeHost(hs.h_off);
-        if (hs.h_key_slot) cudaFreeHost(hs.h_key_slot);
-    }
 }
 
 int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batch)
@@ -630,7 +576,7 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
         if (ck) ctx->cached_kernel = (ck[0] == 'j' || ck[0] == '0') ? 0 : (ck[0] == 'l' ? (ck[1] == '4' ? 4 : 2) : (ck[0] == 'b' && ck[1] == 'a' && ck[2] == '2' ? 3 : 1));   // "jac" / "0": the Jacobian-chain kernel; "l2" / "l4": its lane-split variant
     }
     ctx->dev_cap = round_up32((max_batch + ids.size() - 1) / ids.size());
-    ctx->devs.resize(ids.size());
+    ctx->devs = std::vector<Device>(ids.size());          // Device is not movable: the vector is built at its final size
     const size_t words = ctx->dev_cap / 32;
     const size_t tab_entries = (size_t)FAB_G_WINDOWS * FAB_G_ENTRIES;
     for (size_t d = 0; d < ids.size(); d++) {
@@ -645,85 +591,86 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             if (want == 32 || want == 64 || want == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, want);   // a hint: failure is not an error
             (void)cudaGetLastError();
         }
-        CK(ctx, cudaMalloc(&dv.gtab, tab_entries * sizeof(aff)));
-        CK(ctx, cudaMalloc(&dv.qtab, (size_t)ctx->key_slots * FAB_Q_WINDOWS * FAB_Q_ENTRIES * sizeof(aff)));
+        Grow grow{ctx};
+        grow(dv.gtab, tab_entries * sizeof(aff));
+        grow(dv.qtab, (size_t)ctx->key_slots * FAB_Q_WINDOWS * FAB_Q_ENTRIES * sizeof(aff));
         if (ctx->small_slots > 0) {
-            CK(ctx, cudaMalloc(&dv.stab, (size_t)ctx->small_slots * FAB_S_POINTS * sizeof(aff)));
+            grow(dv.stab, (size_t)ctx->small_slots * FAB_S_POINTS * sizeof(aff));
             // build scratch for up to 16 384 keys per registration, allocated once: growing it later costs a cudaFree + cudaMalloc pair in the
             // middle of traffic (the pair waits for all work in flight)
             const size_t c = (size_t)std::min(ctx->small_slots, 16384);
-            CK(ctx, cudaMalloc(&dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff)));
-            CK(ctx, cudaMalloc(&dv.s_keys, 64 * c));
-            CK(ctx, cudaMalloc(&dv.s_slots, 4 * c));
-            dv.s_cap = c;
+            grow(dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff));
+            grow(dv.s_keys, 64 * c);
+            grow(dv.s_slots, 4 * c);
         }
-        CK(ctx, cudaStreamCreateWithFlags(&dv.s_stream, cudaStreamNonBlocking));
-        CK(ctx, cudaEventCreateWithFlags(&dv.s_ev, cudaEventDisableTiming));
+        if (grow.rc) return grow.rc;
+        cudaStream_t st = nullptr;
+        CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+        dv.s_stream.reset(st);
+        cudaEvent_t ev = nullptr;
+        CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        dv.s_ev.reset(ev);
         for (auto& ds : dv.slot) {
-            CK(ctx, cudaStreamCreateWithFlags(&ds.stream, cudaStreamNonBlocking));
-            for (auto& p : ds.d_in) CK(ctx, cudaMalloc(&p, 32 * ctx->dev_cap));
-            CK(ctx, cudaMalloc(&ds.d_mask, 4 * words));
-            CK(ctx, cudaMalloc(&ds.d_off, 4 * words));
-            CK(ctx, cudaMalloc(&ds.d_key_slot, 4 * ctx->dev_cap));
-            CK(ctx, cudaMalloc(&ds.d_idx, 4 * (ctx->dev_cap + 2)));
-            CK(ctx, cudaMalloc(&ds.d_scal, 64 * ctx->dev_cap));
+            CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+            ds.stream.reset(st);
+            for (auto& p : ds.d_in) grow(p, 32 * ctx->dev_cap);
+            grow(ds.d_mask, 4 * words);
+            grow(ds.d_off, 4 * words);
+            grow(ds.d_key_slot, 4 * ctx->dev_cap);
+            grow(ds.d_idx, 4 * (ctx->dev_cap + 2));
+            grow(ds.d_scal, 64 * ctx->dev_cap);
+            if (grow.rc) return grow.rc;
         }
         {
             cudaMemPoolProps pp; memset(&pp, 0, sizeof pp);
             pp.allocType = cudaMemAllocationTypePinned;
             pp.location.type = cudaMemLocationTypeDevice;
             pp.location.id = dv.id;
-            CK(ctx, cudaMemPoolCreate(&dv.scal_pool, &pp));
+            cudaMemPool_t pool = nullptr;
+            CK(ctx, cudaMemPoolCreate(&pool, &pp));
+            dv.scal_pool.reset(pool);
             uint64_t keep = UINT64_MAX;
-            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool, cudaMemPoolAttrReleaseThreshold, &keep));
+            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool.get(), cudaMemPoolAttrReleaseThreshold, &keep));
             int no = 0;
-            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool, cudaMemPoolReuseAllowInternalDependencies, &no));
+            CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool.get(), cudaMemPoolReuseAllowInternalDependencies, &no));
         }
 #if FAB_G_TWO_LEVEL
         {
-            aff* d_small = nullptr; u256* d_scratch = nullptr;
+            DevArray<u256> d_scratch; DevArray<aff> d_small;
             const size_t nsmall = ((size_t)1 << (FAB_WG / 2)) - 1;
             const size_t threads = (size_t)FAB_G_WINDOWS * 2;
-            CK(ctx, cudaMalloc(&d_scratch, threads * 2 * nsmall * sizeof(u256)));
-            CK(ctx, cudaMalloc(&d_small, threads * nsmall * sizeof(aff)));
-            small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream>>>(nullptr, 1, FAB_WG, FAB_G_WINDOWS, d_small, d_scratch, nullptr);
+            grow(d_scratch, threads * 2 * nsmall * sizeof(u256));
+            grow(d_small, threads * nsmall * sizeof(aff));
+            if (grow.rc) return grow.rc;
+            small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(nullptr, 1, FAB_WG, FAB_G_WINDOWS, d_small.get(), d_scratch.get(), nullptr);
             const size_t threads2 = (size_t)FAB_G_WINDOWS * ((FAB_G_ENTRIES + FAB_TAB_CHUNK - 1) / FAB_TAB_CHUNK);
-            full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream>>>(d_small, nullptr, nullptr, 1, FAB_WG, FAB_G_WINDOWS, dv.gtab);
+            full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), nullptr, nullptr, 1, FAB_WG, FAB_G_WINDOWS, dv.gtab.get());
             ctx->launches += 2;
             CK(ctx, cudaGetLastError());
-            CK(ctx, cudaStreamSynchronize(dv.slot[0].stream));
-            cudaFree(d_small); cudaFree(d_scratch);
+            CK(ctx, cudaStreamSynchronize(dv.slot[0].stream.get()));
         }
 #else
-        build_g_table_kernel<<<(unsigned)((tab_entries + 127) / 128), 128, 0, dv.slot[0].stream>>>(dv.gtab);
+        build_g_table_kernel<<<(unsigned)((tab_entries + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(dv.gtab.get());
         ctx->launches++;
         CK(ctx, cudaGetLastError());
 #endif
     }
     const size_t hwords = (round_up32(max_batch) / 32) + ids.size();
     for (auto& hs : ctx->hslot) {
-        for (auto& p : hs.h_in) CK(ctx, cudaHostAlloc(&p, 32 * round_up32(max_batch), cudaHostAllocPortable));
-        CK(ctx, cudaHostAlloc(&hs.h_mask, 4 * hwords, cudaHostAllocPortable));
-        CK(ctx, cudaHostAlloc(&hs.h_off, 4 * hwords, cudaHostAllocPortable));
-        CK(ctx, cudaHostAlloc(&hs.h_key_slot, 4 * round_up32(max_batch), cudaHostAllocPortable));
-        for (size_t i = 0; i < round_up32(max_batch); i++) hs.h_key_slot[i] = -1;
+        Grow grow{ctx};
+        for (auto& p : hs.h_in) grow(p, 32 * round_up32(max_batch));
+        grow(hs.h_mask, 4 * hwords);
+        grow(hs.h_off, 4 * hwords);
+        grow(hs.h_key_slot, 4 * round_up32(max_batch));
+        if (grow.rc) return grow.rc;
+        for (size_t i = 0; i < round_up32(max_batch); i++) hs.h_key_slot.get()[i] = -1;
     }
     for (auto& dv : ctx->devs) {
         CK(ctx, cudaSetDevice(dv.id));
-        CK(ctx, cudaStreamSynchronize(dv.slot[0].stream));
+        CK(ctx, cudaStreamSynchronize(dv.slot[0].stream.get()));
     }
     return FABGPU_OK;
 }
-
-// device temporaries released on every path (fabgpu_keys_register)
-struct DevTmp {
-    std::vector<void*> p;
-    ~DevTmp() { for (void* q : p) if (q) cudaFree(q); }
-    template <typename T> cudaError_t alloc(T*& out, size_t bytes) { void* q = nullptr; cudaError_t e = cudaMalloc(&q, bytes); out = (T*)q; if (e == cudaSuccess) p.push_back(q); return e; }
-};
-
-template <typename T> int grow_dev(fabgpu_ctx* ctx, T*& p, size_t bytes) { if (p) cudaFree(p); p = nullptr; CK(ctx, cudaMalloc(&p, bytes)); return FABGPU_OK; }
-template <typename T> int grow_host(fabgpu_ctx* ctx, T*& p, size_t bytes) { if (p) cudaFreeHost(p); p = nullptr; CK(ctx, cudaHostAlloc(&p, bytes, cudaHostAllocPortable)); return FABGPU_OK; }
 
 }  // namespace
 
@@ -737,7 +684,6 @@ int fabgpu_init(const int* device_ids, int n_dev, size_t max_batch, fabgpu_ctx**
     int rc = init_impl(ctx, device_ids, n_dev, max_batch);
     if (rc != FABGPU_OK) {
         g_init_error = ctx->last_error;
-        free_all(ctx);
         delete ctx;
         return rc;
     }
@@ -749,7 +695,6 @@ void fabgpu_destroy(fabgpu_ctx* ctx)
 {
     if (!ctx) return;
     for (int s = 0; s < FABGPU_SLOTS; s++) wait_slot(ctx, s);
-    free_all(ctx);
     delete ctx;
 }
 
@@ -763,13 +708,13 @@ int fabgpu_host_buffers(fabgpu_ctx* ctx, int slot, uint8_t** qx, uint8_t** qy, u
 {
     if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
     HostSlot& hs = ctx->hslot[slot];
-    if (qx) *qx = hs.h_in[0];
-    if (qy) *qy = hs.h_in[1];
-    if (e) *e = hs.h_in[2];
-    if (r) *r = hs.h_in[3];
-    if (s) *s = hs.h_in[4];
-    if (mask) *mask = hs.h_mask;
-    if (offcurve) *offcurve = hs.h_off;
+    if (qx) *qx = hs.h_in[0].get();
+    if (qy) *qy = hs.h_in[1].get();
+    if (e) *e = hs.h_in[2].get();
+    if (r) *r = hs.h_in[3].get();
+    if (s) *s = hs.h_in[4].get();
+    if (mask) *mask = hs.h_mask.get();
+    if (offcurve) *offcurve = hs.h_off.get();
     return FABGPU_OK;
 }
 
@@ -796,7 +741,7 @@ int fabgpu_verify_p256_keyed(fabgpu_ctx* ctx, int slot, size_t n)
 int fabgpu_host_key_slots(fabgpu_ctx* ctx, int slot, int32_t** key_slot)
 {
     if (!ctx || slot < 0 || slot >= FABGPU_SLOTS || !key_slot) return FABGPU_E_ARG;
-    *key_slot = ctx->hslot[slot].h_key_slot;
+    *key_slot = ctx->hslot[slot].h_key_slot.get();
     return FABGPU_OK;
 }
 
@@ -849,36 +794,39 @@ int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t
     for (int i = 0; i < F; i++) memcpy(fk.data() + 64 * (size_t)i, keys_xy + 64 * (size_t)fresh[i], 64);
     std::vector<uint32_t> flags(F, 0);
     auto build_on = [&](Device& dv) -> int {
-        DevTmp tmp;
         CK(ctx, cudaSetDevice(dv.id));
         // an evicted slot's table may still be read by a batch in flight: drain this device first (registration is rare)
-        for (auto& ds : dv.slot) CK(ctx, cudaStreamSynchronize(ds.stream));
+        for (auto& ds : dv.slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
         CK(ctx, cudaDeviceSynchronize());            // launches on caller streams (fabgpu_verify_p256_device_keyed) as well
-        uint8_t* d_keys = nullptr; int32_t* d_slots = nullptr; uint32_t* d_flags = nullptr; u256* d_scratch = nullptr;
-        CK(ctx, tmp.alloc(d_keys, fk.size()));
-        CK(ctx, tmp.alloc(d_slots, 4 * (size_t)F));
-        CK(ctx, tmp.alloc(d_flags, 4 * (size_t)F));
-        CK(ctx, cudaMemcpy(d_keys, fk.data(), fk.size(), cudaMemcpyHostToDevice));
-        CK(ctx, cudaMemcpy(d_slots, fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice));
+        DevArray<uint8_t> d_keys; DevArray<int32_t> d_slots; DevArray<uint32_t> d_flags; DevArray<u256> d_scratch;
+        Grow grow{ctx};
+        grow(d_keys, fk.size());
+        grow(d_slots, 4 * (size_t)F);
+        grow(d_flags, 4 * (size_t)F);
+        if (grow.rc) return grow.rc;
+        CK(ctx, cudaMemcpy(d_keys.get(), fk.data(), fk.size(), cudaMemcpyHostToDevice));
+        CK(ctx, cudaMemcpy(d_slots.get(), fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice));
 #if FAB_Q_TWO_LEVEL
-        aff* d_small = nullptr;
+        DevArray<aff> d_small;
         const size_t nsmall = ((size_t)1 << (FAB_WQ / 2)) - 1;
         const size_t threads = (size_t)F * FAB_Q_WINDOWS * 2;
-        CK(ctx, tmp.alloc(d_scratch, threads * 2 * nsmall * sizeof(u256)));
-        CK(ctx, tmp.alloc(d_small, threads * nsmall * sizeof(aff)));
-        small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream>>>(d_keys, F, FAB_WQ, FAB_Q_WINDOWS, d_small, d_scratch, d_flags);
+        grow(d_scratch, threads * 2 * nsmall * sizeof(u256));
+        grow(d_small, threads * nsmall * sizeof(aff));
+        if (grow.rc) return grow.rc;
+        small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(d_keys.get(), F, FAB_WQ, FAB_Q_WINDOWS, d_small.get(), d_scratch.get(), d_flags.get());
         const size_t threads2 = (size_t)F * FAB_Q_WINDOWS * ((FAB_Q_ENTRIES + FAB_TAB_CHUNK - 1) / FAB_TAB_CHUNK);
-        full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream>>>(d_small, d_slots, d_flags, F, FAB_WQ, FAB_Q_WINDOWS, dv.qtab);
+        full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), d_slots.get(), d_flags.get(), F, FAB_WQ, FAB_Q_WINDOWS, dv.qtab.get());
         ctx->launches += 2;
 #else
         const size_t threads = (size_t)F * FAB_Q_WINDOWS;
-        CK(ctx, tmp.alloc(d_scratch, threads * 2 * FAB_Q_ENTRIES * sizeof(u256)));
-        build_key_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream>>>(d_keys, d_slots, F, dv.qtab, d_scratch, d_flags);
+        grow(d_scratch, threads * 2 * FAB_Q_ENTRIES * sizeof(u256));
+        if (grow.rc) return grow.rc;
+        build_key_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(d_keys.get(), d_slots.get(), F, dv.qtab.get(), d_scratch.get(), d_flags.get());
         ctx->launches++;
 #endif
         CK(ctx, cudaGetLastError());
-        CK(ctx, cudaStreamSynchronize(dv.slot[0].stream));
-        CK(ctx, cudaMemcpy(flags.data(), d_flags, 4 * (size_t)F, cudaMemcpyDeviceToHost));
+        CK(ctx, cudaStreamSynchronize(dv.slot[0].stream.get()));
+        CK(ctx, cudaMemcpy(flags.data(), d_flags.get(), 4 * (size_t)F, cudaMemcpyDeviceToHost));
         return FABGPU_OK;
     };
     for (auto& dv : ctx->devs) {
@@ -967,27 +915,25 @@ static int small_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_
     auto build_on = [&](Device& dv) -> int {
         CK(ctx, cudaSetDevice(dv.id));
         auto b0 = tnow();
-        if ((size_t)F > dv.s_cap) {
-            CK(ctx, cudaStreamSynchronize(dv.s_stream));            // an earlier build may still use the scratch
+        if ((size_t)F > dv.s_cap()) {
+            CK(ctx, cudaStreamSynchronize(dv.s_stream.get()));            // an earlier build may still use the scratch
             const size_t c = (size_t)F + (size_t)F / 2 + 256;
-            void* old[] = {dv.s_bases, dv.s_keys, dv.s_slots};
-            for (void* q : old) if (q) cudaFree(q);
-            dv.s_bases = nullptr; dv.s_keys = nullptr; dv.s_slots = nullptr; dv.s_cap = 0;
-            CK(ctx, cudaMalloc(&dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff)));
-            CK(ctx, cudaMalloc(&dv.s_keys, 64 * c));
-            CK(ctx, cudaMalloc(&dv.s_slots, 4 * c));
-            dv.s_cap = c;
+            Grow grow{ctx};
+            grow(dv.s_keys, 64 * c);
+            grow(dv.s_slots, 4 * c);
+            grow(dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff));      // last: it holds s_cap()
+            if (grow.rc) return grow.rc;
         }
         auto b1 = tnow();
-        CK(ctx, cudaMemcpyAsync(dv.s_keys, fk.data(), fk.size(), cudaMemcpyHostToDevice, dv.s_stream));
-        CK(ctx, cudaMemcpyAsync(dv.s_slots, fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice, dv.s_stream));
-        CK(ctx, cudaStreamSynchronize(dv.s_stream));                // the sources are local vectors
+        CK(ctx, cudaMemcpyAsync(dv.s_keys.get(), fk.data(), fk.size(), cudaMemcpyHostToDevice, dv.s_stream.get()));
+        CK(ctx, cudaMemcpyAsync(dv.s_slots.get(), fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice, dv.s_stream.get()));
+        CK(ctx, cudaStreamSynchronize(dv.s_stream.get()));                // the sources are local vectors
         auto b2 = tnow();
-        small_bases_kernel<<<(unsigned)((F + 31) / 32), 32, 0, dv.s_stream>>>(dv.s_keys, dv.s_slots, F, dv.s_bases, dv.stab);
-        small_windows_kernel<<<(unsigned)(((size_t)F * FAB_S_WINDOWS + 127) / 128), 128, 0, dv.s_stream>>>(dv.s_bases, dv.s_slots, F, dv.stab);
+        small_bases_kernel<<<(unsigned)((F + 31) / 32), 32, 0, dv.s_stream.get()>>>(dv.s_keys.get(), dv.s_slots.get(), F, dv.s_bases.get(), dv.stab.get());
+        small_windows_kernel<<<(unsigned)(((size_t)F * FAB_S_WINDOWS + 127) / 128), 128, 0, dv.s_stream.get()>>>(dv.s_bases.get(), dv.s_slots.get(), F, dv.stab.get());
         ctx->launches += 2;
         CK(ctx, cudaGetLastError());
-        CK(ctx, cudaEventRecord(dv.s_ev, dv.s_stream));
+        CK(ctx, cudaEventRecord(dv.s_ev.get(), dv.s_stream.get()));
         dv.s_ev_set = true;
         if (trace) fprintf(stderr, "[fabgpu] small_register F=%d: lock %.0f us, bookkeeping %.0f us, scratch %.0f us, copies %.0f us, launches %.0f us\n", F, tus(tr0, tr1),
                            tus(tr1, tr2), tus(b0, b1), tus(b1, b2), tus(b2, tnow()));
@@ -1034,7 +980,7 @@ int fabgpu_wait(fabgpu_ctx* ctx, int slot)
     // fills slot k+1 while slot k runs).  Stream handles are immutable after fabgpu_init; errors go to a local string first.
     for (auto& dv : ctx->devs) {
         cudaError_t e = cudaSetDevice(dv.id);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(dv.slot[slot].stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(dv.slot[slot].stream.get());
         if (e != cudaSuccess) {
             std::lock_guard<std::mutex> lk(ctx->mu);
             ctx->last_error = std::string("cudaStreamSynchronize failed: ") + cudaGetErrorString(e);
@@ -1059,12 +1005,12 @@ int fabgpu_verify_p256_host(fabgpu_ctx* ctx, const uint8_t* qx, const uint8_t* q
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     HostSlot& hs = ctx->hslot[0];
     const uint8_t* src[5] = {qx, qy, e, r, s};
-    for (int a = 0; a < 5; a++) memcpy(hs.h_in[a], src[a], 32 * n);
+    for (int a = 0; a < 5; a++) memcpy(hs.h_in[a].get(), src[a], 32 * n);
     int rc = fabgpu_verify_p256(ctx, 0, n);
     if (rc) return rc;
     const size_t words = (n + 31) / 32;
-    memcpy(mask, hs.h_mask, 4 * words);
-    if (offcurve) memcpy(offcurve, hs.h_off, 4 * words);
+    memcpy(mask, hs.h_mask.get(), 4 * words);
+    if (offcurve) memcpy(offcurve, hs.h_off.get(), 4 * words);
     return FABGPU_OK;
 }
 
@@ -1107,23 +1053,21 @@ int fabgpu_peer_mask_create(fabgpu_ctx* ctx, int dev_index, int world, int rank,
     static_assert(sizeof(cudaIpcMemHandle_t) <= FABGPU_IPC_HANDLE_BYTES, "IPC handle size");
     Device& dv = ctx->devs[dev_index];
     auto& pr = dv.peer;
-    if (pr.local) { ctx->last_error = "peer mask already created on this device"; return FABGPU_E_ARG; }
+    if (pr.local.get()) { ctx->last_error = "peer mask already created on this device"; return FABGPU_E_ARG; }
     CK(ctx, cudaSetDevice(dv.id));
     const size_t bytes = 4 * peer_buf_words(world, words_per_rank);
-    CK(ctx, cudaMalloc(&pr.local, bytes));
-    CK(ctx, cudaMemset(pr.local, 0, bytes));
-    CK(ctx, cudaMalloc(&pr.done, 8));
-    CK(ctx, cudaMemset(pr.done, 0, 8));
-    pr.timeout = pr.done + 1;
-    CK(ctx, cudaHostAlloc(&pr.h_timeout, 4, cudaHostAllocPortable));
-    *pr.h_timeout = 0;
+    if (int rc = pr.local.reserve(ctx, bytes)) return rc;
+    CK(ctx, cudaMemset(pr.local.get(), 0, bytes));
+    if (int rc = pr.done.reserve(ctx, 8)) return rc;
+    CK(ctx, cudaMemset(pr.done.get(), 0, 8));
+    pr.timeout = pr.done.get() + 1;
+    if (int rc = pr.h_timeout.reserve(ctx, 4)) return rc;
+    *pr.h_timeout.get() = 0;
     cudaIpcMemHandle_t h;
-    CK(ctx, cudaIpcGetMemHandle(&h, pr.local));
+    CK(ctx, cudaIpcGetMemHandle(&h, pr.local.get()));
     memset(handle_out, 0, FABGPU_IPC_HANDLE_BYTES);
     memcpy(handle_out, &h, sizeof h);
     pr.world = world; pr.rank = rank; pr.words_per_rank = words_per_rank;
-    for (int p = 0; p < FAB_PEER_MAX; p++) { pr.mapped[p] = nullptr; pr.opened[p] = false; }
-    pr.mapped[rank] = pr.local;
     pr.ready = world == 1;
     return FABGPU_OK;
 }
@@ -1133,15 +1077,15 @@ int fabgpu_peer_mask_open(fabgpu_ctx* ctx, int dev_index, const uint8_t* handles
     if (!ctx || dev_index < 0 || dev_index >= (int)ctx->devs.size() || !handles) return FABGPU_E_ARG;
     Device& dv = ctx->devs[dev_index];
     auto& pr = dv.peer;
-    if (!pr.local) { ctx->last_error = "fabgpu_peer_mask_create first"; return FABGPU_E_ARG; }
+    if (!pr.local.get()) { ctx->last_error = "fabgpu_peer_mask_create first"; return FABGPU_E_ARG; }
     CK(ctx, cudaSetDevice(dv.id));
     for (int p = 0; p < pr.world; p++) {
-        if (p == pr.rank || pr.opened[p]) continue;
+        if (p == pr.rank || pr.mapped[p]) continue;
         cudaIpcMemHandle_t h;
         memcpy(&h, handles + (size_t)p * FABGPU_IPC_HANDLE_BYTES, sizeof h);
         void* m = nullptr;
         CK(ctx, cudaIpcOpenMemHandle(&m, h, cudaIpcMemLazyEnablePeerAccess));
-        pr.mapped[p] = (uint32_t*)m; pr.opened[p] = true;
+        pr.mapped[p].reset((uint32_t*)m);
     }
     pr.ready = true;
     return FABGPU_OK;
@@ -1154,11 +1098,7 @@ int fabgpu_peer_mask_close(fabgpu_ctx* ctx, int dev_index)
     auto& pr = dv.peer;
     cudaSetDevice(dv.id);
     cudaDeviceSynchronize();
-    for (int p = 0; p < FAB_PEER_MAX; p++) if (pr.opened[p]) { cudaIpcCloseMemHandle(pr.mapped[p]); pr.opened[p] = false; pr.mapped[p] = nullptr; }
-    if (pr.local) cudaFree(pr.local);
-    if (pr.done) cudaFree(pr.done);
-    if (pr.h_timeout) cudaFreeHost(pr.h_timeout);
-    pr = Device::Peer();
+    std::exchange(pr, Device::Peer());      // the old state goes at the end of the statement: mappings closed first (Device::Peer)
     return FABGPU_OK;
 }
 
@@ -1174,25 +1114,25 @@ int fabgpu_verify_p256_device_keyed_allgather(fabgpu_ctx* ctx, int dev_index, in
     if (!pr.ready) { ctx->last_error = "peer masks are not set up (fabgpu_peer_mask_create / _open)"; return FABGPU_E_ARG; }
     if ((n + 31) / 32 > pr.words_per_rank) { ctx->last_error = "batch exceeds words_per_rank"; return FABGPU_E_ARG; }
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
-    if (*pr.h_timeout) { ctx->last_error = "a peer did not publish its bitmask in time"; return FABGPU_E_CUDA; }
+    if (*pr.h_timeout.get()) { ctx->last_error = "a peer did not publish its bitmask in time"; return FABGPU_E_CUDA; }
     CK(ctx, cudaSetDevice(dv.id));
     cudaStream_t st = (cudaStream_t)cuda_stream;
     PeerOut po; memset(&po, 0, sizeof po);
-    for (int p = 0; p < pr.world; p++) po.buf[p] = pr.mapped[p];
-    po.done = pr.done; po.world = (uint32_t)pr.world; po.rank = (uint32_t)pr.rank; po.words_per_rank = (uint32_t)pr.words_per_rank;
+    for (int p = 0; p < pr.world; p++) po.buf[p] = pr.buf(p);
+    po.done = pr.done.get(); po.world = (uint32_t)pr.world; po.rank = (uint32_t)pr.rank; po.words_per_rank = (uint32_t)pr.words_per_rank;
     po.gen_off = (uint32_t)((step % kPeerGens) * pr.world * pr.words_per_rank);
     po.flag_off = (uint32_t)((size_t)kPeerGens * pr.world * pr.words_per_rank);
     po.step = step;
     // the rank's own words also land in its local segment (buf[rank] is the local buffer): `mask` for the kernels is that segment
-    uint32_t* local_seg = pr.local + po.gen_off + (size_t)pr.rank * pr.words_per_rank;
+    uint32_t* local_seg = pr.local.get() + po.gen_off + (size_t)pr.rank * pr.words_per_rank;
     int rc = launch_verify(ctx, dv, all_cached == 2 ? MODE_SMALL : (all_cached ? MODE_CACHED : MODE_MIXED), (const int32_t*)d_key_slot, (const uint8_t*)d_qx, (const uint8_t*)d_qy,
                            (const uint8_t*)d_e, (const uint8_t*)d_r, (const uint8_t*)d_s, n, local_seg, nullptr, st, nullptr, 0, &po);
     if (rc) return rc;
-    peer_wait_kernel<<<1, 32, 0, st>>>(pr.local + po.flag_off, po.world, step, pr.timeout);
+    peer_wait_kernel<<<1, 32, 0, st>>>(pr.local.get() + po.flag_off, po.world, step, pr.timeout);
     ctx->launches++;
     CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpyAsync(pr.h_timeout, pr.timeout, 4, cudaMemcpyDeviceToHost, st));
-    *d_full_mask = pr.local + po.gen_off;
+    CK(ctx, cudaMemcpyAsync(pr.h_timeout.get(), pr.timeout, 4, cudaMemcpyDeviceToHost, st));
+    *d_full_mask = pr.local.get() + po.gen_off;
     return FABGPU_OK;
 }
 
@@ -1213,30 +1153,21 @@ int fabgpu_gate_signature(const uint8_t* sig, size_t sig_len, uint8_t r_out[32],
 static int gate_bufs_reserve(fabgpu_ctx* ctx, int slot, size_t n, size_t sig_bytes, size_t dig_bytes, size_t K)
 {
     auto& gb = ctx->gb[slot];
-    int rc = 0;
-    if (n > gb.n_cap) {
+    Grow grow{ctx};
+    if (n > gb.n_cap()) {
         const size_t c = round_up32(n + (n >> 2) + 1024);
-        gb.n_cap = 0;
-        rc |= grow_host(ctx, gb.h_sig_off, 4 * (c + 1)); rc |= grow_host(ctx, gb.h_dig_off, 4 * (c + 1)); rc |= grow_host(ctx, gb.h_kidx, 4 * c);
-        rc |= grow_host(ctx, gb.h_status, c);
-        rc |= grow_dev(ctx, gb.d_sig_off, 4 * (c + 1)); rc |= grow_dev(ctx, gb.d_dig_off, 4 * (c + 1)); rc |= grow_dev(ctx, gb.d_kidx, 4 * c);
-        rc |= grow_dev(ctx, gb.d_status, c); rc |= grow_dev(ctx, gb.d_pre, c); rc |= grow_dev(ctx, gb.d_r, 32 * c); rc |= grow_dev(ctx, gb.d_s, 32 * c);
-        rc |= grow_dev(ctx, gb.d_e, 32 * c); rc |= grow_dev(ctx, gb.d_qx, 32 * c); rc |= grow_dev(ctx, gb.d_qy, 32 * c); rc |= grow_dev(ctx, gb.d_ks, 4 * c);
-        rc |= grow_dev(ctx, gb.d_mask, c / 8 + 8); rc |= grow_dev(ctx, gb.d_off, c / 8 + 8); rc |= grow_dev(ctx, gb.d_idx, 4 * (c + 2));
-        rc |= grow_dev(ctx, gb.d_scal, 64 * c);
-        if (rc) return FABGPU_E_CUDA;
-        gb.n_cap = c;
+        grow(gb.h_sig_off, 4 * (c + 1)); grow(gb.h_dig_off, 4 * (c + 1)); grow(gb.h_kidx, 4 * c); grow(gb.h_status, c);
+        grow(gb.d_sig_off, 4 * (c + 1)); grow(gb.d_dig_off, 4 * (c + 1)); grow(gb.d_kidx, 4 * c);
+        grow(gb.d_status, c); grow(gb.d_pre, c); grow(gb.d_r, 32 * c); grow(gb.d_s, 32 * c);
+        grow(gb.d_e, 32 * c); grow(gb.d_qx, 32 * c); grow(gb.d_qy, 32 * c); grow(gb.d_ks, 4 * c);
+        grow(gb.d_mask, c / 8 + 8); grow(gb.d_off, c / 8 + 8); grow(gb.d_idx, 4 * (c + 2));
+        grow(gb.d_scal, 64 * c);
+        if (grow.rc) return grow.rc;
     }
-    if (sig_bytes > gb.sig_cap) { const size_t c = sig_bytes + (sig_bytes >> 2) + 4096; gb.sig_cap = 0; rc |= grow_host(ctx, gb.h_sigs, c); rc |= grow_dev(ctx, gb.d_sigs, c); if (rc) return FABGPU_E_CUDA; gb.sig_cap = c; }
-    if (dig_bytes > gb.dig_cap) { const size_t c = dig_bytes + (dig_bytes >> 2) + 4096; gb.dig_cap = 0; rc |= grow_host(ctx, gb.h_digs, c); rc |= grow_dev(ctx, gb.d_digs, c); if (rc) return FABGPU_E_CUDA; gb.dig_cap = c; }
-    if (K > gb.k_cap) {
-        const size_t c = K + 64;
-        gb.k_cap = 0;
-        rc |= grow_host(ctx, gb.h_keys, 64 * c); rc |= grow_host(ctx, gb.h_slot_of, 4 * c); rc |= grow_dev(ctx, gb.d_keys, 64 * c); rc |= grow_dev(ctx, gb.d_slot_of, 4 * c);
-        if (rc) return FABGPU_E_CUDA;
-        gb.k_cap = c;
-    }
-    return FABGPU_OK;
+    if (sig_bytes > gb.sig_cap()) { const size_t c = sig_bytes + (sig_bytes >> 2) + 4096; grow(gb.h_sigs, c); grow(gb.d_sigs, c); if (grow.rc) return grow.rc; }
+    if (dig_bytes > gb.dig_cap()) { const size_t c = dig_bytes + (dig_bytes >> 2) + 4096; grow(gb.h_digs, c); grow(gb.d_digs, c); if (grow.rc) return grow.rc; }
+    if (K > gb.k_cap()) { const size_t c = K + 64; grow(gb.h_keys, 64 * c); grow(gb.h_slot_of, 4 * c); grow(gb.d_keys, 64 * c); grow(gb.d_slot_of, 4 * c); }
+    return grow.rc;
 }
 
 // inplace: the batch already lies in the slot's pinned buffers (fabgpu_bccsp_batch_buffers): nothing is staged.
@@ -1266,45 +1197,45 @@ static int bccsp_device_submit(fabgpu_ctx* ctx, int slot, const uint8_t* keys_xy
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         for (int k = 0; k < K; k++) {
-            gb.h_slot_of[k] = handle_to_slot(ctx, slot_of[k]);
-            if (gb.h_slot_of[k] < 0) all_slots = false;
-            if (gb.h_slot_of[k] == -1) classes |= CLASS_GENERIC; else if (gb.h_slot_of[k] <= -2) classes |= CLASS_SMALL;
+            gb.h_slot_of.get()[k] = handle_to_slot(ctx, slot_of[k]);
+            if (gb.h_slot_of.get()[k] < 0) all_slots = false;
+            if (gb.h_slot_of.get()[k] == -1) classes |= CLASS_GENERIC; else if (gb.h_slot_of.get()[k] <= -2) classes |= CLASS_SMALL;
         }
     }
-    if (K > 0 && !inplace) memcpy(gb.h_keys, keys_xy, 64 * (size_t)K);
+    if (K > 0 && !inplace) memcpy(gb.h_keys.get(), keys_xy, 64 * (size_t)K);
     if (!inplace) ctx->pool->run([&](int tid) {
         auto slice = [&](size_t total, size_t& lo, size_t& hi) { lo = total * (size_t)tid / T; hi = total * (size_t)(tid + 1) / T; };
         size_t lo, hi;
-        slice(sig_bytes, lo, hi); stage_copy(gb.h_sigs + lo, sigs + sig_base + lo, hi - lo);
-        slice(dig_bytes, lo, hi); stage_copy(gb.h_digs + lo, digests + dig_base + lo, hi - lo);
-        slice(4 * (n + 1), lo, hi); stage_copy((uint8_t*)gb.h_sig_off + lo, (const uint8_t*)sig_off + lo, hi - lo);
-        slice(4 * (n + 1), lo, hi); stage_copy((uint8_t*)gb.h_dig_off + lo, (const uint8_t*)dig_off + lo, hi - lo);
-        slice(4 * n, lo, hi); stage_copy((uint8_t*)gb.h_kidx + lo, (const uint8_t*)key_idx + lo, hi - lo);
+        slice(sig_bytes, lo, hi); stage_copy(gb.h_sigs.get() + lo, sigs + sig_base + lo, hi - lo);
+        slice(dig_bytes, lo, hi); stage_copy(gb.h_digs.get() + lo, digests + dig_base + lo, hi - lo);
+        slice(4 * (n + 1), lo, hi); stage_copy((uint8_t*)gb.h_sig_off.get() + lo, (const uint8_t*)sig_off + lo, hi - lo);
+        slice(4 * (n + 1), lo, hi); stage_copy((uint8_t*)gb.h_dig_off.get() + lo, (const uint8_t*)dig_off + lo, hi - lo);
+        slice(4 * n, lo, hi); stage_copy((uint8_t*)gb.h_kidx.get() + lo, (const uint8_t*)key_idx + lo, hi - lo);
         stage_fence();
     });
     auto t1 = now();
-    cudaStream_t st = ds.stream;
-    CK(ctx, cudaMemcpyAsync(gb.d_sigs, gb.h_sigs, sig_bytes, cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemcpyAsync(gb.d_digs, gb.h_digs, dig_bytes, cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemcpyAsync(gb.d_sig_off, gb.h_sig_off, 4 * (n + 1), cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemcpyAsync(gb.d_dig_off, gb.h_dig_off, 4 * (n + 1), cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemcpyAsync(gb.d_kidx, gb.h_kidx, 4 * n, cudaMemcpyHostToDevice, st));
+    cudaStream_t st = ds.stream.get();
+    CK(ctx, cudaMemcpyAsync(gb.d_sigs.get(), gb.h_sigs.get(), sig_bytes, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(gb.d_digs.get(), gb.h_digs.get(), dig_bytes, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(gb.d_sig_off.get(), gb.h_sig_off.get(), 4 * (n + 1), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(gb.d_dig_off.get(), gb.h_dig_off.get(), 4 * (n + 1), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(gb.d_kidx.get(), gb.h_kidx.get(), 4 * n, cudaMemcpyHostToDevice, st));
     if (K > 0) {
-        CK(ctx, cudaMemcpyAsync(gb.d_keys, gb.h_keys, 64 * (size_t)K, cudaMemcpyHostToDevice, st));
-        CK(ctx, cudaMemcpyAsync(gb.d_slot_of, gb.h_slot_of, 4 * (size_t)K, cudaMemcpyHostToDevice, st));
+        CK(ctx, cudaMemcpyAsync(gb.d_keys.get(), gb.h_keys.get(), 64 * (size_t)K, cudaMemcpyHostToDevice, st));
+        CK(ctx, cudaMemcpyAsync(gb.d_slot_of.get(), gb.h_slot_of.get(), 4 * (size_t)K, cudaMemcpyHostToDevice, st));
     }
-    bdev::bccsp_gate_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(gb.d_sigs, gb.d_sig_off, gb.d_digs, gb.d_dig_off, gb.d_kidx, gb.d_slot_of, gb.d_keys, K,
-                                                                        (uint32_t)n, gb.d_r, gb.d_s, gb.d_e, gb.d_ks, (classes & CLASS_GENERIC) ? gb.d_qx : nullptr,
-                                                                        (classes & CLASS_GENERIC) ? gb.d_qy : nullptr, gb.d_pre, sig_base, dig_base);
+    bdev::bccsp_gate_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(gb.d_sigs.get(), gb.d_sig_off.get(), gb.d_digs.get(), gb.d_dig_off.get(), gb.d_kidx.get(), gb.d_slot_of.get(), gb.d_keys.get(), K,
+                                                                        (uint32_t)n, gb.d_r.get(), gb.d_s.get(), gb.d_e.get(), gb.d_ks.get(), (classes & CLASS_GENERIC) ? gb.d_qx.get() : nullptr,
+                                                                        (classes & CLASS_GENERIC) ? gb.d_qy.get() : nullptr, gb.d_pre.get(), sig_base, dig_base);
     ctx->launches++;
     CK(ctx, cudaGetLastError());
-    rc = launch_verify(ctx, dv, all_slots ? MODE_CACHED : MODE_MIXED, gb.d_ks, gb.d_qx, gb.d_qy, gb.d_e, gb.d_r, gb.d_s, n, gb.d_mask, gb.d_off, st, nullptr, 0, nullptr,
-                       gb.d_idx, classes ? classes : CLASS_GENERIC, gb.d_scal);
+    rc = launch_verify(ctx, dv, all_slots ? MODE_CACHED : MODE_MIXED, gb.d_ks.get(), gb.d_qx.get(), gb.d_qy.get(), gb.d_e.get(), gb.d_r.get(), gb.d_s.get(), n, gb.d_mask.get(), gb.d_off.get(), st, nullptr, 0, nullptr,
+                       gb.d_idx.get(), classes ? classes : CLASS_GENERIC, gb.d_scal.get());
     if (rc) return rc;
-    bdev::bccsp_status_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(gb.d_pre, gb.d_mask, gb.d_off, (uint32_t)n, gb.d_status);
+    bdev::bccsp_status_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(gb.d_pre.get(), gb.d_mask.get(), gb.d_off.get(), (uint32_t)n, gb.d_status.get());
     ctx->launches++;
     CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpyAsync(gb.h_status, gb.d_status, n, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(gb.h_status.get(), gb.d_status.get(), n, cudaMemcpyDeviceToHost, st));
     gb.t_submit = t1; gb.n = n;
     ctx->timing[1] = us(t0, t1);
     return FABGPU_OK;
@@ -1319,9 +1250,9 @@ static int bccsp_device_finish(fabgpu_ctx* ctx, int slot, uint8_t* status)
     };
     auto& gb = ctx->gb[slot];
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
-    CK(ctx, cudaStreamSynchronize(ctx->devs[0].slot[slot].stream));
+    CK(ctx, cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()));
     auto t2 = now();
-    memcpy(status, gb.h_status, gb.n);
+    memcpy(status, gb.h_status.get(), gb.n);
     ctx->timing[2] = us(gb.t_submit, t2); ctx->timing[3] = us(t2, now());
     return FABGPU_OK;
 }
@@ -1432,7 +1363,7 @@ int fabgpu_bccsp_verify_batch_async(fabgpu_ctx* ctx, int slot, const uint8_t* ke
     gb.n = n;
     if (device_gates_apply(ctx, dig_off, sig_off, n)) {
         rc = bccsp_device_submit(ctx, slot, keys_xy, K, key_idx, digests, dig_off, sigs, sig_off, n, slot_of);
-        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream); return rc; }
+        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()); return rc; }
         gb.on_device = true;
     } else {
         // host-gated split (several devices, or FABGPU_BCCSP_HOST_GATES=1): it pipelines internally over both pinned SoA
@@ -1456,7 +1387,7 @@ int fabgpu_bccsp_batch_buffers(fabgpu_ctx* ctx, int slot, size_t n_cap, size_t s
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
     int rc = gate_bufs_reserve(ctx, slot, n_cap, sig_bytes_cap, dig_bytes_cap, (size_t)k_cap);
     if (rc) return rc;
-    *keys_xy = gb.h_keys; *key_idx = gb.h_kidx; *digests = gb.h_digs; *dig_off = gb.h_dig_off; *sigs = gb.h_sigs; *sig_off = gb.h_sig_off;
+    *keys_xy = gb.h_keys.get(); *key_idx = gb.h_kidx.get(); *digests = gb.h_digs.get(); *dig_off = gb.h_dig_off.get(); *sigs = gb.h_sigs.get(); *sig_off = gb.h_sig_off.get();
     return FABGPU_OK;
 }
 
@@ -1467,22 +1398,22 @@ int fabgpu_bccsp_verify_batch_inplace_async(fabgpu_ctx* ctx, int slot, int K, si
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& gb = ctx->gb[slot];
     if (gb.busy) { ctx->last_error = "slot already holds a batch: call fabgpu_bccsp_verify_batch_wait first"; return FABGPU_E_ARG; }
-    if (n > gb.n_cap || (size_t)K > gb.k_cap || !gb.h_sig_off) { ctx->last_error = "batch exceeds the capacities given to fabgpu_bccsp_batch_buffers"; return FABGPU_E_ARG; }
-    if (n && (gb.h_sig_off[0] != 0 || gb.h_dig_off[0] != 0 || gb.h_sig_off[n] > gb.sig_cap || gb.h_dig_off[n] > gb.dig_cap)) {
+    if (n > gb.n_cap() || (size_t)K > gb.k_cap() || !gb.h_sig_off.get()) { ctx->last_error = "batch exceeds the capacities given to fabgpu_bccsp_batch_buffers"; return FABGPU_E_ARG; }
+    if (n && (gb.h_sig_off.get()[0] != 0 || gb.h_dig_off.get()[0] != 0 || gb.h_sig_off.get()[n] > gb.sig_cap() || gb.h_dig_off.get()[n] > gb.dig_cap())) {
         ctx->last_error = "offset tables must start at 0 and stay inside the buffers"; return FABGPU_E_ARG;
     }
-    if (!device_gates_apply(ctx, gb.h_dig_off, gb.h_sig_off, n) && n) { ctx->last_error = "the in-place batch form needs the device gates"; return FABGPU_E_ARG; }
+    if (!device_gates_apply(ctx, gb.h_dig_off.get(), gb.h_sig_off.get(), n) && n) { ctx->last_error = "the in-place batch form needs the device gates"; return FABGPU_E_ARG; }
     auto t_start = std::chrono::steady_clock::now();
     ctx->timing[0] = ctx->timing[1] = ctx->timing[2] = ctx->timing[3] = 0;
     std::vector<int32_t> slot_of;
-    int rc = resolve_key_tables(ctx, gb.h_keys, K, gb.h_kidx, n, slot_of);
+    int rc = resolve_key_tables(ctx, gb.h_keys.get(), K, gb.h_kidx.get(), n, slot_of);
     if (rc) return rc;
     ctx->timing[0] = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t_start).count();
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
     gb.n = n;
     if (n) {
-        rc = bccsp_device_submit(ctx, slot, gb.h_keys, K, gb.h_kidx, gb.h_digs, gb.h_dig_off, gb.h_sigs, gb.h_sig_off, n, slot_of, true);
-        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream); return rc; }
+        rc = bccsp_device_submit(ctx, slot, gb.h_keys.get(), K, gb.h_kidx.get(), gb.h_digs.get(), gb.h_dig_off.get(), gb.h_sigs.get(), gb.h_sig_off.get(), n, slot_of, true);
+        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()); return rc; }
         gb.on_device = true;
     } else { gb.done_status.clear(); gb.on_device = false; }
     gb.busy = true;
@@ -1535,7 +1466,7 @@ int fabgpu_bccsp_verify_batch(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, co
                 int rc2 = bccsp_device_finish(ctx, c, status + lo[c]);
                 if (!rc) rc = rc2;
             }
-            if (rc && submitted < FABGPU_SLOTS) cudaStreamSynchronize(ctx->devs[0].slot[submitted].stream);   // a submit that failed half-way
+            if (rc && submitted < FABGPU_SLOTS) cudaStreamSynchronize(ctx->devs[0].slot[submitted].stream.get());   // a submit that failed half-way
             return rc;
         }
     }
@@ -1577,8 +1508,8 @@ static int bccsp_batch_hostgated(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K,
             const size_t lo = cnt * (size_t)tid / T, hi = cnt * (size_t)(tid + 1) / T;
             for (size_t k = lo; k < hi; k++) {
                 if (status[base + k] != FABGPU_ST_VALID) continue;          // decided by a gate
-                const bool ok = (hsl.h_mask[k >> 5] >> (k & 31)) & 1u;
-                const bool oc = (hsl.h_off[k >> 5] >> (k & 31)) & 1u;
+                const bool ok = (hsl.h_mask.get()[k >> 5] >> (k & 31)) & 1u;
+                const bool oc = (hsl.h_off.get()[k >> 5] >> (k & 31)) & 1u;
                 status[base + k] = ok ? FABGPU_ST_VALID : (oc ? FABGPU_ST_ERR_OFF_CURVE : FABGPU_ST_INVALID);
             }
         });
@@ -1616,16 +1547,16 @@ static int bccsp_batch_hostgated(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K,
                         host::hash_to_e(digests + dig_off[i], dl, ebuf);
                         // Qx / Qy are staged even for keys with a table: the handle is resolved again at enqueue time and, had
                         // the slot been recycled by then, the generic kernel verifies against these (never against stale bytes)
-                        stage32(hs.h_in[0] + 32 * k, keys_xy + 64 * (size_t)ki);
-                        stage32(hs.h_in[1] + 32 * k, keys_xy + 64 * (size_t)ki + 32);
-                        stage32(hs.h_in[2] + 32 * k, ebuf);
-                        stage32(hs.h_in[3] + 32 * k, g.r);
-                        stage32(hs.h_in[4] + 32 * k, g.s);
+                        stage32(hs.h_in[0].get() + 32 * k, keys_xy + 64 * (size_t)ki);
+                        stage32(hs.h_in[1].get() + 32 * k, keys_xy + 64 * (size_t)ki + 32);
+                        stage32(hs.h_in[2].get() + 32 * k, ebuf);
+                        stage32(hs.h_in[3].get() + 32 * k, g.r);
+                        stage32(hs.h_in[4].get() + 32 * k, g.s);
                         mine++;
                     }
                 }
-                if (st != FABGPU_ST_VALID) { stage32(hs.h_in[3] + 32 * k, kZero32); stage32(hs.h_in[4] + 32 * k, kZero32); }
-                stage_i32(hs.h_key_slot + k, (st == FABGPU_ST_VALID) ? slot_of[ki] : -1);
+                if (st != FABGPU_ST_VALID) { stage32(hs.h_in[3].get() + 32 * k, kZero32); stage32(hs.h_in[4].get() + 32 * k, kZero32); }
+                stage_i32(hs.h_key_slot.get() + k, (st == FABGPU_ST_VALID) ? slot_of[ki] : -1);
                 status[i] = st;
             }
             stage_fence();
@@ -1699,10 +1630,7 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
     auto& dm = ctx->dm;
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
     // blocks already enqueued on a slot were launched with the OLD tables (passed by value): let them finish before those go away
-    for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream));
-    void* old[] = {dm.id_blob, dm.valid, dm.keys_xy, dm.channel, dm.id_off, dm.key_slot, dm.msp_code, dm.ht_idx, dm.nodes, dm.principal_code, dm.ht_hash,
-                   dm.group, dm.ns_blob, dm.ns_off, dm.ns_root, dm.pbits};
-    for (void* p : old) if (p) cudaFree(p);
+    for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
     dm = fabgpu_ctx::DevMsp();
     // MSP-id codes: equal strings <=> equal codes, shared between identities and policy principals
     std::unordered_map<std::string, int32_t> codes;
@@ -1728,25 +1656,18 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
             if (raw_slot[i] < 0) { dm.all_slots = false; dm.classes |= raw_slot[i] == -1 ? CLASS_GENERIC : CLASS_SMALL; }
         }
     }
-    auto up = [&](auto*& dst, const void* src, size_t bytes) -> int {
-        CK(ctx, cudaMalloc(&dst, bytes + 8));                 // slack: word-wise readers may touch the aligned word past the end
-        if (bytes) CK(ctx, cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+    auto up = [&](auto& dst, const void* src, size_t bytes) -> int {
+        if (int rc = dst.reserve(ctx, bytes + 8)) return rc;   // slack: word-wise readers may touch the aligned word past the end
+        if (bytes) CK(ctx, cudaMemcpy(dst.get(), src, bytes, cudaMemcpyHostToDevice));
         return FABGPU_OK;
     };
     const size_t blob_len = n_ids ? id_off[n_ids] : 0;
-    int rc = 0;
-    rc |= up(dm.id_blob, id_blob, blob_len);
-    rc |= up(dm.id_off, id_off, 4 * (size_t)(n_ids + 1) * (n_ids ? 1 : 0));
-    rc |= up(dm.valid, valid, (size_t)n_ids);
-    rc |= up(dm.keys_xy, keys_xy, 64 * (size_t)n_ids);
-    rc |= up(dm.key_slot, raw_slot.data(), 4 * (size_t)n_ids);
-    rc |= up(dm.msp_code, msp_code.data(), 4 * (size_t)n_ids);
-    rc |= up(dm.ht_hash, hh.data(), 8 * (size_t)hsz);
-    rc |= up(dm.ht_idx, hi.data(), 4 * (size_t)hsz);
-    rc |= up(dm.nodes, policy_nodes, 16 * (size_t)n_nodes);
-    rc |= up(dm.principal_code, pcode.data(), 4 * ctx->principals.size());
-    rc |= up(dm.channel, ctx->channel.data(), ctx->channel.size());
-    if (rc) return FABGPU_E_CUDA;
+    if (up(dm.id_blob, id_blob, blob_len) || up(dm.id_off, id_off, 4 * (size_t)(n_ids + 1) * (n_ids ? 1 : 0)) || up(dm.valid, valid, (size_t)n_ids) ||
+        up(dm.keys_xy, keys_xy, 64 * (size_t)n_ids) || up(dm.key_slot, raw_slot.data(), 4 * (size_t)n_ids) ||
+        up(dm.msp_code, msp_code.data(), 4 * (size_t)n_ids) || up(dm.ht_hash, hh.data(), 8 * (size_t)hsz) || up(dm.ht_idx, hi.data(), 4 * (size_t)hsz) ||
+        up(dm.nodes, policy_nodes, 16 * (size_t)n_nodes) || up(dm.principal_code, pcode.data(), 4 * ctx->principals.size()) ||
+        up(dm.channel, ctx->channel.data(), ctx->channel.size()))
+        return FABGPU_E_CUDA;
     dm.ht_size = n_ids ? hsz : 0; dm.n_ids = n_ids; dm.n_nodes = n_nodes; dm.n_principals = (int32_t)ctx->principals.size();
     dm.channel_len = (uint32_t)ctx->channel.size();
     return FABGPU_OK;
@@ -1862,7 +1783,7 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
 static int drain_block_streams(fabgpu_ctx* ctx)
 {
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
-    for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream));
+    for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
     return FABGPU_OK;
 }
 
@@ -1873,10 +1794,10 @@ int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids)
     auto& dm = ctx->dm;
     if (n_ids != dm.n_ids) { ctx->last_error = "group table does not match the identities given to fabgpu_msp_configure"; return FABGPU_E_ARG; }
     int rc = drain_block_streams(ctx); if (rc) return rc;
-    if (dm.group) { cudaFree(dm.group); dm.group = nullptr; }
+    dm.group = {};
     if (n_ids == 0) return FABGPU_OK;
-    CK(ctx, cudaMalloc(&dm.group, 4 * (size_t)n_ids));
-    CK(ctx, cudaMemcpy(dm.group, group, 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
+    if ((rc = dm.group.reserve(ctx, 4 * (size_t)n_ids))) return rc;
+    CK(ctx, cudaMemcpy(dm.group.get(), group, 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
     return FABGPU_OK;
 }
 
@@ -1890,13 +1811,12 @@ int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, 
         return FABGPU_E_ARG;
     }
     int rc = drain_block_streams(ctx); if (rc) return rc;
-    if (dm.pbits) { cudaFree(dm.pbits); dm.pbits = nullptr; }
-    dm.pbits_words = 0;
+    dm.pbits = {}; dm.pbits_words = 0;
     if (n_ids == 0) return FABGPU_OK;
     const int W = (n_principals + 31) / 32;
     const size_t bytes = 4 * (size_t)n_ids * W;
-    CK(ctx, cudaMalloc(&dm.pbits, bytes + 8));                 // non-null even with no principals: it selects the bit test
-    if (bytes) CK(ctx, cudaMemcpy(dm.pbits, bits, bytes, cudaMemcpyHostToDevice));
+    if ((rc = dm.pbits.reserve(ctx, bytes + 8))) return rc;     // non-null even with no principals: it selects the bit test
+    if (bytes) CK(ctx, cudaMemcpy(dm.pbits.get(), bits, bytes, cudaMemcpyHostToDevice));
     dm.pbits_words = W;
     return FABGPU_OK;
 }
@@ -1909,17 +1829,15 @@ int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uin
     for (int i = 0; i < n_ns; i++)
         if (ns_root[i] < 0 || ns_root[i] >= dm.n_nodes || ns_off[i] > ns_off[i + 1]) { ctx->last_error = "namespace policy root out of range"; return FABGPU_E_ARG; }
     int rc = drain_block_streams(ctx); if (rc) return rc;
-    void* old[] = {dm.ns_blob, dm.ns_off, dm.ns_root};
-    for (void* p : old) if (p) cudaFree(p);
-    dm.ns_blob = nullptr; dm.ns_off = nullptr; dm.ns_root = nullptr; dm.n_ns = 0;
+    dm.ns_blob = {}; dm.ns_off = {}; dm.ns_root = {}; dm.n_ns = 0;
     if (n_ns == 0) return FABGPU_OK;
     const size_t bl = ns_off[n_ns];
-    CK(ctx, cudaMalloc(&dm.ns_blob, bl + 8));
-    if (bl) CK(ctx, cudaMemcpy(dm.ns_blob, ns_blob, bl, cudaMemcpyHostToDevice));
-    CK(ctx, cudaMalloc(&dm.ns_off, 4 * (size_t)(n_ns + 1)));
-    CK(ctx, cudaMemcpy(dm.ns_off, ns_off, 4 * (size_t)(n_ns + 1), cudaMemcpyHostToDevice));
-    CK(ctx, cudaMalloc(&dm.ns_root, 4 * (size_t)n_ns));
-    CK(ctx, cudaMemcpy(dm.ns_root, ns_root, 4 * (size_t)n_ns, cudaMemcpyHostToDevice));
+    if ((rc = dm.ns_blob.reserve(ctx, bl + 8))) return rc;
+    if (bl) CK(ctx, cudaMemcpy(dm.ns_blob.get(), ns_blob, bl, cudaMemcpyHostToDevice));
+    if ((rc = dm.ns_off.reserve(ctx, 4 * (size_t)(n_ns + 1)))) return rc;
+    CK(ctx, cudaMemcpy(dm.ns_off.get(), ns_off, 4 * (size_t)(n_ns + 1), cudaMemcpyHostToDevice));
+    if ((rc = dm.ns_root.reserve(ctx, 4 * (size_t)n_ns))) return rc;
+    CK(ctx, cudaMemcpy(dm.ns_root.get(), ns_root, 4 * (size_t)n_ns, cudaMemcpyHostToDevice));
     dm.n_ns = n_ns;
     return FABGPU_OK;
 }
@@ -1930,11 +1848,9 @@ int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** 
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     auto& bb = ctx->bbs[slot];
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
-    if (bytes > bb.h_block_cap) {
-        if (ctx->dbs[slot].busy) { ctx->last_error = "slot holds a block in flight"; return FABGPU_E_ARG; }
-        int rc = grow_host(ctx, bb.h_block, bytes); if (rc) return rc; bb.h_block_cap = bytes;
-    }
-    *out = bb.h_block;
+    if (bytes > bb.h_block.bytes() && ctx->dbs[slot].busy) { ctx->last_error = "slot holds a block in flight"; return FABGPU_E_ARG; }
+    if (int rc = bb.h_block.reserve(ctx, bytes)) return rc;
+    *out = bb.h_block.get();
     return FABGPU_OK;
 }
 int fabgpu_block_buffer(fabgpu_ctx* ctx, size_t bytes, uint8_t** out) { return fabgpu_block_buffer_slot(ctx, 0, bytes, out); }
@@ -1981,21 +1897,17 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
                 }
             }
             // submitters are serialised by slot0_mu; blocks in flight on the other slots still read dm.key_slot: let them finish first
-            for (auto& dsx : dv.slot) CK(ctx, cudaStreamSynchronize(dsx.stream));
-            CK(ctx, cudaMemcpy(dm.key_slot, raw.data(), 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
+            for (auto& dsx : dv.slot) CK(ctx, cudaStreamSynchronize(dsx.stream.get()));
+            CK(ctx, cudaMemcpy(dm.key_slot.get(), raw.data(), 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
         }
     }
-    if (block_len > bb.block_cap) {
-        const size_t want = block_len + (block_len >> 2);
-        bb.block_cap = 0;                                   // a failed grow leaves no buffer: do not remember the old capacity
-        int rc = grow_dev(ctx, bb.d_block, want + 64);      // slack: word-wise readers (bytes_equal, the SHA loader) touch the aligned words past the end
-        if (rc) return rc;
-        bb.block_cap = want;
-    }
+    // slack: word-wise readers (bytes_equal, the SHA loader) touch the aligned words past the end.  An empty block needs no buffer.
+    if (block_len && block_len + 64 > bb.d_block.bytes())
+        if (int rc = bb.d_block.reserve(ctx, block_len + (block_len >> 2) + 64)) return rc;
     const char* evs = getenv("FABGPU_BLOCK_EVENTS");          // "1": time the device stages with CUDA events (diagnostics)
     db.use_ev = evs && evs[0] == '1';
-    if (db.use_ev) for (auto& e : db.ev) if (!e) CK(ctx, cudaEventCreate(&e));
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[0], ds.stream));
+    if (db.use_ev) for (auto& e : db.ev) if (!e) { cudaEvent_t ev = nullptr; CK(ctx, cudaEventCreate(&ev)); e.reset(ev); }
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[0].get(), ds.stream.get()));
     std::vector<uint32_t> split;
     if (!env_off) {                                           // serialized common.Block: find the envelopes (serial, length-prefixed)
         std::vector<blockval::Seg> envs;
@@ -2008,71 +1920,69 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     db.T = T; db.block = block;
     if (T == 0) return FABGPU_OK;
     const size_t J_cap = T * (1 + BD_ENDS_HINT);
-    if (T > db.tx_cap) {
+    if (T > db.tx_cap()) {
         const size_t tc = T + (T >> 2) + 256, jc = tc * (1 + BD_ENDS_HINT);
-        int rc = 0;
-        db.tx_cap = 0; db.j_cap = 0;                        // reset first: after a partial failure the pointers are gone
-        rc |= grow_dev(ctx, db.d_env_off, 8 * (tc + 1)); rc |= grow_dev(ctx, db.d_txs, sizeof(bdev::TxDev) * tc);
-        rc |= grow_dev(ctx, db.d_raw, sizeof(bdev::RawJob) * jc);
-        rc |= grow_dev(ctx, db.d_sha, sizeof(bdev::ShaJobD) * (jc + 2 * tc)); rc |= grow_dev(ctx, db.d_dig, 32 * (jc + 2 * tc) + 64);
-        rc |= grow_dev(ctx, db.d_r, 32 * jc); rc |= grow_dev(ctx, db.d_s, 32 * jc); rc |= grow_dev(ctx, db.d_qx, 32 * jc); rc |= grow_dev(ctx, db.d_qy, 32 * jc);
-        rc |= grow_dev(ctx, db.d_gate, jc); rc |= grow_dev(ctx, db.d_ks, 4 * jc); rc |= grow_dev(ctx, db.d_ident, 4 * jc);
-        rc |= grow_dev(ctx, db.d_mask, jc / 8 + 8); rc |= grow_dev(ctx, db.d_off, jc / 8 + 8); rc |= grow_dev(ctx, db.d_counter, 16); rc |= grow_dev(ctx, db.d_idx, 4 * (jc + 2));
-        rc |= grow_dev(ctx, db.d_scal, 64 * jc);
-        rc |= grow_dev(ctx, db.d_flags, tc); rc |= grow_dev(ctx, db.d_hash, 8 * tc); rc |= grow_dev(ctx, db.d_seg, 8 * tc);
-        rc |= grow_host(ctx, db.h_flags, tc); rc |= grow_host(ctx, db.h_hash, 8 * tc); rc |= grow_host(ctx, db.h_seg, 8 * tc);
-        rc |= grow_host(ctx, db.h_counter, 16); rc |= grow_host(ctx, db.h_env_off, 8 * (tc + 1));
-        if (rc) return FABGPU_E_CUDA;
-        db.tx_cap = tc; db.j_cap = jc;
+        Grow grow{ctx};
+        grow(db.d_env_off, 8 * (tc + 1)); grow(db.d_txs, sizeof(bdev::TxDev) * tc);
+        grow(db.d_raw, sizeof(bdev::RawJob) * jc);
+        grow(db.d_sha, sizeof(bdev::ShaJobD) * (jc + 2 * tc)); grow(db.d_dig, 32 * (jc + 2 * tc) + 64);
+        grow(db.d_r, 32 * jc); grow(db.d_s, 32 * jc); grow(db.d_qx, 32 * jc); grow(db.d_qy, 32 * jc);
+        grow(db.d_gate, jc); grow(db.d_ks, 4 * jc); grow(db.d_ident, 4 * jc);
+        grow(db.d_mask, jc / 8 + 8); grow(db.d_off, jc / 8 + 8); grow(db.d_counter, 16); grow(db.d_idx, 4 * (jc + 2));
+        grow(db.d_scal, 64 * jc);
+        grow(db.d_flags, tc); grow(db.d_hash, 8 * tc); grow(db.d_seg, 8 * tc);
+        grow(db.h_hash, 8 * tc); grow(db.h_seg, 8 * tc); grow(db.h_counter, 16); grow(db.h_env_off, 8 * (tc + 1));
+        grow(db.h_flags, tc);
+        if (grow.rc) return grow.rc;
     }
     // envelope table on the device: pairs (begin, end) so that both entry points share one kernel
     for (size_t i = 0; i < T; i++) {
-        db.h_env_off[2 * i] = env_off ? env_off[i] : split[2 * i];
-        db.h_env_off[2 * i + 1] = env_off ? env_off[i + 1] : split[2 * i + 1];
+        db.h_env_off.get()[2 * i] = env_off ? env_off[i] : split[2 * i];
+        db.h_env_off.get()[2 * i + 1] = env_off ? env_off[i + 1] : split[2 * i + 1];
     }
-    cudaStream_t st = ds.stream;
-    CK(ctx, cudaMemcpyAsync(db.d_env_off, db.h_env_off, 8 * T, cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemsetAsync(db.d_counter, 0, 16, st));
-    bdev::MspDev m; m.id_blob = dm.id_blob; m.id_off = dm.id_off; m.key_slot = dm.key_slot; m.valid = dm.valid; m.msp_code = dm.msp_code; m.group = dm.group;
-    m.keys_xy = dm.keys_xy; m.ht_hash = dm.ht_hash; m.ht_idx = dm.ht_idx; m.ht_size = dm.ht_size; m.n_ids = dm.n_ids;
-    bdev::PolicyDev pol; pol.nodes = dm.nodes; pol.n_nodes = dm.n_nodes; pol.principal_code = dm.principal_code; pol.n_principals = dm.n_principals;
-    pol.ns_blob = dm.ns_blob; pol.ns_off = dm.ns_off; pol.ns_root = dm.ns_root; pol.n_ns = dm.n_ns;
-    pol.principal_bits = dm.pbits; pol.bits_words = dm.pbits_words;
+    cudaStream_t st = ds.stream.get();
+    CK(ctx, cudaMemcpyAsync(db.d_env_off.get(), db.h_env_off.get(), 8 * T, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemsetAsync(db.d_counter.get(), 0, 16, st));
+    bdev::MspDev m; m.id_blob = dm.id_blob.get(); m.id_off = dm.id_off.get(); m.key_slot = dm.key_slot.get(); m.valid = dm.valid.get(); m.msp_code = dm.msp_code.get(); m.group = dm.group.get();
+    m.keys_xy = dm.keys_xy.get(); m.ht_hash = dm.ht_hash.get(); m.ht_idx = dm.ht_idx.get(); m.ht_size = dm.ht_size; m.n_ids = dm.n_ids;
+    bdev::PolicyDev pol; pol.nodes = dm.nodes.get(); pol.n_nodes = dm.n_nodes; pol.principal_code = dm.principal_code.get(); pol.n_principals = dm.n_principals;
+    pol.ns_blob = dm.ns_blob.get(); pol.ns_off = dm.ns_off.get(); pol.ns_root = dm.ns_root.get(); pol.n_ns = dm.n_ns;
+    pol.principal_bits = dm.pbits.get(); pol.bits_words = dm.pbits_words;
     const bool need_q = (dm.classes & CLASS_GENERIC) != 0;   // only the generic arithmetic reads the key itself
-    bdev::JobArrays ja; ja.sha = db.d_sha; ja.r = db.d_r; ja.s = db.d_s; ja.key_slot = db.d_ks; ja.identity = db.d_ident; ja.qx = need_q ? db.d_qx : nullptr;
-    ja.qy = need_q ? db.d_qy : nullptr; ja.gate_ok = db.d_gate; ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T;
+    bdev::JobArrays ja; ja.sha = db.d_sha.get(); ja.r = db.d_r.get(); ja.s = db.d_s.get(); ja.key_slot = db.d_ks.get(); ja.identity = db.d_ident.get(); ja.qx = need_q ? db.d_qx.get() : nullptr;
+    ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T;
     const uint32_t cnt = (uint32_t)T, E_cap = (uint32_t)(J_cap - T);
     // One copy, then the walk.  (Copying in chunks with a walk per chunk was measured slower, the more chunks the slower: hashing a
     // 4.6 KB payload is a long chain of dependent rounds per thread however few
     // threads a launch has, so per-chunk launches serialise that latency.  What hides the copy is the NEXT block's copy running
     // under this block's kernels: the slots.)
-    CK(ctx, cudaMemcpyAsync(bb.d_block, block, block_len, cudaMemcpyHostToDevice, st));
-    bdev::block_walk_kernel<<<(cnt + 31) / 32, 32, 0, st>>>(bb.d_block, db.d_env_off, 0u, cnt, cnt, dm.channel, dm.channel_len, db.d_txs, db.d_raw, ja, db.d_counter);
-    bdev::block_resolve_kernel<<<(cnt + 63) / 64, 64, 0, st>>>(bb.d_block, db.d_raw, 0u, cnt, m, ja, db.d_txs);                      // creator jobs
-    sha256_segments_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block, reinterpret_cast<const ShaJob*>(db.d_sha), cnt, db.d_dig);
-    sha256_segments_kernel<<<(2 * cnt + 127) / 128, 128, 0, st>>>(bb.d_block, reinterpret_cast<const ShaJob*>(db.d_sha + J_cap), 2 * cnt, db.d_dig + 32 * J_cap);
+    CK(ctx, cudaMemcpyAsync(bb.d_block.get(), block, block_len, cudaMemcpyHostToDevice, st));
+    bdev::block_walk_kernel<<<(cnt + 31) / 32, 32, 0, st>>>(bb.d_block.get(), db.d_env_off.get(), 0u, cnt, cnt, dm.channel.get(), dm.channel_len, db.d_txs.get(), db.d_raw.get(), ja, db.d_counter.get());
+    bdev::block_resolve_kernel<<<(cnt + 63) / 64, 64, 0, st>>>(bb.d_block.get(), db.d_raw.get(), 0u, cnt, m, ja, db.d_txs.get());                      // creator jobs
+    sha256_segments_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), reinterpret_cast<const ShaJob*>(db.d_sha.get()), cnt, db.d_dig.get());
+    sha256_segments_kernel<<<(2 * cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), reinterpret_cast<const ShaJob*>(db.d_sha.get() + J_cap), 2 * cnt, db.d_dig.get() + 32 * J_cap);
     ctx->launches += 4;
     CK(ctx, cudaGetLastError());
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[1], st));
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[2], st));
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[1].get(), st));
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[2].get(), st));
     // endorsement jobs [T, T + *d_counter): launches sized for the worst case, the kernels stop at the device-side count
-    bdev::block_resolve_kernel<<<(E_cap + 63) / 64, 64, 0, st>>>(bb.d_block, db.d_raw, cnt, E_cap, m, ja, db.d_txs, db.d_counter);
-    sha256_segments_kernel<<<(E_cap + 127) / 128, 128, 0, st>>>(bb.d_block, reinterpret_cast<const ShaJob*>(db.d_sha) + T, E_cap, db.d_dig + 32 * T, db.d_counter);
+    bdev::block_resolve_kernel<<<(E_cap + 63) / 64, 64, 0, st>>>(bb.d_block.get(), db.d_raw.get(), cnt, E_cap, m, ja, db.d_txs.get(), db.d_counter.get());
+    sha256_segments_kernel<<<(E_cap + 127) / 128, 128, 0, st>>>(bb.d_block.get(), reinterpret_cast<const ShaJob*>(db.d_sha.get()) + T, E_cap, db.d_dig.get() + 32 * T, db.d_counter.get());
     ctx->launches += 2;
     CK(ctx, cudaGetLastError());
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[3], st));
-    int rc = launch_verify(ctx, dv, dm.all_slots ? MODE_CACHED : MODE_MIXED, db.d_ks, db.d_qx, db.d_qy, db.d_dig, db.d_r, db.d_s, J_cap, db.d_mask, db.d_off, st,
-                           db.d_counter, cnt, nullptr, db.d_idx, dm.classes ? dm.classes : CLASS_GENERIC, db.d_scal);
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[3].get(), st));
+    int rc = launch_verify(ctx, dv, dm.all_slots ? MODE_CACHED : MODE_MIXED, db.d_ks.get(), db.d_qx.get(), db.d_qy.get(), db.d_dig.get(), db.d_r.get(), db.d_s.get(), J_cap, db.d_mask.get(), db.d_off.get(), st,
+                           db.d_counter.get(), cnt, nullptr, db.d_idx.get(), dm.classes ? dm.classes : CLASS_GENERIC, db.d_scal.get());
     if (rc) return rc;
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4], st));
-    bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block, db.d_txs, cnt, m, pol, db.d_mask, db.d_gate, db.d_ident, db.d_dig, (uint32_t)J_cap, db.d_flags,
-                                                               db.d_hash, db.d_seg);
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4].get(), st));
+    bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), db.d_txs.get(), cnt, m, pol, db.d_mask.get(), db.d_gate.get(), db.d_ident.get(), db.d_dig.get(), (uint32_t)J_cap, db.d_flags.get(),
+                                                               db.d_hash.get(), db.d_seg.get());
     ctx->launches++;
     CK(ctx, cudaGetLastError());
-    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[5], st));
-    CK(ctx, cudaMemcpyAsync(db.h_flags, db.d_flags, T, cudaMemcpyDeviceToHost, st));
-    CK(ctx, cudaMemcpyAsync(db.h_hash, db.d_hash, 8 * T, cudaMemcpyDeviceToHost, st));
-    CK(ctx, cudaMemcpyAsync(db.h_seg, db.d_seg, 8 * T, cudaMemcpyDeviceToHost, st));
+    if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[5].get(), st));
+    CK(ctx, cudaMemcpyAsync(db.h_flags.get(), db.d_flags.get(), T, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(db.h_hash.get(), db.d_hash.get(), 8 * T, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(db.h_seg.get(), db.d_seg.get(), 8 * T, cudaMemcpyDeviceToHost, st));
     db.t1 = now();
     return FABGPU_OK;
 }
@@ -2089,10 +1999,10 @@ static int block_finish(fabgpu_ctx* ctx, int slot, uint8_t* flags)
     const size_t T = db.T;
     const uint8_t* block = db.block;
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
-    CK(ctx, cudaStreamSynchronize(ctx->devs[0].slot[slot].stream));
+    CK(ctx, cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()));
     auto t3 = now();
     if (T == 0) return FABGPU_OK;
-    memcpy(flags, db.h_flags, T);
+    memcpy(flags, db.h_flags.get(), T);
     {
         // flat open-addressing table keyed by the 64-bit tx-id hash (0 = empty); equal hashes are confirmed on the bytes
         size_t cap = 16; while (cap < 4 * T) cap <<= 1;
@@ -2100,14 +2010,14 @@ static int block_finish(fabgpu_ctx* ctx, int slot, uint8_t* flags)
         uint64_t* keys = db.dup_keys.data(); uint32_t* idx = db.dup_idx.data();
         for (size_t t = 0; t < T; t++) {
             if (flags[t] != blockval::TX_VALID) continue;
-            const bdev::Seg id = db.h_seg[t];
-            const uint64_t h = db.h_hash[t] ? db.h_hash[t] : 1;
+            const bdev::Seg id = db.h_seg.get()[t];
+            const uint64_t h = db.h_hash.get()[t] ? db.h_hash.get()[t] : 1;
             bool dup = false;
             size_t pos = (size_t)h & (cap - 1);
             for (;; pos = (pos + 1) & (cap - 1)) {
                 if (keys[pos] == 0) break;
                 if (keys[pos] != h) continue;
-                const bdev::Seg o = db.h_seg[idx[pos]];
+                const bdev::Seg o = db.h_seg.get()[idx[pos]];
                 if (o.len == id.len && memcmp(block + o.off, block + id.off, id.len) == 0) { dup = true; break; }
             }
             if (dup) flags[t] = blockval::TX_DUPLICATE_TXID;
@@ -2117,7 +2027,7 @@ static int block_finish(fabgpu_ctx* ctx, int slot, uint8_t* flags)
     auto t4 = now();
     ctx->block_timing[0] = us(db.t0, db.t1); ctx->block_timing[1] = 0; ctx->block_timing[2] = us(db.t1, t3); ctx->block_timing[3] = us(t3, t4);
     ctx->block_timing[4] = us(db.t0, t4);
-    for (int k = 0; k < 5; k++) { float ms = 0; if (db.use_ev) cudaEventElapsedTime(&ms, db.ev[k], db.ev[k + 1]); ctx->block_timing[5 + k] = 1e3 * ms; }
+    for (int k = 0; k < 5; k++) { float ms = 0; if (db.use_ev) cudaEventElapsedTime(&ms, db.ev[k].get(), db.ev[k + 1].get()); ctx->block_timing[5 + k] = 1e3 * ms; }
     return FABGPU_OK;
 }
 
@@ -2139,7 +2049,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
     {
         std::lock_guard<std::mutex> lk0(ctx->slot0_mu);      // key-cache / MSP state: one submitter at a time
         rc = block_submit(ctx, slot, block, block_len, env_off, n_env);
-        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream); return rc; }
+        if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()); return rc; }
         db.on_device = true;
     }
     db.busy = true;
@@ -2159,7 +2069,7 @@ int fabgpu_validate_envelopes_async(fabgpu_ctx* ctx, int slot, const uint8_t* bl
         std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
         auto& db = ctx->dbs[slot];
         if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-        db.T = 0; db.on_device = false; db.done_flags.clear(); db.busy = true;
+        db.T = 0; db.on_device = false; db.busy = true;
         return FABGPU_OK;
     }
     return validate_submit(ctx, slot, blob, env_off[n_env], env_off, n_env);
@@ -2174,13 +2084,12 @@ int fabgpu_validate_wait(fabgpu_ctx* ctx, int slot, uint8_t* flags, size_t flags
     db.busy = false;
     *n_tx_out = db.T;
     if (db.T > flags_cap || (db.T && !flags)) {
-        if (db.on_device) cudaStreamSynchronize(ctx->devs[0].slot[slot].stream);
+        if (db.on_device) cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get());
         ctx->last_error = "flags buffer too small";
         return FABGPU_E_ARG;
     }
     if (db.on_device) return block_finish(ctx, slot, flags);
-    if (db.T) memcpy(flags, db.done_flags.data(), db.T);
-    return FABGPU_OK;
+    return FABGPU_OK;                                         // an empty envelope list: nothing ran
 }
 
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out)
@@ -2216,17 +2125,18 @@ int fabgpu_sha256_segments(fabgpu_ctx* ctx, const uint8_t* buf, size_t buf_len, 
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     Device& dv = ctx->devs[0];
     CK(ctx, cudaSetDevice(dv.id));
-    uint8_t *d_buf = nullptr, *d_dig = nullptr; ShaJob* d_jobs = nullptr;
-    CK(ctx, cudaMalloc(&d_buf, buf_len ? buf_len : 1)); CK(ctx, cudaMalloc(&d_jobs, sizeof(ShaJob) * (n ? n : 1))); CK(ctx, cudaMalloc(&d_dig, 32 * (n ? n : 1)));
-    CK(ctx, cudaMemcpy(d_buf, buf, buf_len, cudaMemcpyHostToDevice));
-    CK(ctx, cudaMemcpy(d_jobs, jobs, sizeof(ShaJob) * n, cudaMemcpyHostToDevice));
+    DevArray<uint8_t> d_buf, d_dig; DevArray<ShaJob> d_jobs;
+    Grow grow{ctx};
+    grow(d_buf, buf_len ? buf_len : 1); grow(d_jobs, sizeof(ShaJob) * (n ? n : 1)); grow(d_dig, 32 * (n ? n : 1));
+    if (grow.rc) return grow.rc;
+    CK(ctx, cudaMemcpy(d_buf.get(), buf, buf_len, cudaMemcpyHostToDevice));
+    CK(ctx, cudaMemcpy(d_jobs.get(), jobs, sizeof(ShaJob) * n, cudaMemcpyHostToDevice));
     if (n) {
-        sha256_segments_kernel<<<(unsigned)((n + 127) / 128), 128>>>(d_buf, d_jobs, (uint32_t)n, d_dig);
+        sha256_segments_kernel<<<(unsigned)((n + 127) / 128), 128>>>(d_buf.get(), d_jobs.get(), (uint32_t)n, d_dig.get());
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
-    CK(ctx, cudaMemcpy(digests, d_dig, 32 * n, cudaMemcpyDeviceToHost));
-    cudaFree(d_buf); cudaFree(d_jobs); cudaFree(d_dig);
+    CK(ctx, cudaMemcpy(digests, d_dig.get(), 32 * n, cudaMemcpyDeviceToHost));
     return FABGPU_OK;
 }
 
@@ -2236,15 +2146,16 @@ int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t
     std::lock_guard<std::mutex> lk(ctx->mu);
     Device& dv = ctx->devs[0];
     CK(ctx, cudaSetDevice(dv.id));
-    uint8_t *da = nullptr, *db = nullptr, *dout = nullptr;
-    CK(ctx, cudaMalloc(&da, 32 * n)); CK(ctx, cudaMalloc(&db, 32 * n)); CK(ctx, cudaMalloc(&dout, 32 * n));
-    CK(ctx, cudaMemcpy(da, a, 32 * n, cudaMemcpyHostToDevice));
-    CK(ctx, cudaMemcpy(db, b, 32 * n, cudaMemcpyHostToDevice));
-    fieldop_kernel<<<(unsigned)((n + 63) / 64), 64>>>(op, da, db, (int)n, dout);
+    DevArray<uint8_t> da, db, dout;
+    Grow grow{ctx};
+    grow(da, 32 * n); grow(db, 32 * n); grow(dout, 32 * n);
+    if (grow.rc) return grow.rc;
+    CK(ctx, cudaMemcpy(da.get(), a, 32 * n, cudaMemcpyHostToDevice));
+    CK(ctx, cudaMemcpy(db.get(), b, 32 * n, cudaMemcpyHostToDevice));
+    fieldop_kernel<<<(unsigned)((n + 63) / 64), 64>>>(op, da.get(), db.get(), (int)n, dout.get());
     ctx->launches++;
     CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dout, 32 * n, cudaMemcpyDeviceToHost));
-    cudaFree(da); cudaFree(db); cudaFree(dout);
+    CK(ctx, cudaMemcpy(out, dout.get(), 32 * n, cudaMemcpyDeviceToHost));
     return FABGPU_OK;
 }
 
@@ -2257,15 +2168,16 @@ int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* win
     if (n == 0) return FABGPU_OK;
     Device& dv = ctx->devs[0];
     CK(ctx, cudaSetDevice(dv.id));
-    const aff* tab = key_slot < 0 ? dv.gtab : dv.qtab + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES;
-    uint32_t *d_w = nullptr, *d_d = nullptr; aff* d_out = nullptr;
-    CK(ctx, cudaMalloc(&d_w, 4 * n)); CK(ctx, cudaMalloc(&d_d, 4 * n)); CK(ctx, cudaMalloc(&d_out, sizeof(aff) * n));
-    CK(ctx, cudaMemcpy(d_w, window, 4 * n, cudaMemcpyHostToDevice));
-    CK(ctx, cudaMemcpy(d_d, digit, 4 * n, cudaMemcpyHostToDevice));
-    table_entries_kernel<<<(unsigned)((n + 127) / 128), 128>>>(tab, wbits, d_w, d_d, (uint32_t)n, d_out);
+    const aff* tab = key_slot < 0 ? dv.gtab.get() : dv.qtab.get() + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES;
+    DevArray<uint32_t> d_w, d_d; DevArray<aff> d_out;
+    Grow grow{ctx};
+    grow(d_w, 4 * n); grow(d_d, 4 * n); grow(d_out, sizeof(aff) * n);
+    if (grow.rc) return grow.rc;
+    CK(ctx, cudaMemcpy(d_w.get(), window, 4 * n, cudaMemcpyHostToDevice));
+    CK(ctx, cudaMemcpy(d_d.get(), digit, 4 * n, cudaMemcpyHostToDevice));
+    table_entries_kernel<<<(unsigned)((n + 127) / 128), 128>>>(tab, wbits, d_w.get(), d_d.get(), (uint32_t)n, d_out.get());
     CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, d_out, sizeof(aff) * n, cudaMemcpyDeviceToHost));
-    cudaFree(d_w); cudaFree(d_d); cudaFree(d_out);
+    CK(ctx, cudaMemcpy(out, d_out.get(), sizeof(aff) * n, cudaMemcpyDeviceToHost));
     return FABGPU_OK;
 }
 
