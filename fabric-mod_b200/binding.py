@@ -24,7 +24,7 @@ EXPORTS = [
     "fabgpu_verify_p256_keyed_async", "fabgpu_verify_p256_device_keyed", "fabgpu_last_timing", "fabgpu_build_info",
     "fabgpu_msp_configure", "fabgpu_validate_block", "fabgpu_validate_envelopes", "fabgpu_block_buffer", "fabgpu_block_timing", "fabgpu_sha256_segments",
     "fabgpu_bccsp_verify_batch_async", "fabgpu_bccsp_verify_batch_wait", "fabgpu_bccsp_batch_buffers", "fabgpu_bccsp_verify_batch_inplace_async",
-    "fabgpu_msp_identity_groups", "fabgpu_namespace_policies", "fabgpu_msp_principal_bits",
+    "fabgpu_msp_identity_groups", "fabgpu_namespace_policies", "fabgpu_msp_principal_bits", "fabgpu_collection_policies",
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
@@ -70,6 +70,14 @@ def lib():
 
 def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+
+
+def _blob(items):
+    """byte strings -> (their concatenation, never empty, as uint8; the len(items) + 1 offsets as uint32)"""
+    off = np.zeros(len(items) + 1, np.uint32)
+    off[1:] = np.cumsum([len(x) for x in items])
+    b = np.frombuffer(b"".join(items) or b"\x00", np.uint8)
+    return np.ascontiguousarray(b), off
 
 
 def identity_groups(identities):
@@ -380,17 +388,12 @@ class Context:
         """identities: list of (serialized: bytes, mspid: str, key_xy: 64 bytes, valid: bool).  policy_nodes may hold several policy
         trees; policies = {namespace: root node index} names the tree of each chaincode namespace (None: node 0 for every namespace).
         The identities' de-duplication groups (Mspid + certificate, identity_groups) are installed as well."""
-        def blob(items):
-            off = np.zeros(len(items) + 1, np.uint32)
-            off[1:] = np.cumsum([len(x) for x in items])
-            b = np.frombuffer(b"".join(items) or b"\x00", np.uint8)
-            return np.ascontiguousarray(b), off
-        idb, ido = blob([bytes(i[0]) for i in identities])
-        mb, mo = blob([i[1].encode() for i in identities])
+        idb, ido = _blob([bytes(i[0]) for i in identities])
+        mb, mo = _blob([i[1].encode() for i in identities])
         keys = np.ascontiguousarray(np.frombuffer(b"".join(bytes(i[2]) for i in identities) or b"\x00" * 64, np.uint8))
         valid = np.array([1 if i[3] else 0 for i in identities] or [0], np.uint8)
         nodes = np.ascontiguousarray(policy_nodes, dtype=np.int32).reshape(-1, 4)
-        pbb, pbo = blob([p.encode() for p in principals])
+        pbb, pbo = _blob([p.encode() for p in principals])
         self._ck(lib().fabgpu_msp_configure(self._h, _p(idb), _p(ido), _p(mb), _p(mo), _p(keys), _p(valid), ctypes.c_int(len(identities)),
                                             _p(nodes), ctypes.c_int(nodes.shape[0]), _p(pbb), _p(pbo), ctypes.c_int(len(principals)),
                                             ctypes.c_char_p(channel.encode())))
@@ -398,7 +401,7 @@ class Context:
             groups = np.ascontiguousarray(identity_groups(identities), np.int32)
             self._ck(lib().fabgpu_msp_identity_groups(self._h, _p(groups), ctypes.c_int(len(identities))))
         names = sorted(policies) if policies else []
-        nb, no = blob([n.encode() for n in names])
+        nb, no = _blob([n.encode() for n in names])
         roots = np.array([policies[n] for n in names] or [0], np.int32)
         self._ck(lib().fabgpu_namespace_policies(self._h, _p(nb), _p(no), _p(roots), ctypes.c_int(len(names))))
 
@@ -410,6 +413,15 @@ class Context:
         words = np.ascontiguousarray(pack_principal_bits(b)).reshape(-1)
         words = words if words.size else np.zeros(1, np.uint32)
         self._ck(lib().fabgpu_msp_principal_bits(self._h, _p(words), ctypes.c_int(b.shape[0]), ctypes.c_int(b.shape[1])))
+
+    def collection_policies(self, table):
+        """table: {(namespace, collection): root node index} -- the endorsement policy a write to that private-data collection is checked
+        against instead of the chaincode's (fabgpu_collection_policies).  None or an empty dict removes the table."""
+        keys = sorted(table) if table else []
+        nb, no = _blob([ns.encode() for ns, _ in keys])
+        cb, co = _blob([c.encode() for _, c in keys])
+        roots = np.array([table[k] for k in keys] or [0], np.int32)
+        self._ck(lib().fabgpu_collection_policies(self._h, _p(nb), _p(no), _p(cb), _p(co), _p(roots), ctypes.c_int(len(keys))))
 
     def block_buffer(self, nbytes, slot=0):
         """Pinned staging buffer (numpy view) for block bytes; one per slot."""

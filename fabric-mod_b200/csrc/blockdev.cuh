@@ -8,6 +8,7 @@
 //   KeyLevelValidator signature set        core/common/validation/statebased/validator_keylevel.go:243-259
 //   SignatureSetToValidIdentities          common/policies/policy.go:365-402
 //   cauthdsl evaluator                     common/cauthdsl/cauthdsl.go:24-92
+//   collection / chaincode policy per write core/common/validation/statebased/validator_keylevel.go:86-142, v20.go:105-163
 //   UnmarshalECDSASignature / IsLowS       bccsp/utils/ecdsa.go:43-92 (Go encoding/asn1 DER rules)
 // No STL, no allocation: everything is offsets into the block buffer and fixed-size records.
 #pragma once
@@ -32,6 +33,7 @@ enum : uint8_t {
 #define BD_MAX_SIGNERS 64       // distinct verified signers one policy evaluation handles (`used` is a 64-bit mask); more -> CPU validator
 #define BD_MAX_NS 4             // namespaces validated per transaction (the invoked chaincode + those it writes to); more -> CPU validator
 #define BD_MAX_NS_SEEN 8        // namespaces of one read/write set checked for duplicates; more -> CPU validator
+#define BD_MAX_COLL 8           // named private-data collections written per transaction; more -> CPU validator while a collection table is installed
 #define BD_MAX_POLICY_DEPTH 12  // deepest node of a policy tree eval_policy walks (root = 0); fabgpu_msp_configure refuses deeper trees
 #define BD_ENDS_HINT 16         // job-array sizing: expected endorsements per transaction (the capacity is a parameter, see JobArrays::J_cap)
 
@@ -292,6 +294,10 @@ struct TxDev {
     uint32_t first_end_job;        // endorsement jobs [first_end_job, first_end_job + n_end_jobs), in endorsement order
     uint32_t n_end_jobs;           // (endorsements without signature bytes get none: they can never verify)
     Seg wr_ns[BD_MAX_NS];
+    uint8_t n_coll;                // written collections in coll[]; BD_MAX_COLL + 1 = more than that
+    uint8_t pub_ns;                // bit i: wr_ns[i] has public writes, or writes to a collection without a name
+    uint8_t coll_ns[BD_MAX_COLL];  // wr_ns index of each written collection's namespace
+    Seg coll[BD_MAX_COLL];         // collection_name of each CollectionHashedReadWriteSet with hashed writes or metadata writes
 };
 
 // Everything plan_tx writes for one transaction besides TxDev: job records live in caller-provided arrays.
@@ -333,10 +339,11 @@ BD_HD bool seg_equal(const uint8_t* base, Seg a, Seg b)
 }
 
 // The plugin dispatcher's structural checks (plugindispatcher/dispatcher.go:102-179), in its order.  chdr_ext: ChannelHeader.extension;
-// prp / prp_ext: ProposalResponsePayload bytes and its extension (peer.ChaincodeAction).  Fills tx.disp, tx.wr_ns, tx.n_ns.
+// prp / prp_ext: ProposalResponsePayload bytes and its extension (peer.ChaincodeAction).  Fills tx.disp, tx.wr_ns, tx.n_ns, and
+// for the collection policies (validator_keylevel.go:86-142) tx.pub_ns and the written collections tx.coll / tx.coll_ns / tx.n_coll.
 BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool has_prp_ext, Seg prp_ext, TxDev& tx)
 {
-    tx.disp = TXC_VALID; tx.n_ns = 0;
+    tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0;
     // hdrExt = ChaincodeHeaderExtension{chaincode_id = 2}, its ChaincodeID{path = 1, name = 2, version = 3} parsed with it
     Seg h_ccid; h_ccid.off = h_ccid.len = 0; bool has_h_ccid = false;
     if (!scan_msg(base, chdr_ext, BD_F(2), 0, [&](uint32_t, Seg b) { h_ccid = b; has_h_ccid = true; })) { tx.disp = TXC_BAD_HEADER_EXTENSION; return; }
@@ -355,24 +362,31 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
         tx.disp = TXC_BAD_RESPONSE_PAYLOAD; return;
     }
     // txRWSet.FromProtoBytes(results): TxReadWriteSet{data_model = 1, ns_rwset = 2}, every namespace with its KVRWSet and hashed collections
-    Seg seen[BD_MAX_NS_SEEN]; bool wrote[BD_MAX_NS_SEEN]; uint32_t n_seen = 0; bool too_many = false, rw_ok = true;
+    Seg seen[BD_MAX_NS_SEEN]; bool wrote[BD_MAX_NS_SEEN], pub[BD_MAX_NS_SEEN]; uint32_t n_seen = 0; bool too_many = false, rw_ok = true;
     const bool top_ok = scan_msg(base, results, BD_F(2), BD_F(1), [&](uint32_t, Seg nsb) {
         if (!rw_ok) return;
         Seg name, kv; name.off = name.len = kv.off = kv.len = 0;
-        bool writes = false;
+        bool writes = false, pub_w = false;
         // NsReadWriteSet{namespace = 1, rwset = 2, collection_hashed_rwset = 3}
         if (!scan_msg(base, nsb, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t f, Seg b) {
                 if (f == 1) name = b; else if (f == 2) kv = b;
                 else {                                                  // CollectionHashedReadWriteSet{collection_name = 1, hashed_rwset = 2, pvt_rwset_hash = 3}
-                    Seg hashed; hashed.off = hashed.len = 0;
-                    if (!scan_msg(base, b, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg c) { if (g == 2) hashed = c; })) { rw_ok = false; return; }
+                    Seg hashed, cname; hashed.off = hashed.len = cname.off = cname.len = 0;
+                    if (!scan_msg(base, b, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg c) { if (g == 1) cname = c; else if (g == 2) hashed = c; })) { rw_ok = false; return; }
                     // HashedRWSet{hashed_reads = 1, hashed_writes = 2, metadata_writes = 3}
-                    if (!scan_msg(base, hashed, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg) { if (g == 2 || g == 3) writes = true; })) rw_ok = false;
+                    bool cw = false;
+                    if (!scan_msg(base, hashed, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg) { if (g == 2 || g == 3) cw = true; })) rw_ok = false;
+                    if (!cw) return;
+                    writes = true;
+                    // no name: the chaincode policy (v20.go:105-106); otherwise recorded against the namespace's index in seen[]
+                    if (cname.len == 0) pub_w = true;
+                    else if (tx.n_coll < BD_MAX_COLL) { tx.coll[tx.n_coll] = cname; tx.coll_ns[tx.n_coll] = (uint8_t)n_seen; tx.n_coll++; }
+                    else tx.n_coll = BD_MAX_COLL + 1;
                 } })) { rw_ok = false; return; }
         if (!rw_ok) return;
         // KVRWSet{reads = 1, range_queries_info = 2, writes = 3, metadata_writes = 4}
-        if (!scan_msg(base, kv, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t g, Seg) { if (g == 3 || g == 4) writes = true; })) { rw_ok = false; return; }
-        if (n_seen < BD_MAX_NS_SEEN) { seen[n_seen] = name; wrote[n_seen] = writes; n_seen++; } else too_many = true;
+        if (!scan_msg(base, kv, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t g, Seg) { if (g == 3 || g == 4) writes = pub_w = true; })) { rw_ok = false; return; }
+        if (n_seen < BD_MAX_NS_SEEN) { seen[n_seen] = name; wrote[n_seen] = writes; pub[n_seen] = pub_w; n_seen++; } else too_many = true;
     });
     if (!top_ok || !rw_ok) { tx.disp = TXC_BAD_RWSET; return; }
     if (!has_h_ccid || !has_r_ccid) { tx.disp = TXC_INVALID_OTHER_REASON; return; }
@@ -388,11 +402,16 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
     for (uint32_t i = 0; i < n_seen; i++) {
         for (uint32_t j = 0; j < i; j++) if (seg_equal(base, seen[i], seen[j])) { tx.disp = TXC_ILLEGAL_WRITESET; return; }
     }
+    uint8_t wr_of[BD_MAX_NS_SEEN];                                     // seen[] index -> wr_ns index, for the namespaces that wrote
     for (uint32_t i = 0; i < n_seen; i++) {
-        if (!wrote[i] || seg_equal(base, seen[i], h_name)) continue;
+        if (!wrote[i]) continue;
+        if (seg_equal(base, seen[i], h_name)) { wr_of[i] = 0; if (pub[i]) tx.pub_ns |= 1; continue; }
         if (tx.n_ns >= BD_MAX_NS) { tx.disp = TXC_NOT_VALIDATED; return; }
+        if (pub[i]) tx.pub_ns |= (uint8_t)(1u << tx.n_ns);
+        wr_of[i] = tx.n_ns;
         tx.wr_ns[tx.n_ns++] = seen[i];
     }
+    for (uint32_t c = 0; c < tx.n_coll && c < BD_MAX_COLL; c++) tx.coll_ns[c] = wr_of[tx.coll_ns[c]];   // a collection write makes its namespace write
 }
 
 // alloc_end(n) must return the first index of n fresh endorsement-job slots (atomicAdd on the device, a counter on the host)
@@ -401,7 +420,7 @@ BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* chan
                    JobArrays& ja, Alloc alloc_end)
 {
     tx.early = TXC_NOT_VALIDATED; tx.htype = 0; tx.endorser_parse_ok = 0; tx.channel_ok = 0; tx.endorsements_parse_ok = 1; tx.overflow = 0;
-    tx.disp = TXC_VALID; tx.n_ns = 0; tx.creator_identity = -1; tx.creator_has_job = 0; tx.first_end_job = 0; tx.n_end_jobs = 0;
+    tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0; tx.creator_identity = -1; tx.creator_has_job = 0; tx.first_end_job = 0; tx.n_end_jobs = 0;
     tx.txid_ascii.off = tx.txid_ascii.len = 0; tx.phash_claimed.off = tx.phash_claimed.len = 0;
     {
         ShaJobD z; for (int k = 0; k < 3; k++) { z.off[k] = 0; z.len[k] = 0; }
@@ -547,7 +566,59 @@ struct PolicyDev {
     const int32_t* nodes; int32_t n_nodes; const int32_t* principal_code; int32_t n_principals;
     const uint8_t* ns_blob; const uint32_t* ns_off; const int32_t* ns_root; int32_t n_ns;     // n_ns = 0: one policy (root 0) for every namespace
     const uint32_t* principal_bits = nullptr; int32_t bits_words = 0;          // a PolicyDev built field by field has no bits
+    // fabgpu_collection_policies: entry i maps (namespace i, collection i) to policy root coll_root[i]; an open-addressing table of
+    // coll_size slots (a power of two) keyed by coll_key_hash finds it.  coll_size = 0: no table, every write falls under its
+    // namespace's chaincode policy.
+    const uint8_t* coll_ns_blob = nullptr; const uint32_t* coll_ns_off = nullptr; const uint8_t* coll_name_blob = nullptr;
+    const uint32_t* coll_name_off = nullptr; const int32_t* coll_root = nullptr; const uint64_t* coll_hash = nullptr; const int32_t* coll_idx = nullptr;
+    uint32_t coll_size = 0;
 };
+
+BD_HD uint64_t coll_key_hash(const uint8_t* ns, uint32_t ns_len, const uint8_t* coll, uint32_t coll_len)
+{
+    uint64_t h = 1469598103934665603ull ^ ns_len;
+    for (uint32_t i = 0; i < ns_len; i++) h = (h ^ ns[i]) * 1099511628211ull;
+    h = (h ^ coll_len) * 1099511628211ull;
+    for (uint32_t i = 0; i < coll_len; i++) h = (h ^ coll[i]) * 1099511628211ull;
+    return h ? h : 1;
+}
+
+// Host side of fabgpu_collection_policies: fills the table (size a power of two above n; hash all zero, idx any) with entries
+// [0, n).  false when two entries name the same (namespace, collection).
+inline bool coll_table_fill(const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off, int32_t n,
+                            uint32_t size, uint64_t* hash, int32_t* idx)
+{
+    for (int32_t i = 0; i < n; i++) {
+        const uint32_t nl = ns_off[i + 1] - ns_off[i], cl = coll_off[i + 1] - coll_off[i];
+        const uint64_t h = coll_key_hash(ns_blob + ns_off[i], nl, coll_blob + coll_off[i], cl);
+        uint32_t pos = (uint32_t)h & (size - 1);
+        for (; hash[pos] != 0; pos = (pos + 1) & (size - 1)) {
+            const int32_t k = idx[pos];
+            if (hash[pos] == h && ns_off[k + 1] - ns_off[k] == nl && coll_off[k + 1] - coll_off[k] == cl &&
+                memcmp(ns_blob + ns_off[k], ns_blob + ns_off[i], nl) == 0 && memcmp(coll_blob + coll_off[k], coll_blob + coll_off[i], cl) == 0)
+                return false;
+        }
+        hash[pos] = h; idx[pos] = i;
+    }
+    return true;
+}
+
+// policy root of collection `coll` of namespace `ns` (both in the block), -1 when the table has no entry for it
+BD_HD int32_t coll_policy_root(const PolicyDev& pol, const uint8_t* base, Seg ns, Seg coll)
+{
+    const uint64_t h = coll_key_hash(base + ns.off, ns.len, base + coll.off, coll.len);
+    for (uint32_t probe = 0, pos = (uint32_t)h & (pol.coll_size - 1); probe < pol.coll_size; probe++, pos = (pos + 1) & (pol.coll_size - 1)) {
+        const uint64_t k = pol.coll_hash[pos];
+        if (k == 0) return -1;
+        if (k != h) continue;
+        const int32_t i = pol.coll_idx[pos];
+        const uint32_t no = pol.coll_ns_off[i], co = pol.coll_name_off[i];
+        if (pol.coll_ns_off[i + 1] - no == ns.len && pol.coll_name_off[i + 1] - co == coll.len &&
+            bytes_equal(pol.coll_ns_blob + no, base + ns.off, ns.len) && bytes_equal(pol.coll_name_blob + co, base + coll.off, coll.len))
+            return pol.coll_root[i];
+    }
+    return -1;
+}
 
 // signer[i]: with principal bits, the identity index of verified signer i; without, its MSP-id code, -1 when Validate() failed.
 BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer, int n_signers, uint64_t& used, int depth)
@@ -609,7 +680,8 @@ BD_HD int32_t policy_root(const PolicyDev& pol, const uint8_t* base, Seg ns)
 
 // ---- per-transaction decision ---------------------------------------------------------------------------------------------
 // sig_ok(j): signature job j verified (gate and curve).  job_identity: JobArrays::identity.  digests: 32 bytes per SHA job.
-// An identity the table does not hold, or a namespace without a policy entry, cannot be decided here: TXC_NOT_VALIDATED hands the
+// An identity the table does not hold, a namespace without a policy entry, or (with a collection table) a written collection without
+// one, cannot be decided here: TXC_NOT_VALIDATED hands the
 // transaction to the CPU validator (the reference deserialises and validates ANY certificate of the channel's CAs,
 // msgvalidation.go:40-57, and reads chaincode definitions from the ledger, dispatcher.go:224-277).
 template <typename SigOk>
@@ -637,10 +709,30 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
     if (tx.disp != TXC_VALID) return tx.disp;                         // the plugin dispatcher's own checks
     if (!tx.endorsements_parse_ok) return TXC_INVALID_OTHER_REASON;
     if (tx.overflow) return TXC_NOT_VALIDATED;                        // job arrays were full: CPU validator
-    int32_t roots[BD_MAX_NS];
+    // The policies to satisfy, each root once (evaluation has no state across policies, so the reference's nsEPChecked memo,
+    // v20.go:105-147, changes no outcome).  Without a collection table: every validated namespace's chaincode policy.  With one, per
+    // namespace as baseEvaluator.Evaluate (validator_keylevel.go:86-142) walks its writes: the collection's policy for each named
+    // collection written, the chaincode policy for public writes and collections without a name, and the chaincode policy when
+    // nothing else was checked (CheckCCEPIfNoEPChecked, v20.go:149-163: the invoked chaincode that only reads).
+    int32_t roots[BD_MAX_NS], need[BD_MAX_NS + BD_MAX_COLL]; int n_need = 0;
+    auto add = [&](int32_t r) { for (int k = 0; k < n_need; k++) if (need[k] == r) return; need[n_need++] = r; };
     for (int i = 0; i < tx.n_ns; i++) {
         roots[i] = policy_root(pol, base, tx.wr_ns[i]);
         if (roots[i] < 0) return TXC_NOT_VALIDATED;                   // no chaincode definition on the device
+    }
+    if (pol.coll_size == 0) {
+        for (int i = 0; i < tx.n_ns; i++) add(roots[i]);
+    } else {
+        if (tx.n_coll > BD_MAX_COLL) return TXC_NOT_VALIDATED;          // more collections than the walk records
+        uint32_t has_coll = 0;
+        for (int c = 0; c < tx.n_coll; c++) {
+            const int32_t r = coll_policy_root(pol, base, tx.wr_ns[tx.coll_ns[c]], tx.coll[c]);
+            if (r < 0) return TXC_NOT_VALIDATED;                        // CollectionValidationInfo would read the ledger
+            add(r);
+            has_coll |= 1u << tx.coll_ns[c];
+        }
+        for (int i = 0; i < tx.n_ns; i++)
+            if (((tx.pub_ns | ~has_coll) >> i) & 1u) add(roots[i]);
     }
     // SignatureSetToValidIdentities (policy.go:365-402): in order; de-duplicated by Mspid + Id against the identities that already
     // VERIFIED; a failed signature drops that entry only.  One set per transaction, shared by every namespace's evaluation.
@@ -664,9 +756,9 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
         if (n_signers >= BD_MAX_SIGNERS) return TXC_NOT_VALIDATED;
         signer[n_signers++] = pol.principal_bits ? idn : msp.valid[idn] ? msp.msp_code[idn] : -1;
     }
-    for (int i = 0; i < tx.n_ns; i++) {
+    for (int k = 0; k < n_need; k++) {
         uint64_t used = 0;
-        if (!eval_policy(pol, roots[i], signer, n_signers, used, 0)) return TXC_ENDORSEMENT_POLICY_FAILURE;
+        if (!eval_policy(pol, need[k], signer, n_signers, used, 0)) return TXC_ENDORSEMENT_POLICY_FAILURE;
     }
     uint64_t hsh = 1469598103934665603ull;
     for (uint32_t k = 0; k < tx.txid_ascii.len; k++) hsh = (hsh ^ base[tx.txid_ascii.off + k]) * 1099511628211ull;

@@ -210,6 +210,8 @@ struct fabgpu_ctx {
         DevArray<int32_t> group;                                      // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
         DevArray<uint8_t> ns_blob; DevArray<uint32_t> ns_off; DevArray<int32_t> ns_root; int32_t n_ns = 0;    // fabgpu_namespace_policies
         DevArray<uint32_t> pbits; int32_t pbits_words = 0;            // fabgpu_msp_principal_bits, null = MSP-id member matching
+        DevArray<uint8_t> cp_ns_blob, cp_name_blob; DevArray<uint32_t> cp_ns_off, cp_name_off;   // fabgpu_collection_policies, cp_size = 0: none
+        DevArray<int32_t> cp_root, cp_idx; DevArray<uint64_t> cp_hash; uint32_t cp_size = 0;
         DevArray<uint64_t> ht_hash; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
         bool all_slots = true; int classes = 0;                    // which non-big classes the identities' keys fall in (CLASS_*)
     } dm;
@@ -1842,6 +1844,40 @@ int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uin
     return FABGPU_OK;
 }
 
+int fabgpu_collection_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                               const int32_t* coll_root, int n)
+{
+    if (!ctx || n < 0) return FABGPU_E_ARG;
+    if (n && (!ns_blob || !ns_off || !coll_blob || !coll_off || !coll_root)) { ctx->last_error = "collection policy arrays missing"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm;
+    for (int i = 0; i < n; i++) {
+        const char* err = coll_root[i] < 0 || coll_root[i] >= dm.n_nodes ? "collection policy root out of range"
+                        : ns_off[i] > ns_off[i + 1] || coll_off[i] > coll_off[i + 1] ? "collection policy offsets decrease"
+                        : coll_off[i] == coll_off[i + 1] ? "collection policy with an empty collection name" : nullptr;
+        if (err) { ctx->last_error = err; return FABGPU_E_ARG; }
+    }
+    uint32_t size = 8; while (size < (uint32_t)(2 * n + 8)) size <<= 1;      // load factor <= 1/2
+    std::vector<uint64_t> hh(size, 0); std::vector<int32_t> hi(size, -1);
+    if (!bdev::coll_table_fill(ns_blob, ns_off, coll_blob, coll_off, n, size, hh.data(), hi.data())) {
+        ctx->last_error = "collection policy given twice for one (namespace, collection)"; return FABGPU_E_ARG;
+    }
+    int rc = drain_block_streams(ctx); if (rc) return rc;
+    dm.cp_ns_blob = {}; dm.cp_name_blob = {}; dm.cp_ns_off = {}; dm.cp_name_off = {}; dm.cp_root = {}; dm.cp_idx = {}; dm.cp_hash = {}; dm.cp_size = 0;
+    if (n == 0) return FABGPU_OK;
+    auto up = [&](auto& dst, const void* src, size_t bytes) -> int {
+        if (int r = dst.reserve(ctx, bytes + 8)) return r;          // slack: bytes_equal reads whole aligned words
+        if (bytes) CK(ctx, cudaMemcpy(dst.get(), src, bytes, cudaMemcpyHostToDevice));
+        return FABGPU_OK;
+    };
+    if ((rc = up(dm.cp_ns_blob, ns_blob, ns_off[n])) || (rc = up(dm.cp_ns_off, ns_off, 4 * (size_t)(n + 1))) ||
+        (rc = up(dm.cp_name_blob, coll_blob, coll_off[n])) || (rc = up(dm.cp_name_off, coll_off, 4 * (size_t)(n + 1))) ||
+        (rc = up(dm.cp_root, coll_root, 4 * (size_t)n)) || (rc = up(dm.cp_hash, hh.data(), 8 * (size_t)size)) || (rc = up(dm.cp_idx, hi.data(), 4 * (size_t)size)))
+        return rc;
+    dm.cp_size = size;
+    return FABGPU_OK;
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -1948,6 +1984,8 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     bdev::PolicyDev pol; pol.nodes = dm.nodes.get(); pol.n_nodes = dm.n_nodes; pol.principal_code = dm.principal_code.get(); pol.n_principals = dm.n_principals;
     pol.ns_blob = dm.ns_blob.get(); pol.ns_off = dm.ns_off.get(); pol.ns_root = dm.ns_root.get(); pol.n_ns = dm.n_ns;
     pol.principal_bits = dm.pbits.get(); pol.bits_words = dm.pbits_words;
+    pol.coll_ns_blob = dm.cp_ns_blob.get(); pol.coll_ns_off = dm.cp_ns_off.get(); pol.coll_name_blob = dm.cp_name_blob.get(); pol.coll_name_off = dm.cp_name_off.get();
+    pol.coll_root = dm.cp_root.get(); pol.coll_hash = dm.cp_hash.get(); pol.coll_idx = dm.cp_idx.get(); pol.coll_size = dm.cp_size;
     const bool need_q = (dm.classes & CLASS_GENERIC) != 0;   // only the generic arithmetic reads the key itself
     bdev::JobArrays ja; ja.sha = db.d_sha.get(); ja.r = db.d_r.get(); ja.s = db.d_s.get(); ja.key_slot = db.d_ks.get(); ja.identity = db.d_ident.get(); ja.qx = need_q ? db.d_qx.get() : nullptr;
     ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T;

@@ -234,7 +234,7 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
                          const int32_t* policy_nodes, int n_nodes, const uint8_t* principal_blob, const uint32_t* principal_off,
                          int n_principals, const char* channel_id);
 /* Optional refinements of the table fabgpu_msp_configure installed (call them after it; each drains the block slots first;
- * fabgpu_msp_configure clears all three):
+ * fabgpu_msp_configure clears all four):
  *   _identity_groups: group[i] = de-duplication id of identity i.  The reference de-duplicates a transaction's signers on
  *       Mspid + certificate digest (common/policies/policy.go:380-386), so two byte-different serializations of ONE certificate
  *       must share a group; without this call every table entry is its own group.
@@ -250,10 +250,24 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
  *       matches a verified, de-duplicated signer iff its bit p is set, whatever its Validate() outcome (an admin-listed
  *       identity satisfies ADMIN without it, mspimpl.go:506-513); the creator's Validate() is still checked.  n_ids and
  *       n_principals must equal fabgpu_msp_configure's, else FABGPU_E_ARG and nothing changes; n_ids = 0 removes the bits
- *       and restores MSP-id member matching. */
+ *       and restores MSP-id member matching.
+ *   _collection_policies: the endorsement policy of private-data collections.  Entry i says that a write to collection coll[i]
+ *       (coll_blob + (n+1) offsets) of namespace ns[i] (ns_blob + (n+1) offsets) is checked against the tree at node coll_root[i] of
+ *       fabgpu_msp_configure's array instead of the chaincode's (core/common/validation/statebased/v20.go:105-147).  The caller
+ *       resolves CollectionValidationInfo (core/chaincode/lifecycle/deployedcc_infoprovider.go:359-394): an implicit
+ *       collection _implicit_org_<MSPID> gets that org's Endorsement policy, or SignedByAnyMember(MSPID) without one; a static
+ *       collection with an EndorsementPolicy gets it; one without gets its chaincode's root.  While a table is installed, each
+ *       validated namespace must satisfy the policy of every named collection it writes (hashed writes or hashed metadata
+ *       writes), its chaincode policy when it has public writes or writes to a collection without a name, and its chaincode
+ *       policy when it wrote nothing else.  A transaction that writes a (namespace, collection) without an entry, or more than
+ *       8 named collections, is flagged 254 (NOT_VALIDATED).  FABGPU_E_ARG, with the previous table kept, for NULL arrays with
+ *       n > 0, a root outside [0, n_nodes), decreasing offsets, an empty collection name or a (namespace, collection) given twice.
+ *       n = 0 removes the table: every write falls under its namespace's chaincode policy, as without this call. */
 int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids);
 int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, int n_principals);
 int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const int32_t* ns_root, int n_ns);
+int fabgpu_collection_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob,
+                               const uint32_t* coll_off, const int32_t* coll_root, int n);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their

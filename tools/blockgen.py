@@ -62,17 +62,36 @@ def hashed_rwset(n_writes, tag=b"k") -> bytes:
                                                                   for i in range(n_writes))
 
 
+def collection_hashed_rwset(n_writes, n_metadata_writes, n_reads, tag=b"k") -> bytes:
+    """kvrwset.HashedRWSet{hashed_reads=1, hashed_writes=2, metadata_writes=3}: KVReadHash{key_hash=1}, KVWriteHash{key_hash=1,
+    value_hash=3}, KVMetadataWriteHash{key_hash=1, entries=2} with one KVMetadataEntry{name=1, value=2}."""
+    h = lambda s: hashlib.sha256(s).digest()
+    return (b"".join(pb.f_bytes(1, pb.f_bytes(1, h(tag + b"-hr%d" % i))) for i in range(n_reads)) +
+            b"".join(pb.f_bytes(2, pb.f_bytes(1, h(tag + b"-hw%d" % i)) + pb.f_bytes(3, h(b"v%d" % i))) for i in range(n_writes)) +
+            b"".join(pb.f_bytes(3, pb.f_bytes(1, h(tag + b"-hm%d" % i)) + pb.f_bytes(2, pb.f_bytes(1, b"VALIDATION_PARAMETER") + pb.f_bytes(2, b"ep")))
+                     for i in range(n_metadata_writes)))
+
+
 def tx_rwset(namespaces, mut=_same) -> bytes:
-    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes[, n_hashed_writes]).  A fourth
-    entry adds one private-data collection, NsReadWriteSet.collection_hashed_rwset = CollectionHashedReadWriteSet{collection_name=1,
-    hashed_rwset=2} with that many hashed writes.  mut(part, bytes): see build_block."""
+    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes[, collections]).  The
+    fourth entry adds private-data collections, NsReadWriteSet.collection_hashed_rwset = CollectionHashedReadWriteSet{collection_name=1,
+    hashed_rwset=2}: an int n is one collection named "collection" with n hashed writes and one hashed read; a list holds one
+    (collection_name, n_hashed_writes, n_metadata_writes, n_hashed_reads) per collection, in order, and a collection_name of None
+    leaves the field out.  mut(part, bytes): see build_block."""
     out = b""
     for ns in namespaces:
         name, nr, nw = ns[:3]
         body = pb.f_bytes(1, name.encode()) + pb.f_bytes(2, mut("KVRWSet", kv_rwset(nr, nw, name.encode())))
-        if len(ns) > 3:
+        if len(ns) > 3 and isinstance(ns[3], int):
             coll = pb.f_bytes(1, b"collection") + pb.f_bytes(2, mut("HashedRWSet", hashed_rwset(ns[3], name.encode())))
             body += pb.f_bytes(3, mut("CollectionHashedReadWriteSet", coll))
+        elif len(ns) > 3:
+            for cname, n_hw, n_mw, n_hr in ns[3]:
+                cn = cname.encode() if isinstance(cname, str) else cname
+                tag = name.encode() + b"/" + (cn or b"")
+                coll = (pb.f_bytes(1, cn) if cn is not None else b"") + \
+                    pb.f_bytes(2, mut("HashedRWSet", collection_hashed_rwset(n_hw, n_mw, n_hr, tag)))
+                body += pb.f_bytes(3, mut("CollectionHashedReadWriteSet", coll))
         out += pb.f_bytes(2, mut("NsReadWriteSet", body))
     return mut("TxReadWriteSet", out)
 

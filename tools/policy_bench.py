@@ -48,6 +48,11 @@ def leg(ctx, cfg, net, pinned, eoff, n_tx, slots, reps_single, reps_flight):
     ctx.msp_configure(ids, nodes, principals, net.channel)
     if bits is not None:
         ctx.msp_principal_bits(bits)
+    return timed(ctx, pinned, eoff, n_tx, slots, reps_single, reps_flight)
+
+
+def timed(ctx, pinned, eoff, n_tx, slots, reps_single, reps_flight):
+    """The configuration ctx holds, on the block in `pinned` (one copy per slot): every flag must be VALID."""
     os.environ["FABGPU_BLOCK_EVENTS"] = "1"
     decide = []
     for _ in range(3):
