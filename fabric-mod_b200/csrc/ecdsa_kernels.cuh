@@ -390,7 +390,7 @@ ecdsa_verify_lanes_kernel(const int32_t* __restrict__ key_slot, const uint8_t* _
         for (int t = 0; t < STEPS; t++) {
             const int j = t * LANES + lane;
             const uint32_t di = dig[j * SIGS + sg];
-            if (di != FAB_BA_INF) acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, (j < FAB_G_WINDOWS ? gtab : qt)[di]);
+            if (di != FAB_BA_INF) acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, load_aff_nc((j < FAB_G_WINDOWS ? gtab : qt) + di));
         }
     }
     // tree-combine the partial sums of the group's lanes

@@ -98,6 +98,24 @@ FAB_HD void prefetch_entry(const aff* p)
 #endif
 }
 
+// The window chains' table gathers go through here: one register copy made of four 128-bit loads on the read-only path.  Handed a
+// reference into global memory instead, the expanded addition loads each limb where it uses it: 16 scalar loads per point, each a
+// divergent request of its own, since every lane of a warp gathers a different random point.  Tables are cudaMalloc'ed arrays of
+// 64-byte points (16-byte aligned) that no kernel writes while a verification reads them.
+FAB_HD aff load_aff_nc(const aff* p)
+{
+#if defined(__CUDA_ARCH__)
+    const uint4* q = reinterpret_cast<const uint4*>(p);
+    const uint4 a = __ldg(q), b = __ldg(q + 1), c = __ldg(q + 2), d = __ldg(q + 3);
+    aff r;
+    r.x = u256_const(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
+    r.y = u256_const(c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w);
+    return r;
+#else
+    return *p;
+#endif
+}
+
 // r += u1 * G using the fixed-base table gtab[window][digit-1] (affine, Montgomery form)
 FAB_HD jac add_fixed_base(jac r, const u256& k, const aff* gtab)
 {
@@ -111,7 +129,7 @@ FAB_HD jac add_fixed_base(jac r, const u256& k, const aff* gtab)
         kk[7] >>= FAB_WG;
         const uint32_t dn = kk[0] & (uint32_t)FAB_G_ENTRIES;
         if (dn && j + 1 < FAB_G_WINDOWS) prefetch_entry(gtab + (size_t)(j + 1) * FAB_G_ENTRIES + (dn - 1));
-        if (d) r = jac_add_aff(r, gtab[(size_t)j * FAB_G_ENTRIES + (d - 1)]);
+        if (d) r = jac_add_aff(r, load_aff_nc(gtab + (size_t)j * FAB_G_ENTRIES + (d - 1)));
     }
     return r;
 }
@@ -203,6 +221,10 @@ FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& 
         }
     }
 #endif
+    // cur: this window's entry (nullptr for a zero digit).  Each pass forms the NEXT window's entry address once, for its prefetch and
+    // as the next pass's gather address.
+    const uint32_t d0 = u1.v[0] & (uint32_t)FAB_G_ENTRIES;
+    const aff* cur = d0 ? gtab + (d0 - 1) : nullptr;
 #pragma unroll 1
     for (int t = 0; t < 2; t++) {
         uint32_t kk[8];
@@ -213,20 +235,20 @@ FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& 
         const int windows = t ? FAB_Q_WINDOWS : FAB_G_WINDOWS;
 #pragma unroll 1
         for (int j = 0; j < windows; j++) {
-            const uint32_t d = kk[0] & entries;
 #pragma unroll
             for (int i = 0; i < 7; i++) kk[i] = (kk[i] >> wbits) | (kk[i + 1] << (32u - wbits));
             kk[7] >>= wbits;
+            // the entry of the next window (or the first window of the key's table)
+            const aff* nx = nullptr;
+            if (j + 1 < windows) { const uint32_t dn = kk[0] & entries; if (dn) nx = tab + (size_t)(j + 1) * entries + (dn - 1); }
+            else if (t == 0) { const uint32_t dn = u2.v[0] & ((1u << FAB_WQ) - 1u); if (dn) nx = qtab + (dn - 1); }
 #if defined(__CUDA_ARCH__) && FAB_JAC_NEXT_PREFETCH
-            {   // the entry of the NEXT window (or the first window of the key's table) is requested from the L2 while this addition runs:
-                // the tables are HBM-resident, so without it one DRAM round trip per addition is exposed
-                const aff* nx = nullptr;
-                if (j + 1 < windows) { const uint32_t dn = kk[0] & entries; if (dn) nx = tab + (size_t)(j + 1) * entries + (dn - 1); }
-                else if (t == 0) { const uint32_t dn = u2.v[0] & ((1u << FAB_WQ) - 1u); if (dn) nx = qtab + (dn - 1); }
-                if (nx) asm volatile("prefetch.global.L2 [%0];" :: "l"(nx));
-            }
+            // requested from the L2 while this addition runs: the tables are HBM-resident, so without it one DRAM round trip per
+            // addition is exposed
+            if (nx) asm volatile("prefetch.global.L2 [%0];" :: "l"(nx));
 #endif
-            if (d) acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, tab[(size_t)j * entries + (d - 1)]);
+            if (cur) acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, load_aff_nc(cur));
+            cur = nx;
         }
     }
     return final_check(acc, r);
@@ -285,7 +307,7 @@ FAB_HD jac add_small_table(jac acc, const u256& k, const aff* stab)
         if (neg) d = (1u << FAB_WS) - d;
         carry = neg ? 1u : 0u;
         if (d) {
-            aff pt = stab[(size_t)j * FAB_S_HALF + (d - 1)];
+            aff pt = load_aff_nc(stab + (size_t)j * FAB_S_HALF + (d - 1));
             if (neg) pt.y = fe_neg(pt.y);
             acc = jac_add_aff(acc, pt);
         }
@@ -333,7 +355,7 @@ FAB_HD uint32_t ecdsa_verify_one_small(const aff* stab, const u256& e, const u25
             if (neg) d = (1u << wbits) - d;
             carry = neg ? 1u : 0u;
             if (d) {
-                aff pt = tab[(size_t)j * stride + (d - 1)];
+                aff pt = load_aff_nc(tab + (size_t)j * stride + (d - 1));
                 if (neg) pt.y = fe_neg(pt.y);
                 acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, pt);
             }

@@ -64,13 +64,15 @@ FAB_HD jac jac_add(const jac& p, const jac& q)
 }
 
 // The two exceptional cases of an addition whose H = 0: same point -> doubling, opposite points -> infinity.  Out of line:
-// never taken on honest inputs, and the doubling must not be expanded into the caller's loop body.
+// never taken on honest inputs, and the doubling must not be expanded into the caller's loop body.  Arguments by value: a
+// reference would need the caller's accumulator in local memory wherever this call can happen, i.e. a store of it on every pass
+// of a verify kernel's window loop; by value it is copied out only when the call is taken.
 #if defined(__CUDA_ARCH__)
 __device__ __noinline__
 #else
 inline
 #endif
-jac jac_add_h_zero(const jac& p, const u256& rr)
+jac jac_add_h_zero(jac p, u256 rr)
 {
     if (u256_is_zero(rr)) return jac_double(p);
     return jac_infinity();
