@@ -25,6 +25,7 @@ EXPORTS = [
     "fabgpu_msp_configure", "fabgpu_validate_block", "fabgpu_validate_envelopes", "fabgpu_block_buffer", "fabgpu_block_timing", "fabgpu_sha256_segments",
     "fabgpu_bccsp_verify_batch_async", "fabgpu_bccsp_verify_batch_wait", "fabgpu_bccsp_batch_buffers", "fabgpu_bccsp_verify_batch_inplace_async",
     "fabgpu_msp_identity_groups", "fabgpu_namespace_policies", "fabgpu_msp_principal_bits", "fabgpu_collection_policies",
+    "fabgpu_key_policies", "fabgpu_key_policies_update",
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
@@ -422,6 +423,28 @@ class Context:
         cb, co = _blob([c.encode() for _, c in keys])
         roots = np.array([table[k] for k in keys] or [0], np.int32)
         self._ck(lib().fabgpu_collection_policies(self._h, _p(nb), _p(no), _p(cb), _p(co), _p(roots), ctypes.c_int(len(keys))))
+
+    def key_policies(self, nodes, table):
+        """nodes: (n, 4) int32 policy nodes of the validation parameters (NOutOf / SignedBy, child indices within `nodes`, SignedBy indexing
+        msp_configure's principals); table: {(namespace, collection, key): root} -- the root node of that key's validation parameter, or -2
+        when the device may not decide it.  collection is "" for a public key; key is str or bytes (the 32-byte key hash for a collection
+        key).  Replaces the key policy table (fabgpu_key_policies); no nodes and an empty table remove it."""
+        self._key_policies(lib().fabgpu_key_policies, nodes, table)
+
+    def key_policies_update(self, nodes, table):
+        """Upserts into the installed key policy table (fabgpu_key_policies_update): same arguments, root -1 removes the key."""
+        self._key_policies(lib().fabgpu_key_policies_update, nodes, table)
+
+    def _key_policies(self, fn, nodes, table):
+        b = lambda x: x.encode() if isinstance(x, str) else bytes(x)
+        keys = list(table) if table else []
+        nb, no = _blob([b(k[0]) for k in keys])
+        cb, co = _blob([b(k[1]) for k in keys])
+        kb, ko = _blob([b(k[2]) for k in keys])
+        roots = np.array([table[k] for k in keys] or [0], np.int32)
+        nd = np.ascontiguousarray(np.asarray(nodes if nodes is not None and len(nodes) else np.zeros((0, 4)), dtype=np.int32).reshape(-1, 4))
+        ndp = nd if nd.shape[0] else np.zeros((1, 4), np.int32)
+        self._ck(fn(self._h, _p(ndp), ctypes.c_int(nd.shape[0]), _p(nb), _p(no), _p(cb), _p(co), _p(kb), _p(ko), _p(roots), ctypes.c_int(len(keys))))
 
     def block_buffer(self, nbytes, slot=0):
         """Pinned staging buffer (numpy view) for block bytes; one per slot."""

@@ -36,6 +36,10 @@ enum : uint8_t {
 #define BD_MAX_COLL 8           // named private-data collections written per transaction; more -> CPU validator while a collection table is installed
 #define BD_MAX_POLICY_DEPTH 12  // deepest node of a policy tree eval_policy walks (root = 0); fabgpu_msp_configure refuses deeper trees
 #define BD_ENDS_HINT 16         // job-array sizing: expected endorsements per transaction (the capacity is a parameter, see JobArrays::J_cap)
+#define BD_WRITES_HINT 8        // write-record sizing while a key policy table is installed: expected writes per transaction (KlArrays::W_cap)
+#define BD_MAX_NEED 16          // distinct policy roots one transaction is checked against; more -> CPU validator
+#define KP_UNDECIDABLE (-2)     // key policy table root: the key's validation parameter is not one the device may evaluate
+#define KP_REMOVED (-3)         // key policy table slot whose entry was removed (probes continue past it)
 
 struct Seg { uint32_t off, len; };
 
@@ -298,10 +302,44 @@ struct TxDev {
     uint8_t pub_ns;                // bit i: wr_ns[i] has public writes, or writes to a collection without a name
     uint8_t coll_ns[BD_MAX_COLL];  // wr_ns index of each written collection's namespace
     Seg coll[BD_MAX_COLL];         // collection_name of each CollectionHashedReadWriteSet with hashed writes or metadata writes
+    Seg results;                   // ChaincodeAction.results (the TxReadWriteSet), once dispatch_plan has read it
+    uint32_t first_w, n_w;         // write records [first_w, first_w + n_w) of KlArrays::w (key policy table installed only)
+    uint8_t kl_bad;                // a write inside the read/write set does not parse: the key-level checks cannot be made here
+};
+
+// One write of a transaction as baseEvaluator.Evaluate walks them (validator_keylevel.go:86-142): a public write, public metadata write,
+// hashed write or hashed metadata write.  coll is empty for public keys; key is the key hash for collection keys.
+struct WriteRec {
+    Seg ns, coll, key;
+    uint32_t tx;
+    uint32_t slot;                 // metadata-write set entry of the key, 0xffffffff = none (set by the walk for metadata records, by
+                                   // the decide stage for the others)
+    uint8_t ns_idx;                // TxDev::wr_ns index of the namespace
+    uint8_t md;                    // a metadata write
+    uint8_t gone;                  // from a transaction that never reaches VSCC (only its metadata writes are recorded)
+    uint8_t alias;                 // the entry's first writer has another key with the same hash: its dependency is not decided here
+};
+
+// Key-level validation state of one block, used only while a key policy table is installed (w = null: off).  The metadata-write set is
+// an open-addressing table of md_size slots keyed by kl_key_hash (0 = empty).  Per entry: md_min, the earliest metadata record
+// ((tx << 32) | record index, all ones = none), and md_sum, the VSCC results of its writers so far, which the resolve stage fills in
+// index order (KL_SUM_*).  Keys with one hash share an entry; the decide stage marks that (KL_SUM_MIXED, WriteRec::alias) and such a
+// dependency is not decided here.
+#define KL_SUM_NIL 1u              // a writer with a nil result
+#define KL_SUM_UNDET 2u            // a writer whose result is not determined by the block
+#define KL_SUM_MIXED 4u            // metadata writers of more than one key
+#define KL_SUM_ANY 8u              // some writer
+struct KlArrays {
+    WriteRec* w = nullptr; uint32_t W_cap = 0;
+    uint32_t* counter = nullptr;   // [0]: records handed out (> W_cap: overflow), [1]: nonzero = the block's dependencies cannot be trusted
+    uint64_t* md_hash = nullptr; unsigned long long* md_min = nullptr; uint32_t* md_sum = nullptr; uint32_t md_size = 0;
+    uint8_t* conflicted = nullptr; // per transaction: bit 0 = an earlier transaction metadata-wrote a key it writes, bit 1 = it metadata-writes
+    uint32_t* clist = nullptr;     // scratch of the resolve stage: the marked transactions in index order
 };
 
 // Everything plan_tx writes for one transaction besides TxDev: job records live in caller-provided arrays.
 struct JobArrays {
+    KlArrays kl;                   // write records and the metadata-write set; all null without a key policy table
     ShaJobD* sha;                  // [J_cap + 2 T]: signature messages, then (txid, proposal hash) per transaction
     uint8_t* r; uint8_t* s;        // [J_cap x 32]
     int32_t* key_slot;             // [J_cap]
@@ -357,6 +395,7 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
             if (f == 1) results = b; else if (f == 2) { events = b; has_events = true; } else if (f == 4) { r_ccid = b; has_r_ccid = true; } })) {
         tx.disp = TXC_BAD_RESPONSE_PAYLOAD; return;
     }
+    tx.results = results;
     Seg r_name, r_ver; r_name.off = r_name.len = r_ver.off = r_ver.len = 0;
     if (has_r_ccid && !scan_msg(base, r_ccid, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t f, Seg b) { if (f == 2) r_name = b; else if (f == 3) r_ver = b; })) {
         tx.disp = TXC_BAD_RESPONSE_PAYLOAD; return;
@@ -414,14 +453,158 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
     for (uint32_t c = 0; c < tx.n_coll && c < BD_MAX_COLL; c++) tx.coll_ns[c] = wr_of[tx.coll_ns[c]];   // a collection write makes its namespace write
 }
 
+// ---- key-level validation parameters: write records and in-block dependencies --------------------------------------------
+// FNV-1a over (namespace, collection, key), each with its length: the key policy table's and the metadata-write set's hash.
+BD_HD uint64_t kl_key_hash(const uint8_t* ns, uint32_t ns_len, const uint8_t* coll, uint32_t coll_len, const uint8_t* key, uint32_t key_len)
+{
+    uint64_t h = 1469598103934665603ull ^ ns_len;
+    for (uint32_t i = 0; i < ns_len; i++) h = (h ^ ns[i]) * 1099511628211ull;
+    h = (h ^ coll_len) * 1099511628211ull;
+    for (uint32_t i = 0; i < coll_len; i++) h = (h ^ coll[i]) * 1099511628211ull;
+    h = (h ^ key_len) * 1099511628211ull;
+    for (uint32_t i = 0; i < key_len; i++) h = (h ^ key[i]) * 1099511628211ull;
+    return h ? h : 1;
+}
+BD_HD uint64_t kl_rec_hash(const uint8_t* base, const WriteRec& w)
+{
+    return kl_key_hash(base + w.ns.off, w.ns.len, base + w.coll.off, w.coll.len, base + w.key.off, w.key.len);
+}
+BD_HD bool kl_same_key(const uint8_t* base, const WriteRec& a, const WriteRec& b)
+{
+    return seg_equal(base, a.ns, b.ns) && seg_equal(base, a.coll, b.coll) && seg_equal(base, a.key, b.key);
+}
+
+BD_HD uint32_t kl_atomic_add(uint32_t* p, uint32_t n)
+{
+#if defined(__CUDA_ARCH__)
+    return atomicAdd(p, n);
+#else
+    const uint32_t b = *p; *p += n; return b;
+#endif
+}
+
+// Every write of a TxReadWriteSet as rwset.FromProtoBytes reads it, in baseEvaluator.Evaluate's terms (validator_keylevel.go:86-142):
+// on_write(namespace, collection, key, is_metadata) for each KVWrite{key = 1} and KVMetadataWrite{key = 1} of a namespace's KVRWSet and each
+// KVWriteHash{key_hash = 1} and KVMetadataWriteHash{key_hash = 1} of its collections.  false when a level does not parse.
+template <typename F>
+BD_HD bool kl_scan_rwset(const uint8_t* base, Seg results, F on_write)
+{
+    bool ok = true;
+    const bool top = scan_msg(base, results, BD_F(2), BD_F(1), [&](uint32_t, Seg nsb) {
+        if (!ok) return;
+        Seg name, kv; name.off = name.len = kv.off = kv.len = 0;          // NsReadWriteSet{namespace = 1, rwset = 2, collection_hashed_rwset = 3}
+        if (!scan_msg(base, nsb, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t f, Seg b) { if (f == 1) name = b; else if (f == 2) kv = b; })) { ok = false; return; }
+        // KVRWSet{reads = 1, range_queries_info = 2, writes = 3, metadata_writes = 4}; KVWrite{key = 1, is_delete = 2, value = 3},
+        // KVMetadataWrite{key = 1, entries = 2}
+        Seg none; none.off = none.len = 0;
+        if (!scan_msg(base, kv, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t g, Seg w) {
+                if (!ok || (g != 3 && g != 4)) return;
+                Seg key; key.off = key.len = 0;
+                if (!scan_msg(base, w, g == 3 ? BD_F(1) | BD_F(3) : BD_F(1) | BD_F(2), g == 3 ? BD_F(2) : 0, [&](uint32_t h, Seg k) { if (h == 1) key = k; })) { ok = false; return; }
+                on_write(name, none, key, g == 4);
+            })) ok = false;
+        if (!ok) return;
+        scan_msg(base, nsb, BD_F(3), 0, [&](uint32_t, Seg cb) {          // CollectionHashedReadWriteSet{collection_name = 1, hashed_rwset = 2, pvt_rwset_hash = 3}
+            if (!ok) return;
+            Seg cname, hashed; cname.off = cname.len = hashed.off = hashed.len = 0;
+            if (!scan_msg(base, cb, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg c) { if (g == 1) cname = c; else if (g == 2) hashed = c; })) { ok = false; return; }
+            // HashedRWSet{hashed_reads = 1, hashed_writes = 2, metadata_writes = 3}; KVWriteHash{key_hash = 1, is_delete = 2, value_hash = 3,
+            // is_purge = 4}, KVMetadataWriteHash{key_hash = 1, entries = 2}
+            if (!scan_msg(base, hashed, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg w) {
+                    if (!ok || (g != 2 && g != 3)) return;
+                    Seg key; key.off = key.len = 0;
+                    if (!scan_msg(base, w, g == 2 ? BD_F(1) | BD_F(3) : BD_F(1) | BD_F(2), g == 2 ? BD_F(2) | BD_F(4) : 0, [&](uint32_t h, Seg k) { if (h == 1) key = k; })) { ok = false; return; }
+                    on_write(name, cname, key, g == 3);
+                })) ok = false;
+        });
+    });
+    return top && ok;
+}
+
+// Appends the write records of transaction t (gone: only its metadata writes, for a transaction that never reaches VSCC) and enters its
+// metadata records into the metadata-write set.
+BD_HD void kl_emit(const uint8_t* base, Seg results, uint32_t t, TxDev& tx, KlArrays& kl, bool gone)
+{
+    uint32_t n = 0;
+    if (!kl_scan_rwset(base, results, [&](Seg, Seg, Seg, bool md) { if (md || !gone) n++; })) {
+        if (!gone) tx.kl_bad = 1;                                     // (a gone transaction's broken read/write set registers nothing, vpmanagerimpl.go:261-285)
+        return;
+    }
+    if (n == 0) return;
+    const uint32_t b = kl_atomic_add(kl.counter, n);
+    if (b + n > kl.W_cap || b + n < b) return;                        // overflow: the decide stage sees counter[0] > W_cap
+    tx.first_w = b; tx.n_w = n;
+    uint32_t q = b;
+    kl_scan_rwset(base, results, [&](Seg ns, Seg coll, Seg key, bool md) {
+        if (!md && gone) return;
+        WriteRec& w = kl.w[q];
+        w.ns = ns; w.coll = coll; w.key = key; w.tx = t; w.slot = 0xffffffffu; w.md = md ? 1 : 0; w.gone = gone ? 1 : 0; w.alias = 0; w.ns_idx = 0;
+        for (uint32_t k = 0; !gone && k < tx.n_ns; k++) if (seg_equal(base, tx.wr_ns[k], ns)) { w.ns_idx = (uint8_t)k; break; }
+        if (md) {
+            const uint64_t h = kl_rec_hash(base, w);
+            bool placed = false;
+            for (uint32_t probe = 0, pos = (uint32_t)h & (kl.md_size - 1); probe < kl.md_size; probe++, pos = (pos + 1) & (kl.md_size - 1)) {
+#if defined(__CUDA_ARCH__)
+                const uint64_t old = atomicCAS(reinterpret_cast<unsigned long long*>(kl.md_hash + pos), 0ull, (unsigned long long)h);
+#else
+                const uint64_t old = kl.md_hash[pos]; if (old == 0) kl.md_hash[pos] = h;
+#endif
+                if (old != 0 && old != h) continue;
+                const unsigned long long me = ((unsigned long long)t << 32) | q;
+#if defined(__CUDA_ARCH__)
+                atomicMin(kl.md_min + pos, me);
+#else
+                if (me < kl.md_min[pos]) kl.md_min[pos] = me;
+#endif
+                w.slot = pos;
+                placed = true; break;
+            }
+            if (!placed) kl.counter[1] = 1;
+        }
+        q++;
+    });
+}
+
+// extractDependenciesForTx (validator_keylevel.go:183-221) for a transaction the walk abandoned before dispatch_plan: the levels down to
+// ChaincodeAction.results, parsed as proto.Unmarshal parses them, whatever the header says.  A level that does not parse registers no
+// dependency; no action, or an action payload without a ChaincodeEndorsedAction, is where the reference dereferences past the end
+// (tx.Actions[0], cap.Action.ProposalResponsePayload) -- no dependency of that block can be trusted.
+BD_HD void kl_lenient(const uint8_t* base, Seg env, uint32_t t, TxDev& tx, KlArrays& kl)
+{
+    auto none = [](uint32_t, Seg) {};
+    Seg payload, data, hdr, a0, capb, act, prp, ext, results;
+    payload.off = payload.len = data.off = data.len = hdr.off = hdr.len = a0.off = a0.len = capb.off = capb.len = 0;
+    act.off = act.len = prp.off = prp.len = ext.off = ext.len = results.off = results.len = 0;
+    bool has_hdr = false, has_act = false, ok = true; uint32_t n_act = 0;
+    if (!scan_msg(base, env, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) { if (f == 1) payload = b; })) return;                 // Envelope
+    if (!scan_msg(base, payload, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) { if (f == 1) { hdr = b; has_hdr = true; } else data = b; })) return;
+    if (has_hdr && !scan_msg(base, hdr, BD_F(1) | BD_F(2), 0, none)) return;                                                      // Header
+    if (!scan_msg(base, data, BD_F(1), 0, [&](uint32_t, Seg b) {                                                                     // Transaction
+            if (!scan_msg(base, b, BD_F(1) | BD_F(2), 0, none)) ok = false;                                                       // TransactionAction
+            if (n_act++ == 0) a0 = b; }) || !ok) return;
+    if (n_act == 0) { kl.counter[1] = 1; return; }
+    scan_msg(base, a0, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) { if (f == 2) capb = b; });
+    if (!scan_msg(base, capb, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) { if (f == 2) { act = b; has_act = true; } })) return;   // ChaincodeActionPayload
+    if (!has_act) { kl.counter[1] = 1; return; }
+    if (!scan_msg(base, act, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) {                                                          // ChaincodeEndorsedAction
+            if (f == 1) prp = b; else if (!scan_msg(base, b, BD_F(1) | BD_F(2), 0, none)) ok = false; }) || !ok) return;           // Endorsement
+    if (!scan_msg(base, prp, BD_F(1) | BD_F(2), 0, [&](uint32_t f, Seg b) { if (f == 2) ext = b; })) return;                        // ProposalResponsePayload
+    if (!scan_msg(base, ext, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t f, Seg b) {                                    // ChaincodeAction
+            if (f == 1) results = b;
+            else if (f == 3) ok = ok && scan_msg(base, b, BD_F(2) | BD_F(3), BD_F(1), none);                                        // Response
+            else if (f == 4) ok = ok && scan_msg(base, b, BD_F(1) | BD_F(2) | BD_F(3), 0, none); }) || !ok) return;                  // ChaincodeID
+    kl_emit(base, results, t, tx, kl, true);
+}
+
 // alloc_end(n) must return the first index of n fresh endorsement-job slots (atomicAdd on the device, a counter on the host)
 template <typename Alloc>
-BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* channel, uint32_t channel_len, TxDev& tx, RawJob* raw,
-                   JobArrays& ja, Alloc alloc_end)
+BD_HD void walk_tx_core(const uint8_t* base, Seg env, uint32_t t, const uint8_t* channel, uint32_t channel_len, TxDev& tx, RawJob* raw,
+                        JobArrays& ja, Alloc alloc_end)
 {
     tx.early = TXC_NOT_VALIDATED; tx.htype = 0; tx.endorser_parse_ok = 0; tx.channel_ok = 0; tx.endorsements_parse_ok = 1; tx.overflow = 0;
     tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0; tx.creator_identity = -1; tx.creator_has_job = 0; tx.first_end_job = 0; tx.n_end_jobs = 0;
     tx.txid_ascii.off = tx.txid_ascii.len = 0; tx.phash_claimed.off = tx.phash_claimed.len = 0;
+    tx.results.off = tx.results.len = 0; tx.first_w = tx.n_w = 0; tx.kl_bad = 0;
     {
         ShaJobD z; for (int k = 0; k < 3; k++) { z.off[k] = 0; z.len[k] = 0; }
         ja.sha[t] = z; ja.sha[ja.J_cap + 2 * t] = z; ja.sha[ja.J_cap + 2 * t + 1] = z;
@@ -486,6 +669,8 @@ BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* chan
     tx.phash_claimed = pr.s[0];
     tx.endorser_parse_ok = 1;
     dispatch_plan(base, ch.s[2], has_prp, pr.present[1], pr.s[1], tx);
+    // key policy table installed: the writes the key-level checks walk (a transaction the dispatcher stops is walk_tx's)
+    if (ja.kl.w && tx.disp == TXC_VALID) kl_emit(base, tx.results, t, tx, ja.kl, false);
     // endorsements: one pass to count those that carry a signature, one to emit their jobs (contiguous, in endorsement order)
     uint32_t n_jobs = 0;
     {
@@ -529,6 +714,17 @@ BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* chan
     }
 }
 
+// The walk of one transaction.  With a key policy table, a transaction that does not reach the VSCC stage on structure alone (the walk
+// or the dispatcher stops it) still registers the dependencies of its metadata writes: it never signals a result, so a later writer of
+// the same key would wait for it forever (vpmanagerimpl.go:196-230).
+template <typename Alloc>
+BD_HD void walk_tx(const uint8_t* base, Seg env, uint32_t t, const uint8_t* channel, uint32_t channel_len, TxDev& tx, RawJob* raw,
+                   JobArrays& ja, Alloc alloc_end)
+{
+    walk_tx_core(base, env, t, channel, channel_len, tx, raw, ja, alloc_end);
+    if (ja.kl.w && !(tx.endorser_parse_ok && tx.disp == TXC_VALID)) kl_lenient(base, env, t, tx, ja.kl);
+}
+
 // One signature job: identity lookup in the MSP table, DER / low-S gate, operands for the verify kernel, and (creator jobs) the
 // identity index written back into the transaction record.
 BD_HD void resolve_job(const uint8_t* base, uint32_t j, const RawJob* raw, const MspDev& msp, JobArrays& ja, TxDev* txs)
@@ -557,6 +753,10 @@ BD_HD void resolve_job(const uint8_t* base, uint32_t j, const RawJob* raw, const
     }
 }
 
+// One slot of the key policy table: the entry's namespace, collection and key lie back to back at kp_blob + off.  hash 0 = empty.
+// root: a node of the policy array, KP_UNDECIDABLE, or KP_REMOVED.
+struct KpSlot { uint64_t hash; uint32_t off, ns_len, coll_len, key_len; int32_t root; uint32_t pad; };
+
 // ---- policy evaluator: cauthdsl.go:24-92, `used` as a bit mask over at most BD_MAX_SIGNERS signers ------------------------
 // Several policies share one node array (one tree per chaincode namespace); ns_* name the root of each.
 // Node types: 0 = NOutOf(n), 1 = SignedBy(principal n), 2 = ImplicitMeta with threshold n (implicitmeta.go:69-103).
@@ -572,7 +772,93 @@ struct PolicyDev {
     const uint8_t* coll_ns_blob = nullptr; const uint32_t* coll_ns_off = nullptr; const uint8_t* coll_name_blob = nullptr;
     const uint32_t* coll_name_off = nullptr; const int32_t* coll_root = nullptr; const uint64_t* coll_hash = nullptr; const int32_t* coll_idx = nullptr;
     uint32_t coll_size = 0;
+    // fabgpu_key_policies: key-level validation parameters, kp_size slots (a power of two) keyed by kl_key_hash; kp_size = 0: no table
+    const KpSlot* kp_slots = nullptr; const uint8_t* kp_blob = nullptr; uint32_t kp_size = 0;
 };
+
+// root of the validation parameter of (ns, coll, key) (all in the block), -1 when the table holds none
+BD_HD int32_t kp_find(const PolicyDev& pol, const uint8_t* base, Seg ns, Seg coll, Seg key)
+{
+    const uint64_t h = kl_key_hash(base + ns.off, ns.len, base + coll.off, coll.len, base + key.off, key.len);
+    for (uint32_t probe = 0, pos = (uint32_t)h & (pol.kp_size - 1); probe < pol.kp_size; probe++, pos = (pos + 1) & (pol.kp_size - 1)) {
+        const KpSlot s = pol.kp_slots[pos];
+        if (s.hash == 0) return -1;
+        if (s.hash != h || s.ns_len != ns.len || s.coll_len != coll.len || s.key_len != key.len) continue;
+        const uint8_t* e = pol.kp_blob + s.off;
+        if (bytes_equal(e, base + ns.off, ns.len) && bytes_equal(e + ns.len, base + coll.off, coll.len) &&
+            bytes_equal(e + ns.len + coll.len, base + key.off, key.len))
+            return s.root == KP_REMOVED ? -1 : s.root;
+    }
+    return -1;
+}
+
+// metadata-write set entry of record w's key, 0xffffffff when no transaction of the block metadata-writes a key with its hash
+BD_HD uint32_t kl_md_find(const KlArrays& kl, const uint8_t* base, const WriteRec& w)
+{
+    const uint64_t h = kl_rec_hash(base, w);
+    for (uint32_t probe = 0, pos = (uint32_t)h & (kl.md_size - 1); probe < kl.md_size; probe++, pos = (pos + 1) & (kl.md_size - 1)) {
+        const uint64_t k = kl.md_hash[pos];
+        if (k == 0) return 0xffffffffu;
+        if (k == h) return pos;
+    }
+    return 0xffffffffu;
+}
+
+// Decide stage, every transaction t (before decide_tx): marks t as a metadata writer, and an entry whose metadata writers do not all
+// share its first writer's key as mixed.
+BD_HD void kl_mark(const uint8_t* base, uint32_t t, const TxDev& tx, KlArrays& kl)
+{
+    uint8_t mark = 0;
+    for (uint32_t q = 0; q < tx.n_w; q++) {
+        const WriteRec& w = kl.w[tx.first_w + q];
+        if (!w.md || w.slot == 0xffffffffu) continue;
+        mark = 2;
+        if (!kl_same_key(base, kl.w[(uint32_t)kl.md_min[w.slot]], w)) {
+#if defined(__CUDA_ARCH__)
+            atomicOr(kl.md_sum + w.slot, KL_SUM_MIXED);
+#else
+            kl.md_sum[w.slot] |= KL_SUM_MIXED;
+#endif
+        }
+    }
+    kl.conflicted[t] = mark;
+}
+
+// The resolve rule, applied to the marked transactions in index order (vpmanagerimpl.go:196-230).  A transaction t that writes a key some
+// earlier transaction j metadata-wrote waits for j's VSCC result for that namespace, and fails with a policy error if any is nil.  It is
+// read off j's final flag (final when t's turn comes; the duplicate-tx-id pass runs after VSCC): VALID -> nil; ENDORSEMENT_POLICY_FAILURE
+// with one validated namespace (the written one) -> non-nil; anything else -> undetermined: j never reached that namespace's VSCC
+// (rejected before it, or the dispatcher stopped at another namespace first, dispatcher.go:190-217) and the reference would wait
+// forever -- or j is one the device did not decide.  Undetermined gives NOT_VALIDATED, else any nil gives ENDORSEMENT_POLICY_FAILURE,
+// else t keeps its own decision.  Each entry's md_sum folds in its writers as they are passed, so a step costs t's own records: a key
+// that every transaction of the block writes and metadata-writes costs the block O(T), not O(T^2).
+BD_HD void kl_resolve_step(uint32_t t, const TxDev* txs, KlArrays& kl, uint8_t* flags)
+{
+    const TxDev& x = txs[t];
+    const uint8_t mark = kl.conflicted[t];
+    uint8_t f = flags[t];
+    if ((mark & 1) && (f == TXC_VALID || f == TXC_ENDORSEMENT_POLICY_FAILURE)) {
+        uint32_t s = 0;
+        for (uint32_t q = 0; q < x.n_w; q++) {
+            const WriteRec& w = kl.w[x.first_w + q];
+            if (w.slot == 0xffffffffu) continue;
+            const uint32_t u = kl.md_sum[w.slot];
+            if (!(u & KL_SUM_ANY)) continue;                          // no earlier writer of this hash
+            s |= (w.alias || (u & KL_SUM_MIXED)) ? KL_SUM_UNDET : (u & (KL_SUM_NIL | KL_SUM_UNDET));
+        }
+        f = (s & KL_SUM_UNDET) ? TXC_NOT_VALIDATED : (s & KL_SUM_NIL) ? TXC_ENDORSEMENT_POLICY_FAILURE : f;
+        flags[t] = f;
+    }
+    if (mark & 2) {
+        const bool gone = x.n_w && kl.w[x.first_w].gone;
+        const uint32_t st = KL_SUM_ANY | (f == TXC_VALID && !gone ? KL_SUM_NIL
+                                          : f == TXC_ENDORSEMENT_POLICY_FAILURE && x.n_ns == 1 && !gone ? 0u : KL_SUM_UNDET);
+        for (uint32_t q = 0; q < x.n_w; q++) {
+            const WriteRec& w = kl.w[x.first_w + q];
+            if (w.md && w.slot != 0xffffffffu) kl.md_sum[w.slot] |= st;
+        }
+    }
+}
 
 BD_HD uint64_t coll_key_hash(const uint8_t* ns, uint32_t ns_len, const uint8_t* coll, uint32_t coll_len)
 {
@@ -684,9 +970,11 @@ BD_HD int32_t policy_root(const PolicyDev& pol, const uint8_t* base, Seg ns)
 // one, cannot be decided here: TXC_NOT_VALIDATED hands the
 // transaction to the CPU validator (the reference deserialises and validates ANY certificate of the channel's CAs,
 // msgvalidation.go:40-57, and reads chaincode definitions from the ledger, dispatcher.go:224-277).
+// kl: the block's write records and metadata-write set, used while a key policy table is installed (pol.kp_size != 0); decide_tx then
+// sets bit 0 of kl->conflicted[t] when an earlier transaction metadata-wrote a key t writes, for the resolve stage (kl_resolve_step).
 template <typename SigOk>
 BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const MspDev& msp, const PolicyDev& pol, SigOk sig_ok,
-                        const int32_t* job_identity, const uint8_t* digests, uint32_t J_cap, uint64_t* txid_hash_out)
+                        const int32_t* job_identity, const uint8_t* digests, uint32_t J_cap, uint64_t* txid_hash_out, KlArrays* kl = nullptr)
 {
     const char hex[] = "0123456789abcdef";
     if (tx.early != TXC_NOT_VALIDATED) return tx.early;
@@ -714,13 +1002,37 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
     // namespace as baseEvaluator.Evaluate (validator_keylevel.go:86-142) walks its writes: the collection's policy for each named
     // collection written, the chaincode policy for public writes and collections without a name, and the chaincode policy when
     // nothing else was checked (CheckCCEPIfNoEPChecked, v20.go:149-163: the invoked chaincode that only reads).
-    int32_t roots[BD_MAX_NS], need[BD_MAX_NS + BD_MAX_COLL]; int n_need = 0;
-    auto add = [&](int32_t r) { for (int k = 0; k < n_need; k++) if (need[k] == r) return; need[n_need++] = r; };
+    int32_t roots[BD_MAX_NS], need[BD_MAX_NEED]; int n_need = 0; bool too_many = false;
+    auto add = [&](int32_t r) {
+        for (int k = 0; k < n_need; k++) if (need[k] == r) return;
+        if (n_need == BD_MAX_NEED) too_many = true; else need[n_need++] = r;
+    };
     for (int i = 0; i < tx.n_ns; i++) {
         roots[i] = policy_root(pol, base, tx.wr_ns[i]);
         if (roots[i] < 0) return TXC_NOT_VALIDATED;                   // no chaincode definition on the device
     }
-    if (pol.coll_size == 0) {
+    const bool keylevel = kl && pol.kp_size;
+    if (keylevel) {
+        // checkSBAndCCEP per write (validator_keylevel.go:37-84): the key's validation parameter if it has one (and then not the
+        // chaincode's or collection's policy for that write), else CheckCCEPIfNotChecked; CheckCCEPIfNoEPChecked for a namespace none
+        // of whose writes checked anything -- one without writes, since every write checks something.
+        if (kl->counter[0] > kl->W_cap || kl->counter[1] || tx.kl_bad) return TXC_NOT_VALIDATED;   // records lost, or unreadable
+        uint32_t has_w = 0;
+        for (uint32_t q = 0; q < tx.n_w; q++) {
+            const WriteRec& w = kl->w[tx.first_w + q];
+            // With a collection table, a collection it does not hold may be one the chaincode does not define, where the reference skips
+            // the key's parameter (CollConfigNotDefinedError, validator_keylevel.go:53-54) and then fails: not decided here, VP or not.
+            const int32_t cr = w.coll.len && pol.coll_size ? coll_policy_root(pol, base, w.ns, w.coll) : -1;
+            if (w.coll.len && pol.coll_size && cr < 0) return TXC_NOT_VALIDATED;
+            int32_t r = kp_find(pol, base, w.ns, w.coll, w.key);
+            if (r == KP_UNDECIDABLE) return TXC_NOT_VALIDATED;
+            if (r < 0) r = w.coll.len && pol.coll_size ? cr : roots[w.ns_idx];
+            add(r);
+            has_w |= 1u << w.ns_idx;
+        }
+        for (int i = 0; i < tx.n_ns; i++) if (!((has_w >> i) & 1u)) add(roots[i]);
+        if (too_many) return TXC_NOT_VALIDATED;
+    } else if (pol.coll_size == 0) {
         for (int i = 0; i < tx.n_ns; i++) add(roots[i]);
     } else {
         if (tx.n_coll > BD_MAX_COLL) return TXC_NOT_VALIDATED;          // more collections than the walk records
@@ -756,10 +1068,25 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
         if (n_signers >= BD_MAX_SIGNERS) return TXC_NOT_VALIDATED;
         signer[n_signers++] = pol.principal_bits ? idn : msp.valid[idn] ? msp.msp_code[idn] : -1;
     }
-    for (int k = 0; k < n_need; k++) {
+    bool pass = true;
+    for (int k = 0; k < n_need && pass; k++) {
         uint64_t used = 0;
-        if (!eval_policy(pol, need[k], signer, n_signers, used, 0)) return TXC_ENDORSEMENT_POLICY_FAILURE;
+        pass = eval_policy(pol, need[k], signer, n_signers, used, 0);
     }
+    if (keylevel) {                                                   // an earlier metadata write of a key t writes: resolved later
+        bool dep = false;
+        for (uint32_t q = 0; q < tx.n_w; q++) {
+            WriteRec& w = kl->w[tx.first_w + q];
+            if (!w.md) w.slot = kl_md_find(*kl, base, w);
+            if (w.slot == 0xffffffffu) continue;
+            const unsigned long long m = kl->md_min[w.slot];
+            if ((uint32_t)(m >> 32) >= t) continue;                   // every metadata writer of this hash comes later
+            dep = true;
+            if (!kl_same_key(base, kl->w[(uint32_t)m], w)) w.alias = 1;
+        }
+        if (dep) kl->conflicted[t] |= 1;
+    }
+    if (!pass) return TXC_ENDORSEMENT_POLICY_FAILURE;
     uint64_t hsh = 1469598103934665603ull;
     for (uint32_t k = 0; k < tx.txid_ascii.len; k++) hsh = (hsh ^ base[tx.txid_ascii.off + k]) * 1099511628211ull;
     *txid_hash_out = hsh;

@@ -35,14 +35,53 @@ __global__ void __launch_bounds__(128)
 block_decide_kernel(const uint8_t* __restrict__ block, const TxDev* __restrict__ txs, uint32_t T, MspDev msp, PolicyDev pol,
                     const uint32_t* __restrict__ mask, const uint8_t* __restrict__ gate_ok, const int32_t* __restrict__ job_identity,
                     const uint8_t* __restrict__ digests, uint32_t J_cap,
-                    uint8_t* __restrict__ flags, uint64_t* __restrict__ txid_hash, Seg* __restrict__ txid_seg)
+                    uint8_t* __restrict__ flags, uint64_t* __restrict__ txid_hash, Seg* __restrict__ txid_seg, KlArrays kl)
 {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     uint64_t h = 0;
-    flags[t] = decide_tx(block, txs[t], t, msp, pol, [&](uint32_t j) { return gate_ok[j] && ((mask[j >> 5] >> (j & 31)) & 1u); }, job_identity, digests, J_cap, &h);
+    if (kl.w) kl_mark(block, t, txs[t], kl);
+    flags[t] = decide_tx(block, txs[t], t, msp, pol, [&](uint32_t j) { return gate_ok[j] && ((mask[j >> 5] >> (j & 31)) & 1u); }, job_identity, digests, J_cap, &h,
+                         kl.w ? &kl : nullptr);
     txid_hash[t] = h;
     txid_seg[t] = txs[t].txid_ascii;
+}
+
+// Key policy table installed: the resolve stage.  One CTA: the marked transactions (a dependency, or metadata writes) are compacted by a
+// block-wide scan, then one thread runs kl_resolve_step over them in index order, so a chain sees final flags; each step costs the
+// transaction's own records.
+__global__ void __launch_bounds__(256)
+block_kl_resolve_kernel(const TxDev* __restrict__ txs, uint32_t T, KlArrays kl, uint8_t* __restrict__ flags)
+{
+    __shared__ uint32_t warp_sum[32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, per = (T + blockDim.x - 1) / blockDim.x;
+    const uint32_t lo = min(T, tid * per), hi = min(T, lo + per);
+    uint32_t c = 0;
+    for (uint32_t t = lo; t < hi; t++) c += kl.conflicted[t] != 0;
+    uint32_t x = c;                                                 // inclusive scan within the warp, then over the warps
+    for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, d); if (lane >= d) x += y; }
+    if (lane == 31) warp_sum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t v = lane < blockDim.x / 32 ? warp_sum[lane] : 0;
+        for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += y; }
+        warp_sum[lane] = v;
+    }
+    __syncthreads();
+    uint32_t off = x - c + (warp ? warp_sum[warp - 1] : 0);
+    for (uint32_t t = lo; t < hi; t++) if (kl.conflicted[t]) kl.clist[off++] = t;
+    const uint32_t total = warp_sum[31];
+    __syncthreads();
+    if (tid != 0) return;
+    for (uint32_t k = 0; k < total; k++) kl_resolve_step(kl.clist[k], txs, kl, flags);
+}
+
+// fabgpu_key_policies_update: writes the changed slots of the key policy table
+__global__ void __launch_bounds__(256)
+kp_scatter_kernel(KpSlot* __restrict__ slots, const uint32_t* __restrict__ idx, const KpSlot* __restrict__ val, uint32_t n)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) slots[idx[i]] = val[i];
 }
 
 // ---- bccsp-level batch with the gates on the device (SURVEY.md section 8f rank 3) ------------------------------------------

@@ -25,6 +25,7 @@
 #include "cuda_owned.hpp"
 #include "sha256.cuh"
 #include "blockdev_kernels.cuh"
+#include "keypolicy.hpp"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -212,9 +213,15 @@ struct fabgpu_ctx {
         DevArray<uint32_t> pbits; int32_t pbits_words = 0;            // fabgpu_msp_principal_bits, null = MSP-id member matching
         DevArray<uint8_t> cp_ns_blob, cp_name_blob; DevArray<uint32_t> cp_ns_off, cp_name_off;   // fabgpu_collection_policies, cp_size = 0: none
         DevArray<int32_t> cp_root, cp_idx; DevArray<uint64_t> cp_hash; uint32_t cp_size = 0;
+        // fabgpu_key_policies: slots, entry bytes, and the table's nodes after the configured ones in `nodes`; kp_size = 0: none.
+        // kp_idx / kp_val stage the changed slots of an update.
+        DevArray<bdev::KpSlot> kp_slots, kp_val; DevArray<uint8_t> kp_blob; DevArray<uint32_t> kp_idx; uint32_t kp_size = 0; int32_t kp_n_nodes = 0;
+        bool nodes_lost = false;                                      // a failed key-table call lost the configured nodes: no blocks
         DevArray<uint64_t> ht_hash; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
         bool all_slots = true; int classes = 0;                    // which non-big classes the identities' keys fall in (CLASS_*)
     } dm;
+    bdev::KeyPolicyTable kpt;                                      // host mirror of the key policy table
+    std::atomic<uint32_t> kl_hint{BD_WRITES_HINT};                 // write records per transaction the block slots are sized for; grows on overflow
     struct GateBufs {                          // fabgpu_bccsp_verify_batch with device-side gates
         // Four groups, each grown together (gate_bufs_reserve).  A group's capacity is read from the array it grows last: signatures
         // (n_cap), signature and digest bytes, keys.
@@ -238,8 +245,10 @@ struct fabgpu_ctx {
         DevArray<bdev::Seg> d_seg; DevArray<uint4> d_scal;
         HostArray<uint64_t> h_hash; HostArray<bdev::Seg> h_seg; HostArray<uint32_t> h_counter, h_env_off; HostArray<uint8_t> h_flags;
         size_t tx_cap() const { return h_flags.bytes(); }
+        // key policy table installed: write records, the metadata-write set, conflicted transactions (grown together, per block)
+        DevArray<bdev::WriteRec> d_w; DevArray<uint64_t> d_md_hash; DevArray<unsigned long long> d_md_min; DevArray<uint32_t> d_md_sum, d_clist; DevArray<uint8_t> d_conf;
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
-        bool busy = false, on_device = false, use_ev = false; size_t T = 0; const uint8_t* block = nullptr;
+        bool busy = false, on_device = false, use_ev = false, kl_on = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
@@ -1634,6 +1643,7 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
     // blocks already enqueued on a slot were launched with the OLD tables (passed by value): let them finish before those go away
     for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
     dm = fabgpu_ctx::DevMsp();
+    ctx->kpt = bdev::KeyPolicyTable();                       // its SignedBy nodes index the principals being replaced
     // MSP-id codes: equal strings <=> equal codes, shared between identities and policy principals
     std::unordered_map<std::string, int32_t> codes;
     auto code_of = [&](const std::string& sname) { auto it = codes.find(sname); if (it != codes.end()) return it->second; int32_t c = (int32_t)codes.size(); codes[sname] = c; return c; };
@@ -1878,6 +1888,95 @@ int fabgpu_collection_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const ui
     return FABGPU_OK;
 }
 
+// Brings the device copy of the key policy table up to ctx->kpt after a call changed it: the whole table after a rebuild, else the
+// changed slots (scattered by kp_scatter_kernel), the new entry bytes and the new nodes.  Arrays grow by doubling, so an update costs
+// what it changed.
+static int kp_upload(fabgpu_ctx* ctx)
+{
+    auto& dm = ctx->dm; auto& k = ctx->kpt;
+    if (!k.installed()) { dm.kp_slots = {}; dm.kp_blob = {}; dm.kp_val = {}; dm.kp_idx = {}; dm.kp_size = 0; dm.kp_n_nodes = 0; return FABGPU_OK; }
+    dm.kp_size = 0;                                              // until the copy is complete
+    auto grown = [](size_t need, size_t have) { return need <= have ? have : std::max(need, 2 * have); };
+    // nodes: the configured ones, then the table's
+    const size_t cfg = 16 * (size_t)dm.n_nodes, tail = 4 * k.nodes.size();
+    if (k.full || cfg + tail + 8 > dm.nodes.bytes()) {
+        std::vector<int32_t> all;
+        for (const auto& nd : ctx->policy) { all.push_back(nd.type); all.push_back(nd.n); all.push_back(nd.first_child); all.push_back(nd.n_children); }
+        all.insert(all.end(), k.nodes.begin(), k.nodes.end());
+        if (int rc = dm.nodes.reserve(ctx, grown(cfg + tail + 8, dm.nodes.bytes()))) return rc;
+        if (!all.empty()) CK(ctx, cudaMemcpy(dm.nodes.get(), all.data(), 4 * all.size(), cudaMemcpyHostToDevice));
+    } else if (k.nodes.size() > k.nodes_from) {
+        CK(ctx, cudaMemcpy(reinterpret_cast<uint8_t*>(dm.nodes.get()) + cfg + 4 * k.nodes_from, k.nodes.data() + k.nodes_from,
+                           4 * (k.nodes.size() - k.nodes_from), cudaMemcpyHostToDevice));
+    }
+    // entry bytes (slack: bytes_equal reads whole aligned words)
+    if (k.full || k.blob.size() + 8 > dm.kp_blob.bytes()) {
+        if (int rc = dm.kp_blob.reserve(ctx, grown(k.blob.size() + 8, dm.kp_blob.bytes()))) return rc;
+        if (!k.blob.empty()) CK(ctx, cudaMemcpy(dm.kp_blob.get(), k.blob.data(), k.blob.size(), cudaMemcpyHostToDevice));
+    } else if (k.blob.size() > k.blob_from) {
+        CK(ctx, cudaMemcpy(dm.kp_blob.get() + k.blob_from, k.blob.data() + k.blob_from, k.blob.size() - k.blob_from, cudaMemcpyHostToDevice));
+    }
+    // slots
+    const size_t sb = sizeof(bdev::KpSlot) * k.slots.size();
+    if (k.full || dm.kp_slots.bytes() != sb) {
+        dm.kp_slots = {};
+        if (int rc = dm.kp_slots.reserve(ctx, sb)) return rc;
+        CK(ctx, cudaMemcpy(dm.kp_slots.get(), k.slots.data(), sb, cudaMemcpyHostToDevice));
+    } else if (!k.dirty.empty()) {
+        const size_t n = k.dirty.size();
+        std::vector<bdev::KpSlot> val(n);
+        for (size_t i = 0; i < n; i++) val[i] = k.slots[k.dirty[i]];
+        if (int rc = dm.kp_idx.reserve(ctx, grown(4 * n, dm.kp_idx.bytes()))) return rc;
+        if (int rc = dm.kp_val.reserve(ctx, grown(sizeof(bdev::KpSlot) * n, dm.kp_val.bytes()))) return rc;
+        CK(ctx, cudaMemcpy(dm.kp_idx.get(), k.dirty.data(), 4 * n, cudaMemcpyHostToDevice));
+        CK(ctx, cudaMemcpy(dm.kp_val.get(), val.data(), sizeof(bdev::KpSlot) * n, cudaMemcpyHostToDevice));
+        bdev::kp_scatter_kernel<<<(unsigned)((n + 255) / 256), 256>>>(dm.kp_slots.get(), dm.kp_idx.get(), dm.kp_val.get(), (uint32_t)n);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaDeviceSynchronize());
+    }
+    dm.kp_size = (uint32_t)k.slots.size(); dm.kp_n_nodes = k.n_nodes();
+    return FABGPU_OK;
+}
+
+static int key_policies(fabgpu_ctx* ctx, bool replace, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off,
+                        const uint8_t* coll_blob, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off, const int32_t* root, int n)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm;
+    int rc = drain_block_streams(ctx); if (rc) return rc;
+    // a refused call leaves the table as it was (apply checks everything before it changes anything)
+    if (const char* err = ctx->kpt.apply(replace, dm.n_nodes, dm.n_principals, nodes, n_nodes, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, root, n)) {
+        ctx->last_error = err; return FABGPU_E_ARG;
+    }
+    if ((rc = kp_upload(ctx))) {
+        // A failed copy removes the table.  The node array also holds the configured policies, and growing it frees it first: put
+        // those back, and if even that fails, refuse blocks until fabgpu_msp_configure installs them again.
+        const std::string err = ctx->last_error;
+        ctx->kpt = bdev::KeyPolicyTable(); dm.kp_size = 0; dm.kp_n_nodes = 0;
+        std::vector<int32_t> cfg;
+        for (const auto& nd : ctx->policy) { cfg.push_back(nd.type); cfg.push_back(nd.n); cfg.push_back(nd.first_child); cfg.push_back(nd.n_children); }
+        const size_t bytes = 4 * cfg.size();
+        dm.nodes_lost = !(bytes + 8 <= dm.nodes.bytes() || dm.nodes.reserve(ctx, bytes + 8) == FABGPU_OK) ||
+                        (bytes && cudaMemcpy(dm.nodes.get(), cfg.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess);
+        ctx->last_error = err;
+    }
+    return rc;
+}
+
+int fabgpu_key_policies(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob,
+                        const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off, const int32_t* root, int n)
+{
+    return key_policies(ctx, true, nodes, n_nodes, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, root, n);
+}
+
+int fabgpu_key_policies_update(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob,
+                               const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off, const int32_t* root, int n)
+{
+    return key_policies(ctx, false, nodes, n_nodes, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, root, n);
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -1952,6 +2051,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
         split.resize(2 * n_env + 2);
         for (size_t i = 0; i < n_env; i++) { split[2 * i] = envs[i].off; split[2 * i + 1] = envs[i].off + envs[i].len; }
     }
+    if (dm.nodes_lost) { ctx->last_error = "policy nodes lost by a failed fabgpu_key_policies call: call fabgpu_msp_configure again"; return FABGPU_E_CUDA; }
     const size_t T = n_env;
     db.T = T; db.block = block;
     if (T == 0) return FABGPU_OK;
@@ -1986,9 +2086,26 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     pol.principal_bits = dm.pbits.get(); pol.bits_words = dm.pbits_words;
     pol.coll_ns_blob = dm.cp_ns_blob.get(); pol.coll_ns_off = dm.cp_ns_off.get(); pol.coll_name_blob = dm.cp_name_blob.get(); pol.coll_name_off = dm.cp_name_off.get();
     pol.coll_root = dm.cp_root.get(); pol.coll_hash = dm.cp_hash.get(); pol.coll_idx = dm.cp_idx.get(); pol.coll_size = dm.cp_size;
+    pol.n_nodes = dm.n_nodes + dm.kp_n_nodes; pol.kp_slots = dm.kp_slots.get(); pol.kp_blob = dm.kp_blob.get(); pol.kp_size = dm.kp_size;
+    bdev::KlArrays kl;                                        // key policy table installed: write records and the metadata-write set
+    db.kl_on = dm.kp_size != 0;
+    if (db.kl_on) {
+        const size_t W_cap = T * ctx->kl_hint.load();
+        size_t md = 64; while (md < 2 * W_cap) md <<= 1;
+        Grow grow{ctx};
+        grow(db.d_w, sizeof(bdev::WriteRec) * W_cap); grow(db.d_md_hash, 8 * md); grow(db.d_clist, 4 * T); grow(db.d_conf, T);
+        grow(db.d_md_min, 8 * md); grow(db.d_md_sum, 4 * md);
+        if (grow.rc) return grow.rc;
+        CK(ctx, cudaMemsetAsync(db.d_md_hash.get(), 0, 8 * md, ds.stream.get()));
+        CK(ctx, cudaMemsetAsync(db.d_md_min.get(), 0xff, 8 * md, ds.stream.get()));
+        CK(ctx, cudaMemsetAsync(db.d_md_sum.get(), 0, 4 * md, ds.stream.get()));
+        kl.w = db.d_w.get(); kl.W_cap = (uint32_t)W_cap; kl.counter = db.d_counter.get() + 2; kl.md_hash = db.d_md_hash.get();
+        kl.md_min = db.d_md_min.get(); kl.md_sum = db.d_md_sum.get(); kl.md_size = (uint32_t)md; kl.conflicted = db.d_conf.get(); kl.clist = db.d_clist.get();
+        db.W_cap = W_cap;
+    }
     const bool need_q = (dm.classes & CLASS_GENERIC) != 0;   // only the generic arithmetic reads the key itself
     bdev::JobArrays ja; ja.sha = db.d_sha.get(); ja.r = db.d_r.get(); ja.s = db.d_s.get(); ja.key_slot = db.d_ks.get(); ja.identity = db.d_ident.get(); ja.qx = need_q ? db.d_qx.get() : nullptr;
-    ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T;
+    ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T; ja.kl = kl;
     const uint32_t cnt = (uint32_t)T, E_cap = (uint32_t)(J_cap - T);
     // One copy, then the walk.  (Copying in chunks with a walk per chunk was measured slower, the more chunks the slower: hashing a
     // 4.6 KB payload is a long chain of dependent rounds per thread however few
@@ -2014,8 +2131,13 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     if (rc) return rc;
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4].get(), st));
     bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), db.d_txs.get(), cnt, m, pol, db.d_mask.get(), db.d_gate.get(), db.d_ident.get(), db.d_dig.get(), (uint32_t)J_cap, db.d_flags.get(),
-                                                               db.d_hash.get(), db.d_seg.get());
+                                                               db.d_hash.get(), db.d_seg.get(), kl);
     ctx->launches++;
+    if (db.kl_on) {
+        bdev::block_kl_resolve_kernel<<<1, 256, 0, st>>>(db.d_txs.get(), cnt, kl, db.d_flags.get());
+        ctx->launches++;
+        CK(ctx, cudaMemcpyAsync(db.h_counter.get(), db.d_counter.get(), 16, cudaMemcpyDeviceToHost, st));   // write records used
+    }
     CK(ctx, cudaGetLastError());
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[5].get(), st));
     CK(ctx, cudaMemcpyAsync(db.h_flags.get(), db.d_flags.get(), T, cudaMemcpyDeviceToHost, st));
@@ -2041,6 +2163,11 @@ static int block_finish(fabgpu_ctx* ctx, int slot, uint8_t* flags)
     auto t3 = now();
     if (T == 0) return FABGPU_OK;
     memcpy(flags, db.h_flags.get(), T);
+    if (db.kl_on && db.h_counter.get()[2] > db.W_cap) {        // write records overflowed (that block's flags say 254): size later blocks for it
+        const uint32_t want = (uint32_t)((db.h_counter.get()[2] + T - 1) / T) + 1;
+        uint32_t cur = ctx->kl_hint.load();
+        while (cur < want && !ctx->kl_hint.compare_exchange_weak(cur, want)) {}
+    }
     {
         // flat open-addressing table keyed by the 64-bit tx-id hash (0 = empty); equal hashes are confirmed on the bytes
         size_t cap = 16; while (cap < 4 * T) cap <<= 1;

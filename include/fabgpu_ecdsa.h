@@ -268,6 +268,34 @@ int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, 
 int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const int32_t* ns_root, int n_ns);
 int fabgpu_collection_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob,
                                const uint32_t* coll_off, const int32_t* coll_root, int n);
+/* Key-level endorsement policies (state-based endorsement; core/common/validation/statebased/validator_keylevel.go:37-142,
+ * vpmanagerimpl.go:196-362).  Also a refinement: it drains the block slots, and fabgpu_msp_configure clears it.
+ *   _key_policies replaces the table.  Entry i maps (namespace ns[i], collection coll[i], key key[i]) -- three blobs with (n+1)
+ *       offsets each; the collection is empty for a public key, and for a private-data key the key is its 32-byte key hash -- to
+ *       the validation parameter compiled to `nodes` (n_nodes x 4 ints in fabgpu_msp_configure's format, NOutOf and SignedBy only,
+ *       child indices counted within this call's array, SignedBy indexing fabgpu_msp_configure's principals): root[i] is a node of
+ *       this call's array, or -2 when the key's parameter is not one the device may decide (it does not translate, or names a
+ *       principal outside the configured list); a transaction writing such a key is flagged 254.  The library appends the nodes
+ *       after the configured ones.  n = 0 with n_nodes = 0 removes the table.
+ *   _key_policies_update upserts entries into the installed table with the same arguments; root -1 removes an entry (removing an
+ *       absent key does nothing).  Its cost follows the size of the change, not of the table: what a peer calls after committing
+ *       each block, with the validation parameters that block's valid metadata writes set or cleared.
+ *   While a table is installed, each write of a validated namespace -- public write, public metadata write, hashed write, hashed
+ *   metadata write -- is checked against its key's entry if it has one and then not against its chaincode or collection policy;
+ *   otherwise against its collection's policy (with a collection table; a written collection without an entry is flagged 254) or
+ *   its chaincode's.  A validated namespace without writes is checked against its chaincode policy.  More than 16 distinct
+ *   policies for one transaction is flagged 254.  A transaction that writes a key some earlier transaction of the block
+ *   metadata-wrote waits for that transaction's result: ENDORSEMENT_POLICY_FAILURE (10) if it was VALID, its own flag if it failed
+ *   its policy for its only namespace, and 254 in every other case (the reference would wait for a result that never comes).
+ *   Both calls return FABGPU_E_ARG with a fabgpu_last_error text, and keep the previous table, for NULL arrays with n > 0,
+ *   decreasing offsets, a node type other than 0 or 1, a child or root out of range, a cycle, a tree deeper than 12, a principal
+ *   out of range, a (namespace, collection, key) given twice, -1 in a replacing call, and an update with no table installed. */
+int fabgpu_key_policies(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off,
+                        const uint8_t* coll_blob, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off,
+                        const int32_t* root, int n);
+int fabgpu_key_policies_update(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off,
+                               const uint8_t* coll_blob, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off,
+                               const int32_t* root, int n);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their

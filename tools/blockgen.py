@@ -72,16 +72,41 @@ def collection_hashed_rwset(n_writes, n_metadata_writes, n_reads, tag=b"k") -> b
                      for i in range(n_metadata_writes)))
 
 
+def _md_entry() -> bytes:
+    """one KVMetadataEntry{name=1, value=2}: a validation parameter"""
+    return pb.f_bytes(2, pb.f_bytes(1, b"VALIDATION_PARAMETER") + pb.f_bytes(2, b"ep"))
+
+
+def named_kv_rwset(n_reads, writes, md_writes, tag) -> bytes:
+    """kv_rwset with named keys: KVWrite{key=1, value=3} per key of `writes` (or int: kv_rwset's keys), then KVMetadataWrite{key=1,
+    entries=2} per key of md_writes."""
+    out = kv_rwset(n_reads, writes if isinstance(writes, int) else 0, tag)
+    if not isinstance(writes, int):
+        out += b"".join(pb.f_bytes(3, pb.f_bytes(1, k.encode()) + pb.f_bytes(3, b"value")) for k in writes)
+    return out + b"".join(pb.f_bytes(4, pb.f_bytes(1, k.encode()) + _md_entry()) for k in md_writes)
+
+
+def key_hash(key: str) -> bytes:
+    """KVWriteHash.key_hash of a private-data key"""
+    return hashlib.sha256(key.encode()).digest()
+
+
 def tx_rwset(namespaces, mut=_same) -> bytes:
-    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes[, collections]).  The
-    fourth entry adds private-data collections, NsReadWriteSet.collection_hashed_rwset = CollectionHashedReadWriteSet{collection_name=1,
-    hashed_rwset=2}: an int n is one collection named "collection" with n hashed writes and one hashed read; a list holds one
-    (collection_name, n_hashed_writes, n_metadata_writes, n_hashed_reads) per collection, in order, and a collection_name of None
-    leaves the field out.  mut(part, bytes): see build_block."""
+    """rwset.TxReadWriteSet{data_model=1 (KV = 0), ns_rwset=2}; namespaces: list of (name, n_reads, n_writes[, collections[,
+    metadata_writes]]).  The fourth entry adds private-data collections, NsReadWriteSet.collection_hashed_rwset =
+    CollectionHashedReadWriteSet{collection_name=1, hashed_rwset=2}: an int n is one collection named "collection" with n hashed writes
+    and one hashed read; a list holds one (collection_name, n_hashed_writes, n_metadata_writes, n_hashed_reads) per collection, in
+    order, and a collection_name of None leaves the field out.  Keys by name: n_writes may be a list of public write keys, the fifth
+    entry a list of public metadata-write keys, and a collection's n_hashed_writes / n_metadata_writes lists of keys (written as their
+    key_hash).  mut(part, bytes): see build_block."""
     out = b""
     for ns in namespaces:
         name, nr, nw = ns[:3]
-        body = pb.f_bytes(1, name.encode()) + pb.f_bytes(2, mut("KVRWSet", kv_rwset(nr, nw, name.encode())))
+        if isinstance(nw, int) and len(ns) < 5:
+            kv = kv_rwset(nr, nw, name.encode())
+        else:
+            kv = named_kv_rwset(nr, nw, ns[4] if len(ns) > 4 else [], name.encode())
+        body = pb.f_bytes(1, name.encode()) + pb.f_bytes(2, mut("KVRWSet", kv))
         if len(ns) > 3 and isinstance(ns[3], int):
             coll = pb.f_bytes(1, b"collection") + pb.f_bytes(2, mut("HashedRWSet", hashed_rwset(ns[3], name.encode())))
             body += pb.f_bytes(3, mut("CollectionHashedReadWriteSet", coll))
@@ -89,8 +114,15 @@ def tx_rwset(namespaces, mut=_same) -> bytes:
             for cname, n_hw, n_mw, n_hr in ns[3]:
                 cn = cname.encode() if isinstance(cname, str) else cname
                 tag = name.encode() + b"/" + (cn or b"")
-                coll = (pb.f_bytes(1, cn) if cn is not None else b"") + \
-                    pb.f_bytes(2, mut("HashedRWSet", collection_hashed_rwset(n_hw, n_mw, n_hr, tag)))
+                if isinstance(n_hw, int) and isinstance(n_mw, int):
+                    hashed = collection_hashed_rwset(n_hw, n_mw, n_hr, tag)
+                else:
+                    hw = n_hw if not isinstance(n_hw, int) else []
+                    mw = n_mw if not isinstance(n_mw, int) else []
+                    hashed = (collection_hashed_rwset(n_hw if isinstance(n_hw, int) else 0, n_mw if isinstance(n_mw, int) else 0, n_hr, tag) +
+                              b"".join(pb.f_bytes(2, pb.f_bytes(1, key_hash(k)) + pb.f_bytes(3, key_hash("v"))) for k in hw) +
+                              b"".join(pb.f_bytes(3, pb.f_bytes(1, key_hash(k)) + _md_entry()) for k in mw))
+                coll = (pb.f_bytes(1, cn) if cn is not None else b"") + pb.f_bytes(2, mut("HashedRWSet", hashed))
                 body += pb.f_bytes(3, mut("CollectionHashedReadWriteSet", coll))
         out += pb.f_bytes(2, mut("NsReadWriteSet", body))
     return mut("TxReadWriteSet", out)
