@@ -527,7 +527,8 @@ class Context:
         return out
 
     def test_table_entries(self, key_slot, window, digit):
-        """Sampled window-table entries (key_slot < 0: generator table) -> (n, 16) little-endian u32 limbs, X then Y, Montgomery form."""
+        """Sampled table entries -> (n, 16) little-endian u32 limbs, X then Y, Montgomery form.  key_slot -1: the generator table;
+        >= 0: the window table in that raw key slot; <= -2: the small table of that keys_register_small handle (FabGpuError if stale)."""
         window = np.ascontiguousarray(window, dtype=np.uint32)
         digit = np.ascontiguousarray(digit, dtype=np.uint32)
         out = np.zeros((window.shape[0], 64), np.uint8)

@@ -694,12 +694,12 @@ full_tables_kernel(const aff* __restrict__ small, const int32_t* __restrict__ sl
     build_window_chunk(lo, lo + nsmall, half, x0, count, tab + (slot * windows + j) * (size_t)entries);
 }
 
-// Test hook: out[i] = entry (window[i], digit[i]) of a table (digit >= 1).
-__global__ void table_entries_kernel(const aff* __restrict__ tab, int wbits, const uint32_t* __restrict__ window, const uint32_t* __restrict__ digit,
+// Test hook: out[i] = entry (window[i], digit[i]) of a table of `stride` entries per window (digit >= 1).
+__global__ void table_entries_kernel(const aff* __restrict__ tab, uint32_t stride, const uint32_t* __restrict__ window, const uint32_t* __restrict__ digit,
                                      uint32_t n, aff* __restrict__ out)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = tab[(size_t)window[i] * ((1u << wbits) - 1u) + (digit[i] - 1u)];
+    if (i < n) out[i] = tab[(size_t)window[i] * stride + (digit[i] - 1u)];
 }
 
 // Unit-test hook: out[i] = op(a[i], b[i]) on the device primitives, op from the table of fieldops.cuh (tests/test_gpu_field.py).

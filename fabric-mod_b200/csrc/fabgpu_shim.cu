@@ -2327,20 +2327,35 @@ int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t
 int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* window, const uint32_t* digit, size_t n, uint8_t* out)
 {
     if (!ctx || !window || !digit || !out || key_slot >= ctx->key_slots) return FABGPU_E_ARG;
-    const int wbits = key_slot < 0 ? FAB_WG : FAB_WQ, windows = key_slot < 0 ? FAB_G_WINDOWS : FAB_Q_WINDOWS;
-    for (size_t i = 0; i < n; i++)
-        if (window[i] >= (uint32_t)windows || digit[i] == 0 || digit[i] >= (1u << wbits)) return FABGPU_E_ARG;
-    if (n == 0) return FABGPU_OK;
+    std::lock_guard<std::mutex> lk(ctx->mu);            // a small slot cannot be recycled, nor a new build enqueued, until the copy-back
     Device& dv = ctx->devs[0];
+    const aff* tab;
+    int windows;
+    uint32_t stride, dmax;                              // entries per window, largest digit
+    if (key_slot <= -2) {
+        const int32_t code = handle_to_slot(ctx, key_slot);
+        if (code == -1) return FABGPU_E_ARG;            // stale handle, or the slot is no longer in use
+        tab = dv.stab.get() + (size_t)(-2 - code) * FAB_S_POINTS;
+        windows = FAB_S_WINDOWS; stride = dmax = FAB_S_HALF;
+    } else if (key_slot == -1) {
+        tab = dv.gtab.get(); windows = FAB_G_WINDOWS; stride = dmax = FAB_G_ENTRIES;
+    } else {
+        tab = dv.qtab.get() + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES; windows = FAB_Q_WINDOWS; stride = dmax = FAB_Q_ENTRIES;
+    }
+    for (size_t i = 0; i < n; i++)
+        if (window[i] >= (uint32_t)windows || digit[i] == 0 || digit[i] > dmax) return FABGPU_E_ARG;
+    if (n == 0) return FABGPU_OK;
     CK(ctx, cudaSetDevice(dv.id));
-    const aff* tab = key_slot < 0 ? dv.gtab.get() : dv.qtab.get() + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES;
     DevArray<uint32_t> d_w, d_d; DevArray<aff> d_out;
     Grow grow{ctx};
     grow(d_w, 4 * n); grow(d_d, 4 * n); grow(d_out, sizeof(aff) * n);
     if (grow.rc) return grow.rc;
     CK(ctx, cudaMemcpy(d_w.get(), window, 4 * n, cudaMemcpyHostToDevice));
     CK(ctx, cudaMemcpy(d_d.get(), digit, 4 * n, cudaMemcpyHostToDevice));
-    table_entries_kernel<<<(unsigned)((n + 127) / 128), 128>>>(tab, wbits, d_w.get(), d_d.get(), (uint32_t)n, d_out.get());
+    // small tables are built on s_stream, which the legacy stream does not wait for: read only after the last build
+    if (dv.s_ev_set) CK(ctx, cudaStreamWaitEvent(0, dv.s_ev.get(), 0));
+    table_entries_kernel<<<(unsigned)((n + 127) / 128), 128>>>(tab, stride, d_w.get(), d_d.get(), (uint32_t)n, d_out.get());
+    ctx->launches++;
     CK(ctx, cudaGetLastError());
     CK(ctx, cudaMemcpy(out, d_out.get(), sizeof(aff) * n, cudaMemcpyDeviceToHost));
     return FABGPU_OK;

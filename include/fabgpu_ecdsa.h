@@ -326,9 +326,11 @@ int fabgpu_sha256_segments(fabgpu_ctx* ctx, const uint8_t* buf, size_t buf_len, 
 /* Device field primitives on arrays: out[i] = op(a[i], b[i]), 32 big-endian bytes each.  op is a code of the table in
  * fabric-mod_b200/csrc/fieldops.cuh (0 fe_mul ... 16); FABGPU_E_ARG for any other value. */
 int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t* b, size_t n, uint8_t* out);
-/* Sampled entries of a device window table: out[i] (64 bytes: X then Y, Montgomery form, little-endian 32-bit limbs) =
- * entry (window[i], digit[i]) = digit * 2^(w * window) * P, digit in [1, 2^w).  key_slot < 0: the generator's table
- * (w = g_window_bits of fabgpu_build_info); otherwise the table in that raw key slot (w = key_window_bits). */
+/* Sampled entries of a device point table: out[i] (64 bytes: X then Y, Montgomery form, little-endian 32-bit limbs) =
+ * entry (window[i], digit[i]) = digit * 2^(w * window) * P.  key_slot == -1: the generator's table (w = g_window_bits of
+ * fabgpu_build_info, digit in [1, 2^w)); key_slot >= 0: the window table in that raw key slot (w = key_window_bits, digit in
+ * [1, 2^w)); key_slot <= -2: a small handle from fabgpu_keys_register_small (w and the window count from fabgpu_small_table_info,
+ * digit in [1, 2^(w-1)]), FABGPU_E_ARG when the handle is stale.  Reads a small table only after its build has finished. */
 int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* window, const uint32_t* digit, size_t n, uint8_t* out);
 /* Phase times of the last fabgpu_bccsp_verify_batch call, microseconds: [0] key-table lookup/registration,
  * [1] staging copy into pinned memory (host gates + packing on the host-gated path), [2] H2D + kernels + D2H (enqueue to
