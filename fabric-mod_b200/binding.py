@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # FABGPU_LIB: development knob, points the binding at another build of the same library (kernel A/B runs)
 LIB_PATH = os.environ.get("FABGPU_LIB") or os.path.join(_HERE, "lib", "libfabgpu_ecdsa.so")
 SLOTS = 3
+CAP_V2_0, CAP_V1_3 = 0, 1      # fabgpu_channel_capability
 
 OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
 (ST_VALID, ST_INVALID, ST_ERR_NIL_KEY, ST_ERR_EMPTY_SIG, ST_ERR_EMPTY_DIGEST, ST_ERR_UNMARSHAL, ST_ERR_R_NOT_POSITIVE,
@@ -25,7 +26,7 @@ EXPORTS = [
     "fabgpu_msp_configure", "fabgpu_validate_block", "fabgpu_validate_envelopes", "fabgpu_block_buffer", "fabgpu_block_timing", "fabgpu_sha256_segments",
     "fabgpu_bccsp_verify_batch_async", "fabgpu_bccsp_verify_batch_wait", "fabgpu_bccsp_batch_buffers", "fabgpu_bccsp_verify_batch_inplace_async",
     "fabgpu_msp_identity_groups", "fabgpu_namespace_policies", "fabgpu_msp_principal_bits", "fabgpu_collection_policies",
-    "fabgpu_key_policies", "fabgpu_key_policies_update",
+    "fabgpu_key_policies", "fabgpu_key_policies_update", "fabgpu_channel_capability", "fabgpu_namespace_versions",
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
@@ -405,6 +406,19 @@ class Context:
         nb, no = _blob([n.encode() for n in names])
         roots = np.array([policies[n] for n in names] or [0], np.int32)
         self._ck(lib().fabgpu_namespace_policies(self._h, _p(nb), _p(no), _p(roots), ctypes.c_int(len(names))))
+        self._ns_names = names
+
+    def channel_capability(self, cap):
+        """cap: CAP_V2_0 (the default after msp_configure) for a channel with V2_0Validation, CAP_V1_3 for a V1_3 / V1_4_2 / V1_4_3
+        channel: the v1.4 validator with the builtin v13 VSCC (fabgpu_channel_capability)."""
+        self._ck(lib().fabgpu_channel_capability(self._h, ctypes.c_int(cap)))
+
+    def namespace_versions(self, versions):
+        """versions: {namespace: lscc ChaincodeData.Version} for the namespaces msp_configure's policies named; a namespace left out has
+        no version (its invocations are 254 in CAP_V1_3 mode), so None or an empty dict clears them (fabgpu_namespace_versions)."""
+        names = getattr(self, "_ns_names", [])
+        vb, vo = _blob([(versions or {}).get(n, "").encode() for n in names])
+        self._ck(lib().fabgpu_namespace_versions(self._h, _p(vb), _p(vo), ctypes.c_int(len(names))))
 
     def msp_principal_bits(self, bits):
         """bits: bool [n_ids, n_principals], bits[i, p] = identity i satisfies principal p (msp Identity.SatisfiesPrincipal), for the

@@ -27,8 +27,19 @@ enum : uint8_t {
     TXC_VALID = 0, TXC_BAD_PAYLOAD = 2, TXC_BAD_COMMON_HEADER = 3, TXC_BAD_CREATOR_SIGNATURE = 4, TXC_INVALID_ENDORSER_TRANSACTION = 5,
     TXC_UNSUPPORTED_TX_PAYLOAD = 7, TXC_BAD_PROPOSAL_TXID = 8, TXC_DUPLICATE_TXID = 9, TXC_ENDORSEMENT_POLICY_FAILURE = 10,
     TXC_TARGET_CHAIN_NOT_FOUND = 14, TXC_BAD_HEADER_EXTENSION = 19, TXC_BAD_RESPONSE_PAYLOAD = 21, TXC_BAD_RWSET = 22, TXC_ILLEGAL_WRITESET = 23,
-    TXC_INVALID_CHAINCODE = 25, TXC_NOT_VALIDATED = 254, TXC_INVALID_OTHER_REASON = 255
+    TXC_INVALID_CHAINCODE = 25, TXC_NOT_VALIDATED = 254, TXC_INVALID_OTHER_REASON = 255,
+    // fabric-protos-go peer/transaction.proto: set only by the v1.4 validator (channels without V2_0Validation)
+    TXC_EXPIRED_CHAINCODE = 17, TXC_CHAINCODE_VERSION_CONFLICT = 18
 };
+
+// Validator of the channel (core/committer/txvalidator/router.go:43): v20/validator.go with the plugin dispatcher (V2_0Validation), or
+// v14/validator.go with the builtin v13 VSCC and chaincode definitions from lscc (V1_3 / V1_4_2 / V1_4_3).
+#define BD_MODE_V20 0
+#define BD_MODE_V13 1
+// TxDev::v13_sys: what the invoked chaincode is to the v1.4 validator (v14/vscc_validator.go:407-417)
+#define BD_SYS_APP 0            // an application chaincode: the invoked and every written namespace are validated
+#define BD_SYS_QUERY 1          // qscc or cscc: only the invoked namespace is validated, without a version check
+#define BD_SYS_LSCC 2           // lscc: deploy / upgrade validation, left to the CPU validator (recorded as soon as the header names it)
 
 #define BD_MAX_SIGNERS 64       // distinct verified signers one policy evaluation handles (`used` is a 64-bit mask); more -> CPU validator
 #define BD_MAX_NS 4             // namespaces validated per transaction (the invoked chaincode + those it writes to); more -> CPU validator
@@ -305,6 +316,8 @@ struct TxDev {
     Seg results;                   // ChaincodeAction.results (the TxReadWriteSet), once dispatch_plan has read it
     uint32_t first_w, n_w;         // write records [first_w, first_w + n_w) of KlArrays::w (key policy table installed only)
     uint8_t kl_bad;                // a write inside the read/write set does not parse: the key-level checks cannot be made here
+    uint8_t v13_sys;               // v1.3 mode: BD_SYS_* of the invoked chaincode
+    Seg r_ver;                     // ChaincodeAction.chaincode_id.version, once dispatch_plan has read it
 };
 
 // One write of a transaction as baseEvaluator.Evaluate walks them (validator_keylevel.go:86-142): a public write, public metadata write,
@@ -348,6 +361,7 @@ struct JobArrays {
     uint8_t* gate_ok;              // [J_cap]
     uint32_t J_cap;                // capacity; creator jobs occupy [0, T), endorsement jobs [T, T + n_end)
     uint32_t T;
+    uint8_t mode = BD_MODE_V20;    // the channel's validator: the dispatcher's codes differ (dispatch_plan)
 };
 
 // What the walk leaves for one signature; identity lookup and DER gate are done per job by resolve_job (four times
@@ -376,17 +390,29 @@ BD_HD bool seg_equal(const uint8_t* base, Seg a, Seg b)
     return true;
 }
 
+// the four-letter system chaincode names of v14/vscc_validator.go:407-417
+BD_HD bool seg_is(const uint8_t* base, Seg a, const char* name)
+{
+    if (a.len != 4) return false;
+    for (uint32_t i = 0; i < 4; i++) if (base[a.off + i] != (uint8_t)name[i]) return false;
+    return true;
+}
+
 // The plugin dispatcher's structural checks (plugindispatcher/dispatcher.go:102-179), in its order.  chdr_ext: ChannelHeader.extension;
 // prp / prp_ext: ProposalResponsePayload bytes and its extension (peer.ChaincodeAction).  Fills tx.disp, tx.wr_ns, tx.n_ns, and
 // for the collection policies (validator_keylevel.go:86-142) tx.pub_ns and the written collections tx.coll / tx.coll_ns / tx.n_coll.
-BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool has_prp_ext, Seg prp_ext, TxDev& tx)
+// mode BD_MODE_V13: the same walk with the v1.4 validator's codes (v14/vscc_validator.go:69-270): 255 for the chaincode-name and
+// version checks, its system-chaincode rules, and tx.v13_sys.
+BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool has_prp_ext, Seg prp_ext, TxDev& tx, uint8_t mode = BD_MODE_V20)
 {
-    tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0;
+    tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0; tx.v13_sys = BD_SYS_APP;
     // hdrExt = ChaincodeHeaderExtension{chaincode_id = 2}, its ChaincodeID{path = 1, name = 2, version = 3} parsed with it
     Seg h_ccid; h_ccid.off = h_ccid.len = 0; bool has_h_ccid = false;
     if (!scan_msg(base, chdr_ext, BD_F(2), 0, [&](uint32_t, Seg b) { h_ccid = b; has_h_ccid = true; })) { tx.disp = TXC_BAD_HEADER_EXTENSION; return; }
     Seg h_name; h_name.off = h_name.len = 0;
     if (has_h_ccid && !scan_msg(base, h_ccid, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t f, Seg b) { if (f == 2) h_name = b; })) { tx.disp = TXC_BAD_HEADER_EXTENSION; return; }
+    // v1.3 mode: an lscc invocation, before any later check -- whatever stops it at 254 (lscc_mark), the reference may accept the upgrade
+    if (mode == BD_MODE_V13 && seg_is(base, h_name, "lscc")) tx.v13_sys = BD_SYS_LSCC;
     // respPayload = GetActionFromEnvelope: ChaincodeAction{results = 1, events = 2, response = 3, chaincode_id = 4}
     if (!has_prp || !has_prp_ext) { tx.disp = TXC_BAD_RESPONSE_PAYLOAD; return; }
     Seg results, events, r_ccid; results.off = results.len = events.off = events.len = r_ccid.off = r_ccid.len = 0;
@@ -400,6 +426,7 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
     if (has_r_ccid && !scan_msg(base, r_ccid, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t f, Seg b) { if (f == 2) r_name = b; else if (f == 3) r_ver = b; })) {
         tx.disp = TXC_BAD_RESPONSE_PAYLOAD; return;
     }
+    tx.r_ver = r_ver;
     // txRWSet.FromProtoBytes(results): TxReadWriteSet{data_model = 1, ns_rwset = 2}, every namespace with its KVRWSet and hashed collections
     Seg seen[BD_MAX_NS_SEEN]; bool wrote[BD_MAX_NS_SEEN], pub[BD_MAX_NS_SEEN]; uint32_t n_seen = 0; bool too_many = false, rw_ok = true;
     const bool top_ok = scan_msg(base, results, BD_F(2), BD_F(1), [&](uint32_t, Seg nsb) {
@@ -429,7 +456,7 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
     });
     if (!top_ok || !rw_ok) { tx.disp = TXC_BAD_RWSET; return; }
     if (!has_h_ccid || !has_r_ccid) { tx.disp = TXC_INVALID_OTHER_REASON; return; }
-    if (h_name.len == 0 || !seg_equal(base, h_name, r_name) || r_ver.len == 0) { tx.disp = TXC_INVALID_CHAINCODE; return; }
+    if (h_name.len == 0 || !seg_equal(base, h_name, r_name) || r_ver.len == 0) { tx.disp = mode == BD_MODE_V13 ? TXC_INVALID_OTHER_REASON : TXC_INVALID_CHAINCODE; return; }
     if (has_events) {                                                  // ChaincodeEvent{chaincode_id = 1 (string), tx_id = 2, event_name = 3, payload = 4}
         Seg ev_cc; ev_cc.off = ev_cc.len = 0;
         if (!scan_msg(base, events, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t f, Seg b) { if (f == 1) ev_cc = b; }) || !seg_equal(base, ev_cc, h_name)) {
@@ -440,6 +467,20 @@ BD_HD void dispatch_plan(const uint8_t* base, Seg chdr_ext, bool has_prp, bool h
     tx.wr_ns[0] = h_name; tx.n_ns = 1;
     for (uint32_t i = 0; i < n_seen; i++) {
         for (uint32_t j = 0; j < i; j++) if (seg_equal(base, seen[i], seen[j])) { tx.disp = TXC_ILLEGAL_WRITESET; return; }
+    }
+    if (mode == BD_MODE_V13) {                                        // v14/vscc_validator.go:151-160,176-190,230-238
+        bool w_lscc = false, w_sys = false;
+        for (uint32_t i = 0; i < n_seen; i++) {
+            if (!wrote[i]) continue;
+            w_lscc = w_lscc || seg_is(base, seen[i], "lscc");
+            w_sys = w_sys || seg_is(base, seen[i], "vscc") || seg_is(base, seen[i], "escc") || seg_is(base, seen[i], "cscc");
+        }
+        if (seg_is(base, h_name, "vscc") || seg_is(base, h_name, "escc")) { tx.disp = TXC_ILLEGAL_WRITESET; return; }
+        if (tx.v13_sys == BD_SYS_LSCC) { tx.disp = TXC_NOT_VALIDATED; return; }
+        if (seg_is(base, h_name, "qscc") || seg_is(base, h_name, "cscc")) {
+            tx.v13_sys = BD_SYS_QUERY; tx.wr_ns[0] = h_name; tx.n_ns = 1; tx.n_coll = 0; return;
+        }
+        if (w_lscc || w_sys) { tx.disp = TXC_ILLEGAL_WRITESET; return; }
     }
     uint8_t wr_of[BD_MAX_NS_SEEN];                                     // seen[] index -> wr_ns index, for the namespaces that wrote
     for (uint32_t i = 0; i < n_seen; i++) {
@@ -604,7 +645,7 @@ BD_HD void walk_tx_core(const uint8_t* base, Seg env, uint32_t t, const uint8_t*
     tx.early = TXC_NOT_VALIDATED; tx.htype = 0; tx.endorser_parse_ok = 0; tx.channel_ok = 0; tx.endorsements_parse_ok = 1; tx.overflow = 0;
     tx.disp = TXC_VALID; tx.n_ns = 0; tx.n_coll = 0; tx.pub_ns = 0; tx.creator_identity = -1; tx.creator_has_job = 0; tx.first_end_job = 0; tx.n_end_jobs = 0;
     tx.txid_ascii.off = tx.txid_ascii.len = 0; tx.phash_claimed.off = tx.phash_claimed.len = 0;
-    tx.results.off = tx.results.len = 0; tx.first_w = tx.n_w = 0; tx.kl_bad = 0;
+    tx.results.off = tx.results.len = 0; tx.first_w = tx.n_w = 0; tx.kl_bad = 0; tx.v13_sys = BD_SYS_APP; tx.r_ver.off = tx.r_ver.len = 0;
     {
         ShaJobD z; for (int k = 0; k < 3; k++) { z.off[k] = 0; z.len[k] = 0; }
         ja.sha[t] = z; ja.sha[ja.J_cap + 2 * t] = z; ja.sha[ja.J_cap + 2 * t + 1] = z;
@@ -668,7 +709,7 @@ BD_HD void walk_tx_core(const uint8_t* base, Seg env, uint32_t t, const uint8_t*
       b.off[0] = chdr_b.off; b.len[0] = chdr_b.len; b.off[1] = ta.s[0].off; b.len[1] = ta.s[0].len; b.off[2] = cap.s[0].off; b.len[2] = cap.s[0].len; }
     tx.phash_claimed = pr.s[0];
     tx.endorser_parse_ok = 1;
-    dispatch_plan(base, ch.s[2], has_prp, pr.present[1], pr.s[1], tx);
+    dispatch_plan(base, ch.s[2], has_prp, pr.present[1], pr.s[1], tx, ja.mode);
     // key policy table installed: the writes the key-level checks walk (a transaction the dispatcher stops is walk_tx's)
     if (ja.kl.w && tx.disp == TXC_VALID) kl_emit(base, tx.results, t, tx, ja.kl, false);
     // endorsements: one pass to count those that carry a signature, one to emit their jobs (contiguous, in endorsement order)
@@ -774,6 +815,9 @@ struct PolicyDev {
     uint32_t coll_size = 0;
     // fabgpu_key_policies: key-level validation parameters, kp_size slots (a power of two) keyed by kl_key_hash; kp_size = 0: no table
     const KpSlot* kp_slots = nullptr; const uint8_t* kp_blob = nullptr; uint32_t kp_size = 0;
+    // fabgpu_channel_capability: BD_MODE_V13 selects the v1.4 validator (decide_tx); fabgpu_namespace_versions: the lscc version of
+    // namespace table entry i at ver_blob + ver_off[i] .. ver_off[i + 1] (empty: none), null = no versions
+    uint8_t mode = BD_MODE_V20; const uint8_t* ver_blob = nullptr; const uint32_t* ver_off = nullptr;
 };
 
 // root of the validation parameter of (ns, coll, key) (all in the block), -1 when the table holds none
@@ -851,8 +895,10 @@ BD_HD void kl_resolve_step(uint32_t t, const TxDev* txs, KlArrays& kl, uint8_t* 
     }
     if (mark & 2) {
         const bool gone = x.n_w && kl.w[x.first_w].gone;
-        const uint32_t st = KL_SUM_ANY | (f == TXC_VALID && !gone ? KL_SUM_NIL
-                                          : f == TXC_ENDORSEMENT_POLICY_FAILURE && x.n_ns == 1 && !gone ? 0u : KL_SUM_UNDET);
+        // (a v1.3-mode qscc / cscc invocation validates only its own namespace, whatever it metadata-writes: undetermined)
+        const bool decided = !gone && x.v13_sys == BD_SYS_APP;
+        const uint32_t st = KL_SUM_ANY | (f == TXC_VALID && decided ? KL_SUM_NIL
+                                          : f == TXC_ENDORSEMENT_POLICY_FAILURE && x.n_ns == 1 && decided ? 0u : KL_SUM_UNDET);
         for (uint32_t q = 0; q < x.n_w; q++) {
             const WriteRec& w = kl.w[x.first_w + q];
             if (w.md && w.slot != 0xffffffffu) kl.md_sum[w.slot] |= st;
@@ -950,18 +996,137 @@ BD_HD bool eval_policy(const PolicyDev& pol, int idx, const int32_t* signer, int
     return false;
 }
 
-// root node of namespace `ns`'s policy, -1 when the table has no chaincode definition for it
-BD_HD int32_t policy_root(const PolicyDev& pol, const uint8_t* base, Seg ns)
+// entry of namespace `ns` in the namespace table, -1 when it has none
+BD_HD int32_t policy_index(const PolicyDev& pol, const uint8_t* base, Seg ns)
 {
-    if (pol.n_ns == 0) return pol.n_nodes > 0 ? 0 : -1;
     for (int32_t i = 0; i < pol.n_ns; i++) {
         const uint32_t o = pol.ns_off[i], l = pol.ns_off[i + 1] - o;
         if (l != ns.len) continue;
         bool eq = true;
         for (uint32_t k = 0; k < l && eq; k++) eq = pol.ns_blob[o + k] == base[ns.off + k];
-        if (eq) return pol.ns_root[i];
+        if (eq) return i;
     }
     return -1;
+}
+
+// root node of namespace `ns`'s policy, -1 when the table has no chaincode definition for it
+BD_HD int32_t policy_root(const PolicyDev& pol, const uint8_t* base, Seg ns)
+{
+    if (pol.n_ns == 0) return pol.n_nodes > 0 ? 0 : -1;
+    const int32_t i = policy_index(pol, base, ns);
+    return i < 0 ? -1 : pol.ns_root[i];
+}
+
+// SignatureSetToValidIdentities (policy.go:365-402): in order; de-duplicated by Mspid + Id against the identities that already
+// VERIFIED; a failed signature drops that entry only.  One set per transaction, shared by every namespace's evaluation.
+// With principal bits a signer is its identity index: the caller's SatisfiesPrincipal answers already include Validate() where
+// the reference checks it (an admin-listed identity satisfies ADMIN without it, mspimpl.go:506-513).  Without, it is its MSP-id
+// code, -1 when Validate() failed (ROLE MEMBER, mspimpl.go:501-505).  false: not decided here (an endorser the table does not hold,
+// or more signers than BD_MAX_SIGNERS).
+template <typename SigOk>
+BD_HD bool signer_set(const TxDev& tx, const MspDev& msp, const PolicyDev& pol, SigOk sig_ok, const int32_t* job_identity, int32_t* signer,
+                      int& n_signers)
+{
+    n_signers = 0;
+    for (uint32_t i = 0; i < tx.n_end_jobs; i++) {
+        const uint32_t j = tx.first_end_job + i;
+        const int32_t idn = job_identity[j];
+        if (idn < 0) return false;
+        const int32_t grp = msp.group ? msp.group[idn] : idn;
+        bool dup = false;
+        for (uint32_t i2 = 0; i2 < i && !dup; i2++) {
+            const uint32_t j2 = tx.first_end_job + i2;
+            const int32_t id2 = job_identity[j2];
+            dup = (msp.group ? msp.group[id2] : id2) == grp && sig_ok(j2);
+        }
+        if (dup) continue;
+        if (!sig_ok(j)) continue;
+        if (n_signers >= BD_MAX_SIGNERS) return false;
+        signer[n_signers++] = pol.principal_bits ? idn : msp.valid[idn] ? msp.msp_code[idn] : -1;
+    }
+    return true;
+}
+
+// An earlier metadata write of a key t writes: marks t for the resolve stage (kl_resolve_step)
+BD_HD void kl_mark_deps(const uint8_t* base, const TxDev& tx, uint32_t t, KlArrays* kl)
+{
+    bool dep = false;
+    for (uint32_t q = 0; q < tx.n_w; q++) {
+        WriteRec& w = kl->w[tx.first_w + q];
+        if (!w.md) w.slot = kl_md_find(*kl, base, w);
+        if (w.slot == 0xffffffffu) continue;
+        const unsigned long long m = kl->md_min[w.slot];
+        if ((uint32_t)(m >> 32) >= t) continue;                       // every metadata writer of this hash comes later
+        dep = true;
+        if (!kl_same_key(base, kl->w[(uint32_t)m], w)) w.alias = 1;
+    }
+    if (dep) kl->conflicted[t] |= 1;
+}
+
+BD_HD uint64_t txid_hash(const uint8_t* base, const TxDev& tx)
+{
+    uint64_t hsh = 1469598103934665603ull;
+    for (uint32_t k = 0; k < tx.txid_ascii.len; k++) hsh = (hsh ^ base[tx.txid_ascii.off + k]) * 1099511628211ull;
+    return hsh;
+}
+
+// The v1.4 validator's VSCC stage (v14/vscc_validator.go:117-229,230-270 with builtin/v13): the validated namespaces in order -- the
+// invoked chaincode, then the others in read/write-set order -- and the first that fails decides.  Per namespace: its table entry
+// (none: 254), for the invoked application chaincode the lscc version (:195-208; none installed: 254, another: EXPIRED_CHAINCODE),
+// then its own writes only (baseEvaluator.Evaluate, statebased/v13.go): the key's validation parameter if it has one, otherwise the
+// chaincode policy -- no collection policies.  A namespace without writes is checked against its chaincode policy.
+template <typename SigOk>
+BD_HD uint8_t decide_v13(const uint8_t* base, const TxDev& tx, uint32_t t, const MspDev& msp, const PolicyDev& pol, SigOk sig_ok,
+                         const int32_t* job_identity, uint64_t* txid_hash_out, KlArrays* kl)
+{
+    const bool keylevel = kl && pol.kp_size;
+    if (keylevel) {
+        if (kl->counter[0] > kl->W_cap || kl->counter[1] || tx.kl_bad) return TXC_NOT_VALIDATED;
+        for (uint32_t q = 0; q < tx.n_w; q++)                         // a qscc / cscc invocation writing elsewhere: not decided here
+            if (tx.v13_sys != BD_SYS_APP && !seg_equal(base, kl->w[tx.first_w + q].ns, tx.wr_ns[0])) return TXC_NOT_VALIDATED;
+    }
+    int32_t signer[BD_MAX_SIGNERS]; int n_signers = -1;              // built at the first policy evaluation
+    for (int i = 0; i < tx.n_ns; i++) {
+        const int32_t cc_root = policy_root(pol, base, tx.wr_ns[i]);
+        if (cc_root < 0) return TXC_NOT_VALIDATED;
+        if (i == 0 && tx.v13_sys == BD_SYS_APP) {
+            const int32_t k = pol.ver_off ? policy_index(pol, base, tx.wr_ns[0]) : -1;
+            const uint32_t vo = k < 0 ? 0 : pol.ver_off[k], vl = k < 0 ? 0 : pol.ver_off[k + 1] - vo;
+            if (vl == 0) return TXC_NOT_VALIDATED;                    // no lscc version on the device
+            if (vl != tx.r_ver.len || !bytes_equal(pol.ver_blob + vo, base + tx.r_ver.off, vl)) return TXC_EXPIRED_CHAINCODE;
+        }
+        int32_t need[BD_MAX_NEED]; int n_need = 0; bool too_many = false;
+        auto add = [&](int32_t r) {
+            for (int k = 0; k < n_need; k++) if (need[k] == r) return;
+            if (n_need == BD_MAX_NEED) too_many = true; else need[n_need++] = r;
+        };
+        bool wrote = false;
+        for (uint32_t q = 0; keylevel && q < tx.n_w; q++) {
+            const WriteRec& w = kl->w[tx.first_w + q];
+            if (w.ns_idx != i) continue;
+            const int32_t cr = w.coll.len && pol.coll_size ? coll_policy_root(pol, base, w.ns, w.coll) : -1;
+            if (w.coll.len && pol.coll_size && cr < 0) return TXC_NOT_VALIDATED;   // as in v2.0 mode: the collection may be undefined
+            const int32_t r = kp_find(pol, base, w.ns, w.coll, w.key);
+            if (r == KP_UNDECIDABLE) return TXC_NOT_VALIDATED;
+            add(r < 0 ? cc_root : r);
+            wrote = true;
+        }
+        if (!wrote) add(cc_root);
+        if (too_many) return TXC_NOT_VALIDATED;
+        if (n_signers < 0 && !signer_set(tx, msp, pol, sig_ok, job_identity, signer, n_signers)) return TXC_NOT_VALIDATED;
+        bool pass = true;
+        for (int k = 0; k < n_need && pass; k++) {
+            uint64_t used = 0;
+            pass = eval_policy(pol, need[k], signer, n_signers, used, 0);
+        }
+        if (!pass) {
+            if (keylevel) kl_mark_deps(base, tx, t, kl);
+            return TXC_ENDORSEMENT_POLICY_FAILURE;
+        }
+    }
+    if (keylevel) kl_mark_deps(base, tx, t, kl);
+    *txid_hash_out = txid_hash(base, tx);
+    return TXC_VALID;
 }
 
 // ---- per-transaction decision ---------------------------------------------------------------------------------------------
@@ -997,6 +1162,7 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
     if (tx.disp != TXC_VALID) return tx.disp;                         // the plugin dispatcher's own checks
     if (!tx.endorsements_parse_ok) return TXC_INVALID_OTHER_REASON;
     if (tx.overflow) return TXC_NOT_VALIDATED;                        // job arrays were full: CPU validator
+    if (pol.mode == BD_MODE_V13) return decide_v13(base, tx, t, msp, pol, sig_ok, job_identity, txid_hash_out, kl);
     // The policies to satisfy, each root once (evaluation has no state across policies, so the reference's nsEPChecked memo,
     // v20.go:105-147, changes no outcome).  Without a collection table: every validated namespace's chaincode policy.  With one, per
     // namespace as baseEvaluator.Evaluate (validator_keylevel.go:86-142) walks its writes: the collection's policy for each named
@@ -1046,51 +1212,25 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
         for (int i = 0; i < tx.n_ns; i++)
             if (((tx.pub_ns | ~has_coll) >> i) & 1u) add(roots[i]);
     }
-    // SignatureSetToValidIdentities (policy.go:365-402): in order; de-duplicated by Mspid + Id against the identities that already
-    // VERIFIED; a failed signature drops that entry only.  One set per transaction, shared by every namespace's evaluation.
-    // With principal bits a signer is its identity index: the caller's SatisfiesPrincipal answers already include Validate() where
-    // the reference checks it (an admin-listed identity satisfies ADMIN without it, mspimpl.go:506-513).  Without, it is its MSP-id
-    // code, -1 when Validate() failed (ROLE MEMBER, mspimpl.go:501-505).
     int32_t signer[BD_MAX_SIGNERS]; int n_signers = 0;
-    for (uint32_t i = 0; i < tx.n_end_jobs; i++) {
-        const uint32_t j = tx.first_end_job + i;
-        const int32_t idn = job_identity[j];
-        if (idn < 0) return TXC_NOT_VALIDATED;
-        const int32_t grp = msp.group ? msp.group[idn] : idn;
-        bool dup = false;
-        for (uint32_t i2 = 0; i2 < i && !dup; i2++) {
-            const uint32_t j2 = tx.first_end_job + i2;
-            const int32_t id2 = job_identity[j2];
-            dup = (msp.group ? msp.group[id2] : id2) == grp && sig_ok(j2);
-        }
-        if (dup) continue;
-        if (!sig_ok(j)) continue;
-        if (n_signers >= BD_MAX_SIGNERS) return TXC_NOT_VALIDATED;
-        signer[n_signers++] = pol.principal_bits ? idn : msp.valid[idn] ? msp.msp_code[idn] : -1;
-    }
+    if (!signer_set(tx, msp, pol, sig_ok, job_identity, signer, n_signers)) return TXC_NOT_VALIDATED;
     bool pass = true;
     for (int k = 0; k < n_need && pass; k++) {
         uint64_t used = 0;
         pass = eval_policy(pol, need[k], signer, n_signers, used, 0);
     }
-    if (keylevel) {                                                   // an earlier metadata write of a key t writes: resolved later
-        bool dep = false;
-        for (uint32_t q = 0; q < tx.n_w; q++) {
-            WriteRec& w = kl->w[tx.first_w + q];
-            if (!w.md) w.slot = kl_md_find(*kl, base, w);
-            if (w.slot == 0xffffffffu) continue;
-            const unsigned long long m = kl->md_min[w.slot];
-            if ((uint32_t)(m >> 32) >= t) continue;                   // every metadata writer of this hash comes later
-            dep = true;
-            if (!kl_same_key(base, kl->w[(uint32_t)m], w)) w.alias = 1;
-        }
-        if (dep) kl->conflicted[t] |= 1;
-    }
+    if (keylevel) kl_mark_deps(base, tx, t, kl);                      // an earlier metadata write of a key t writes: resolved later
     if (!pass) return TXC_ENDORSEMENT_POLICY_FAILURE;
-    uint64_t hsh = 1469598103934665603ull;
-    for (uint32_t k = 0; k < tx.txid_ascii.len; k++) hsh = (hsh ^ base[tx.txid_ascii.off + k]) * 1099511628211ull;
-    *txid_hash_out = hsh;
+    *txid_hash_out = txid_hash(base, tx);
     return TXC_VALID;
+}
+
+// v1.3 mode, after decide_tx: a transaction invoking lscc that the device flags 254 -- at its lscc check, or earlier (a creator outside the
+// table, more namespaces than the walk records, ...) -- may be an upgrade the reference accepts, which then invalidates the block's later
+// invocations of that chaincode (v14/validator.go:210-220,487-530).  Sets *lscc_seen: every VALID flag of the block becomes 254.
+BD_HD void lscc_mark(const TxDev& tx, uint8_t flag, uint32_t* lscc_seen)
+{
+    if (tx.v13_sys == BD_SYS_LSCC && flag == TXC_NOT_VALIDATED) *lscc_seen = 1;
 }
 
 } }  // namespace fabgpu::bdev

@@ -30,19 +30,23 @@ block_resolve_kernel(const uint8_t* __restrict__ block, const RawJob* __restrict
     resolve_job(block, j0 + i, raw, msp, ja, txs);
 }
 
-// Replays the reference's decision order for every transaction on the verification bitmask and the digests.
+// Replays the reference's decision order for every transaction on the verification bitmask and the digests.  lscc_seen (v1.3 mode,
+// else null): set when an lscc invocation of the block is flagged 254 (lscc_mark).
 __global__ void __launch_bounds__(128)
 block_decide_kernel(const uint8_t* __restrict__ block, const TxDev* __restrict__ txs, uint32_t T, MspDev msp, PolicyDev pol,
                     const uint32_t* __restrict__ mask, const uint8_t* __restrict__ gate_ok, const int32_t* __restrict__ job_identity,
                     const uint8_t* __restrict__ digests, uint32_t J_cap,
-                    uint8_t* __restrict__ flags, uint64_t* __restrict__ txid_hash, Seg* __restrict__ txid_seg, KlArrays kl)
+                    uint8_t* __restrict__ flags, uint64_t* __restrict__ txid_hash, Seg* __restrict__ txid_seg, KlArrays kl,
+                    uint32_t* __restrict__ lscc_seen)
 {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     uint64_t h = 0;
     if (kl.w) kl_mark(block, t, txs[t], kl);
-    flags[t] = decide_tx(block, txs[t], t, msp, pol, [&](uint32_t j) { return gate_ok[j] && ((mask[j >> 5] >> (j & 31)) & 1u); }, job_identity, digests, J_cap, &h,
-                         kl.w ? &kl : nullptr);
+    const uint8_t f = decide_tx(block, txs[t], t, msp, pol, [&](uint32_t j) { return gate_ok[j] && ((mask[j >> 5] >> (j & 31)) & 1u); }, job_identity, digests,
+                                J_cap, &h, kl.w ? &kl : nullptr);
+    flags[t] = f;
+    if (lscc_seen) lscc_mark(txs[t], f, lscc_seen);
     txid_hash[t] = h;
     txid_seg[t] = txs[t].txid_ascii;
 }

@@ -22,6 +22,7 @@
 #include "../../include/fabgpu_ecdsa.h"
 #include "bccsp_host.hpp"
 #include "blockval.hpp"
+#include "capability.hpp"
 #include "cuda_owned.hpp"
 #include "sha256.cuh"
 #include "blockdev_kernels.cuh"
@@ -210,6 +211,9 @@ struct fabgpu_ctx {
         DevArray<uint32_t> id_off; DevArray<int32_t> key_slot, msp_code, ht_idx, nodes, principal_code;
         DevArray<int32_t> group;                                      // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
         DevArray<uint8_t> ns_blob; DevArray<uint32_t> ns_off; DevArray<int32_t> ns_root; int32_t n_ns = 0;    // fabgpu_namespace_policies
+        std::vector<int32_t> ns_root_host;                            // the same roots, for the v1.3 mode's ImplicitMeta check
+        uint8_t mode = BD_MODE_V20;                       // fabgpu_channel_capability
+        DevArray<uint8_t> ver_blob; DevArray<uint32_t> ver_off;       // fabgpu_namespace_versions, null = none
         DevArray<uint32_t> pbits; int32_t pbits_words = 0;            // fabgpu_msp_principal_bits, null = MSP-id member matching
         DevArray<uint8_t> cp_ns_blob, cp_name_blob; DevArray<uint32_t> cp_ns_off, cp_name_off;   // fabgpu_collection_policies, cp_size = 0: none
         DevArray<int32_t> cp_root, cp_idx; DevArray<uint64_t> cp_hash; uint32_t cp_size = 0;
@@ -248,7 +252,7 @@ struct fabgpu_ctx {
         // key policy table installed: write records, the metadata-write set, conflicted transactions (grown together, per block)
         DevArray<bdev::WriteRec> d_w; DevArray<uint64_t> d_md_hash; DevArray<unsigned long long> d_md_min; DevArray<uint32_t> d_md_sum, d_clist; DevArray<uint8_t> d_conf;
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
-        bool busy = false, on_device = false, use_ev = false, kl_on = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
+        bool busy = false, on_device = false, use_ev = false, kl_on = false, v13 = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
@@ -1840,8 +1844,10 @@ int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uin
     auto& dm = ctx->dm;
     for (int i = 0; i < n_ns; i++)
         if (ns_root[i] < 0 || ns_root[i] >= dm.n_nodes || ns_off[i] > ns_off[i + 1]) { ctx->last_error = "namespace policy root out of range"; return FABGPU_E_ARG; }
+    if (const char* err = capability::check_namespace_table(dm.mode == BD_MODE_V13, ctx->policy, ns_root, n_ns)) { ctx->last_error = err; return FABGPU_E_ARG; }
     int rc = drain_block_streams(ctx); if (rc) return rc;
-    dm.ns_blob = {}; dm.ns_off = {}; dm.ns_root = {}; dm.n_ns = 0;
+    dm.ns_blob = {}; dm.ns_off = {}; dm.ns_root = {}; dm.n_ns = 0; dm.ns_root_host.clear();
+    dm.ver_blob = {}; dm.ver_off = {};                                // versions name the entries of the table being replaced
     if (n_ns == 0) return FABGPU_OK;
     const size_t bl = ns_off[n_ns];
     if ((rc = dm.ns_blob.reserve(ctx, bl + 8))) return rc;
@@ -1850,7 +1856,36 @@ int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uin
     CK(ctx, cudaMemcpy(dm.ns_off.get(), ns_off, 4 * (size_t)(n_ns + 1), cudaMemcpyHostToDevice));
     if ((rc = dm.ns_root.reserve(ctx, 4 * (size_t)n_ns))) return rc;
     CK(ctx, cudaMemcpy(dm.ns_root.get(), ns_root, 4 * (size_t)n_ns, cudaMemcpyHostToDevice));
-    dm.n_ns = n_ns;
+    dm.n_ns = n_ns; dm.ns_root_host.assign(ns_root, ns_root + n_ns);
+    return FABGPU_OK;
+}
+
+int fabgpu_channel_capability(fabgpu_ctx* ctx, int cap)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm;
+    if (const char* err = capability::check_capability(cap, ctx->policy, dm.ns_root_host.data(), dm.n_ns)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    int rc = drain_block_streams(ctx); if (rc) return rc;
+    dm.mode = cap == FABGPU_CAP_V1_3 ? BD_MODE_V13 : BD_MODE_V20;
+    return FABGPU_OK;
+}
+
+int fabgpu_namespace_versions(fabgpu_ctx* ctx, const uint8_t* ver_blob, const uint32_t* ver_off, int n_ns)
+{
+    if (!ctx || n_ns < 0 || (n_ns && (!ver_blob || !ver_off))) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm;
+    if (const char* err = capability::check_versions(ver_off, n_ns, dm.n_ns)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    int rc = drain_block_streams(ctx); if (rc) return rc;
+    dm.ver_blob = {}; dm.ver_off = {};
+    if (n_ns == 0) return FABGPU_OK;
+    if ((rc = dm.ver_blob.reserve(ctx, ver_off[n_ns] + 8))) return rc;   // slack: bytes_equal reads whole aligned words
+    if (ver_off[n_ns]) CK(ctx, cudaMemcpy(dm.ver_blob.get(), ver_blob, ver_off[n_ns], cudaMemcpyHostToDevice));
+    if ((rc = dm.ver_off.reserve(ctx, 4 * (size_t)(n_ns + 1)))) { dm.ver_blob = {}; return rc; }
+    if (cudaMemcpy(dm.ver_off.get(), ver_off, 4 * (size_t)(n_ns + 1), cudaMemcpyHostToDevice) != cudaSuccess) {
+        dm.ver_blob = {}; dm.ver_off = {}; ctx->last_error = "namespace version upload failed"; return FABGPU_E_CUDA;
+    }
     return FABGPU_OK;
 }
 
@@ -2087,6 +2122,8 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     pol.coll_ns_blob = dm.cp_ns_blob.get(); pol.coll_ns_off = dm.cp_ns_off.get(); pol.coll_name_blob = dm.cp_name_blob.get(); pol.coll_name_off = dm.cp_name_off.get();
     pol.coll_root = dm.cp_root.get(); pol.coll_hash = dm.cp_hash.get(); pol.coll_idx = dm.cp_idx.get(); pol.coll_size = dm.cp_size;
     pol.n_nodes = dm.n_nodes + dm.kp_n_nodes; pol.kp_slots = dm.kp_slots.get(); pol.kp_blob = dm.kp_blob.get(); pol.kp_size = dm.kp_size;
+    pol.mode = dm.mode; pol.ver_blob = dm.ver_blob.get(); pol.ver_off = dm.ver_off.get();
+    db.v13 = dm.mode == BD_MODE_V13;
     bdev::KlArrays kl;                                        // key policy table installed: write records and the metadata-write set
     db.kl_on = dm.kp_size != 0;
     if (db.kl_on) {
@@ -2105,7 +2142,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     }
     const bool need_q = (dm.classes & CLASS_GENERIC) != 0;   // only the generic arithmetic reads the key itself
     bdev::JobArrays ja; ja.sha = db.d_sha.get(); ja.r = db.d_r.get(); ja.s = db.d_s.get(); ja.key_slot = db.d_ks.get(); ja.identity = db.d_ident.get(); ja.qx = need_q ? db.d_qx.get() : nullptr;
-    ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T; ja.kl = kl;
+    ja.qy = need_q ? db.d_qy.get() : nullptr; ja.gate_ok = db.d_gate.get(); ja.J_cap = (uint32_t)J_cap; ja.T = (uint32_t)T; ja.kl = kl; ja.mode = dm.mode;
     const uint32_t cnt = (uint32_t)T, E_cap = (uint32_t)(J_cap - T);
     // One copy, then the walk.  (Copying in chunks with a walk per chunk was measured slower, the more chunks the slower: hashing a
     // 4.6 KB payload is a long chain of dependent rounds per thread however few
@@ -2131,13 +2168,14 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     if (rc) return rc;
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4].get(), st));
     bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), db.d_txs.get(), cnt, m, pol, db.d_mask.get(), db.d_gate.get(), db.d_ident.get(), db.d_dig.get(), (uint32_t)J_cap, db.d_flags.get(),
-                                                               db.d_hash.get(), db.d_seg.get(), kl);
+                                                               db.d_hash.get(), db.d_seg.get(), kl, db.v13 ? db.d_counter.get() + 1 : nullptr);
     ctx->launches++;
     if (db.kl_on) {
         bdev::block_kl_resolve_kernel<<<1, 256, 0, st>>>(db.d_txs.get(), cnt, kl, db.d_flags.get());
         ctx->launches++;
-        CK(ctx, cudaMemcpyAsync(db.h_counter.get(), db.d_counter.get(), 16, cudaMemcpyDeviceToHost, st));   // write records used
     }
+    // [1]: an lscc invocation was flagged 254 (v1.3 mode); [2]: write records used (key policy table)
+    if (db.kl_on || db.v13) CK(ctx, cudaMemcpyAsync(db.h_counter.get(), db.d_counter.get(), 16, cudaMemcpyDeviceToHost, st));
     CK(ctx, cudaGetLastError());
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[5].get(), st));
     CK(ctx, cudaMemcpyAsync(db.h_flags.get(), db.d_flags.get(), T, cudaMemcpyDeviceToHost, st));
@@ -2189,6 +2227,11 @@ static int block_finish(fabgpu_ctx* ctx, int slot, uint8_t* flags)
             else { keys[pos] = h; idx[pos] = (uint32_t)t; }
         }
     }
+    // v1.3 mode, a block with an lscc invocation flagged 254 (lscc_mark): the reference invalidates the still-VALID invocations of a chaincode an upgrade of the
+    // block names (CHAINCODE_VERSION_CONFLICT, v14/validator.go:210-220,487-530); the device does not decide the upgrade, so every
+    // VALID transaction goes to the CPU validator.  After the duplicate pass and the key-level resolve stage, and fed into neither.
+    if (db.v13 && db.h_counter.get()[1])
+        for (size_t t = 0; t < T; t++) if (flags[t] == blockval::TX_VALID) flags[t] = bdev::TXC_NOT_VALIDATED;
     auto t4 = now();
     ctx->block_timing[0] = us(db.t0, db.t1); ctx->block_timing[1] = 0; ctx->block_timing[2] = us(db.t1, t3); ctx->block_timing[3] = us(t3, t4);
     ctx->block_timing[4] = us(db.t0, t4);

@@ -296,6 +296,38 @@ int fabgpu_key_policies(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, cons
 int fabgpu_key_policies_update(fabgpu_ctx* ctx, const int32_t* nodes, int n_nodes, const uint8_t* ns_blob, const uint32_t* ns_off,
                                const uint8_t* coll_blob, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off,
                                const int32_t* root, int n);
+/* The channel's validator (core/committer/txvalidator/router.go:43).  Also refinements: each drains the block slots, and
+ * fabgpu_msp_configure resets both (back to FABGPU_CAP_V2_0, versions dropped).
+ *   _channel_capability: FABGPU_CAP_V2_0 (the default) for a channel whose application capability has V2_0Validation: the v2.0
+ *       validator with the plugin dispatcher.  FABGPU_CAP_V1_3 for a V1_3, V1_4_2 or V1_4_3 channel: the v1.4 validator
+ *       (core/committer/txvalidator/v14) with the builtin v13 VSCC.  In that mode:
+ *       - an empty or mismatched chaincode name, or an empty version, is INVALID_OTHER_REASON (255) instead of 25;
+ *       - an application chaincode writing to lscc, vscc, escc or cscc, and an invocation of vscc or escc, is ILLEGAL_WRITESET (23);
+ *       - an invocation of qscc or cscc validates only that namespace, against its namespace-table entry (the reference uses
+ *         SignedByAnyMember over the channel's MSP ids), without a version check;
+ *       - an application chaincode's namespaces are validated in order, the invoked one first, and the first failure decides: a
+ *         namespace without a table entry is 254 only when those before it passed;
+ *       - the invoked chaincode's version (ChaincodeAction.chaincode_id.version) must equal its lscc version: EXPIRED_CHAINCODE (17)
+ *         otherwise, 254 when no version is installed for it;
+ *       - each namespace is checked on its own writes: a key's validation parameter if the key table holds one, otherwise the
+ *         chaincode policy; the collection policies are not used;
+ *       - an invocation of lscc (deploy / upgrade) is 254, and so is every transaction of that block that would be VALID: an
+ *         upgrade invalidates the block's later invocations of the chaincode it names, which the device does not decide.  This
+ *         holds for every lscc invocation flagged 254, whatever stopped it (a creator outside the table, more than 8 namespaces);
+ *         one flagged with another code is one the reference rejects too, and leaves the block's flags alone.
+ *       Any other value is FABGPU_E_ARG and the mode is kept.  So is FABGPU_CAP_V1_3 while a namespace root reaches an ImplicitMeta
+ *       node: lscc chaincode definitions hold signature policies.  V1_2 and older capabilities are not supported.
+ *   _namespace_versions: the lscc ChaincodeData.Version of each entry of the installed namespace table (_namespace_policies, in
+ *       its order): ver_blob with (n_ns + 1) offsets, an empty string for no version.  n_ns must equal the table's size, else
+ *       FABGPU_E_ARG and nothing changes; n_ns = 0 with an empty table drops the versions.  _namespace_policies drops them too.
+ *   On a V1_3 channel the namespace table lists the chaincodes whose lscc ChaincodeData.Vscc is "vscc", with the policy of their
+ *   ChaincodeData.Policy, plus qscc and cscc with SignedByAnyMember(channel MSP ids); a chaincode with another VSCC is left out,
+ *   so its transactions are 254.  While FABGPU_CAP_V1_3 is set, _namespace_policies refuses a root that reaches an ImplicitMeta
+ *   node, and an empty table (n_ns = 0) when node 0 -- then every namespace's policy -- reaches one (FABGPU_E_ARG, the previous
+ *   table kept). */
+enum { FABGPU_CAP_V2_0 = 0, FABGPU_CAP_V1_3 = 1 };
+int fabgpu_channel_capability(fabgpu_ctx* ctx, int cap);
+int fabgpu_namespace_versions(fabgpu_ctx* ctx, const uint8_t* ver_blob, const uint32_t* ver_off, int n_ns);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their

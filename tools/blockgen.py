@@ -188,13 +188,15 @@ class Network:
 
 
 def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, seed=7, number=1, nthreads=None, mutate=None, namespaces=None,
-                endorsers=None, events=None):
+                endorsers=None, events=None, chaincode=None):
     """faults: {tx_index: fault_name}.  Returns (block_bytes, info); the oracle decides the validation codes.
     mutate(t, part, data) -> bytes rewrites the serialized message `part` (one of PARTS; t = None for the Block) of transaction t as
     it is assembled: the tx id, the proposal hash, the endorsement and creator signatures and every enclosing length prefix are
     then computed from the returned bytes, as a client and its endorsers would.  namespaces(t) -> the read/write set's namespaces
     (see tx_rwset); endorsers(t) -> the Identity list that endorses t; events(t) -> True: the chaincode action carries a
-    ChaincodeEvent of the invoked chaincode.  Without these arguments the output does not depend on them."""
+    ChaincodeEvent of the invoked chaincode; chaincode(t) -> (name, version) of the invoked chaincode, in the header extension and the
+    chaincode action (default (CHAINCODE, "1.0")): "lscc" makes an lscc invocation, and namespaces(t) may name system namespaces such as
+    "lscc" or "escc" to write them.  Without these arguments the output does not depend on them."""
     import ctypes
     faults = faults or {}
     rng = np.random.default_rng(seed)
@@ -230,7 +232,8 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
             txid = hashlib.sha256(b"x" + nonce + creator).hexdigest()
         channel = net.channel if f != "wrong_channel" else "other-channel"
         htype = pb.HEADER_TYPE_ENDORSER_TRANSACTION if f != "config_update_type" else pb.HEADER_TYPE_CONFIG_UPDATE
-        hext = pb.f_bytes(2, mut("ChaincodeID", chaincode_id(CHAINCODE)))  # peer.ChaincodeHeaderExtension{chaincode_id = 2}
+        cc_name, cc_ver = chaincode(t) if chaincode else (CHAINCODE, "1.0")
+        hext = pb.f_bytes(2, mut("ChaincodeID", chaincode_id(cc_name)))    # peer.ChaincodeHeaderExtension{chaincode_id = 2}
         if f == "bad_header_extension":
             hext = b"\x12\x7fshort"                                         # length prefix runs past the end
         hext = mut("ChaincodeHeaderExtension", hext)
@@ -251,8 +254,8 @@ def build_block(net: Network, n_tx: int, n_endorsements: int = 3, faults=None, s
         rwset = tx_rwset(nss, mut)
         if f == "bad_rwset":
             rwset = pb.f_bytes(2, b"\x0a\x7fnamespace-length-runs-past-the-end")
-        ccact = pb.f_bytes(1, rwset) + pb.f_bytes(4, mut("ChaincodeID", chaincode_id("othercc" if f == "cc_name_mismatch" else CHAINCODE,
-                                                                                     "" if f == "empty_cc_version" else "1.0")))
+        ccact = pb.f_bytes(1, rwset) + pb.f_bytes(4, mut("ChaincodeID", chaincode_id("othercc" if f == "cc_name_mismatch" else cc_name,
+                                                                                     "" if f == "empty_cc_version" else cc_ver)))
         if f == "event_wrong_cc":
             ccact += pb.f_bytes(2, mut("ChaincodeEvent", pb.f_bytes(1, b"othercc") + pb.f_bytes(3, b"evt")))
         elif events and events(t):                                         # ChaincodeEvent{chaincode_id=1, event_name=3, payload=4}
