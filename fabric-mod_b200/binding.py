@@ -30,6 +30,7 @@ EXPORTS = [
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
+    "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info",
 ]
 
 
@@ -459,6 +460,31 @@ class Context:
         nd = np.ascontiguousarray(np.asarray(nodes if nodes is not None and len(nodes) else np.zeros((0, 4)), dtype=np.int32).reshape(-1, 4))
         ndp = nd if nd.shape[0] else np.zeros((1, 4), np.int32)
         self._ck(fn(self._h, _p(ndp), ctypes.c_int(nd.shape[0]), _p(nb), _p(no), _p(cb), _p(co), _p(kb), _p(ko), _p(roots), ctypes.c_int(len(keys))))
+
+    def committed_txids(self, ids, kinds=None, capacity=0):
+        """Replaces the ledger's committed tx-id set (fabgpu_committed_txids).  ids: tx id strings (str or bytes, as in ChannelHeader.tx_id);
+        kinds: one per id, 0 = committed (a transaction with that id is DUPLICATE_TXID), 1 = indexed but GetTransactionByID fails (254);
+        None = all 0.  capacity sizes the table for that many ids.  No ids and capacity 0 remove the set."""
+        self._committed_txids(lib().fabgpu_committed_txids, ids, kinds, (ctypes.c_size_t(capacity),))
+
+    def committed_txids_add(self, ids, kinds=None):
+        """Upserts ids into the installed set (fabgpu_committed_txids_add) without draining the blocks in flight: seen by every block
+        submitted after this returns, by none submitted before."""
+        self._committed_txids(lib().fabgpu_committed_txids_add, ids, kinds, ())
+
+    def committed_txids_info(self):
+        """(distinct ids held, table slots)"""
+        out = (ctypes.c_ulonglong * 2)()
+        self._ck(lib().fabgpu_committed_txids_info(self._h, out))
+        return int(out[0]), int(out[1])
+
+    def _committed_txids(self, fn, ids, kinds, extra):
+        ids = [x.encode() if isinstance(x, str) else bytes(x) for x in ids]
+        b, o = _blob(ids)
+        k = None if kinds is None else np.ascontiguousarray(np.asarray(list(kinds) or [0], np.uint8))
+        if k is not None and len(ids) and k.shape[0] != len(ids):
+            raise ValueError("one kind per id")
+        self._ck(fn(self._h, _p(b), _p(o), _p(k), ctypes.c_size_t(len(ids)), *extra))
 
     def block_buffer(self, nbytes, slot=0):
         """Pinned staging buffer (numpy view) for block bytes; one per slot."""

@@ -21,6 +21,8 @@
 #define BD_HD inline
 #endif
 
+#include "txidset.cuh"
+
 namespace fabgpu { namespace bdev {
 
 enum : uint8_t {
@@ -1137,9 +1139,11 @@ BD_HD uint8_t decide_v13(const uint8_t* base, const TxDev& tx, uint32_t t, const
 // msgvalidation.go:40-57, and reads chaincode definitions from the ledger, dispatcher.go:224-277).
 // kl: the block's write records and metadata-write set, used while a key policy table is installed (pol.kp_size != 0); decide_tx then
 // sets bit 0 of kl->conflicted[t] when an earlier transaction metadata-wrote a key t writes, for the resolve stage (kl_resolve_step).
+// txids: the committed tx-id set (fabgpu_committed_txids), null = none installed.
 template <typename SigOk>
 BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const MspDev& msp, const PolicyDev& pol, SigOk sig_ok,
-                        const int32_t* job_identity, const uint8_t* digests, uint32_t J_cap, uint64_t* txid_hash_out, KlArrays* kl = nullptr)
+                        const int32_t* job_identity, const uint8_t* digests, uint32_t J_cap, uint64_t* txid_hash_out, KlArrays* kl = nullptr,
+                        const TxidSetDev* txids = nullptr)
 {
     const char hex[] = "0123456789abcdef";
     if (tx.early != TXC_NOT_VALIDATED) return tx.early;
@@ -1159,6 +1163,11 @@ BD_HD uint8_t decide_tx(const uint8_t* base, const TxDev& tx, uint32_t t, const 
     if (tx.phash_claimed.len != 32 || !bytes_equal(base + tx.phash_claimed.off, digests + 32 * (size_t)(J_cap + 2 * t + 1), 32))
         return TXC_INVALID_ENDORSER_TRANSACTION;
     if (!tx.channel_ok) return TXC_TARGET_CHAIN_NOT_FOUND;
+    if (txids) {                                                      // checkTxIdDupsLedger, both validators: the id is the CheckTxID digest
+        const uint32_t st = txid_lookup(*txids, digests + 32 * (size_t)(J_cap + 2 * t));
+        if (st == TXID_COMMITTED) return TXC_DUPLICATE_TXID;
+        if (st == TXID_UNANSWERABLE) return TXC_NOT_VALIDATED;        // GetTransactionByID fails: a terminal error of the reference's block
+    }
     if (tx.disp != TXC_VALID) return tx.disp;                         // the plugin dispatcher's own checks
     if (!tx.endorsements_parse_ok) return TXC_INVALID_OTHER_REASON;
     if (tx.overflow) return TXC_NOT_VALIDATED;                        // job arrays were full: CPU validator

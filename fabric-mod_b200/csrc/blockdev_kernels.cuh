@@ -31,20 +31,21 @@ block_resolve_kernel(const uint8_t* __restrict__ block, const RawJob* __restrict
 }
 
 // Replays the reference's decision order for every transaction on the verification bitmask and the digests.  lscc_seen (v1.3 mode,
-// else null): set when an lscc invocation of the block is flagged 254 (lscc_mark).
+// else null): set when an lscc invocation of the block is flagged 254 (lscc_mark).  txids: the committed tx-id set as it stood when the
+// block was submitted; slots null and broken 0 = none installed.
 __global__ void __launch_bounds__(128)
 block_decide_kernel(const uint8_t* __restrict__ block, const TxDev* __restrict__ txs, uint32_t T, MspDev msp, PolicyDev pol,
                     const uint32_t* __restrict__ mask, const uint8_t* __restrict__ gate_ok, const int32_t* __restrict__ job_identity,
                     const uint8_t* __restrict__ digests, uint32_t J_cap,
                     uint8_t* __restrict__ flags, uint64_t* __restrict__ txid_hash, Seg* __restrict__ txid_seg, KlArrays kl,
-                    uint32_t* __restrict__ lscc_seen)
+                    uint32_t* __restrict__ lscc_seen, TxidSetDev txids)
 {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     uint64_t h = 0;
     if (kl.w) kl_mark(block, t, txs[t], kl);
     const uint8_t f = decide_tx(block, txs[t], t, msp, pol, [&](uint32_t j) { return gate_ok[j] && ((mask[j >> 5] >> (j & 31)) & 1u); }, job_identity, digests,
-                                J_cap, &h, kl.w ? &kl : nullptr);
+                                J_cap, &h, kl.w ? &kl : nullptr, txids.slots || txids.broken ? &txids : nullptr);
     flags[t] = f;
     if (lscc_seen) lscc_mark(txs[t], f, lscc_seen);
     txid_hash[t] = h;
@@ -78,6 +79,31 @@ block_kl_resolve_kernel(const TxDev* __restrict__ txs, uint32_t T, KlArrays kl, 
     __syncthreads();
     if (tid != 0) return;
     for (uint32_t k = 0; k < total; k++) kl_resolve_step(kl.clist[k], txs, kl, flags);
+}
+
+// fabgpu_committed_txids / _add: one thread per id of the call (ids distinct within the call).  *count += the ids that were new.
+__global__ void __launch_bounds__(256)
+txid_insert_kernel(TxidSlot* __restrict__ tab, uint32_t mask, uint64_t seed, const TxidSlot* __restrict__ rec, uint32_t n,
+                   unsigned long long* __restrict__ count)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t w[8];
+    for (int k = 0; k < 8; k++) w[k] = rec[i].w[k];
+    if (txid_insert(tab, mask, seed, w, rec[i].state) == 1) atomicAdd(count, 1ull);
+}
+
+// Growth: one thread per slot of the old table re-inserts its id into the new one
+__global__ void __launch_bounds__(256)
+txid_rehash_kernel(TxidSlot* __restrict__ tab, uint32_t mask, uint64_t seed, const TxidSlot* __restrict__ old, uint64_t n_old)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_old) return;
+    const uint32_t st = old[i].state;
+    if (st < TXID_COMMITTED) return;
+    uint32_t w[8];
+    for (int k = 0; k < 8; k++) w[k] = old[i].w[k];
+    txid_insert(tab, mask, seed, w, st);
 }
 
 // fabgpu_key_policies_update: writes the changed slots of the key policy table

@@ -27,6 +27,7 @@
 #include "sha256.cuh"
 #include "blockdev_kernels.cuh"
 #include "keypolicy.hpp"
+#include "txidset.hpp"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -258,6 +259,23 @@ struct fabgpu_ctx {
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
     } dbs[FABGPU_SLOTS];
     std::mutex blk_mu[FABGPU_SLOTS];
+    // fabgpu_committed_txids: the ledger's tx ids on device 0 (txidset.cuh); ledger state, so fabgpu_msp_configure keeps it.  A mutation runs
+    // on `stream` under slot0_mu: it first waits for every slot's last block_decide_kernel (decide_ev) -- blocks submitted before it never
+    // see it -- and records `ev`, which every later block_submit makes its decide stage wait for.  The host never waits for an add (that
+    // would wait for the decide stage of the block just submitted): the pinned staging buffers rotate, each guarded by its own event, and
+    // growth is decided on `count` (exact as of the last finished mutation) + `pending` (ids sent since, an upper bound of the new ones).
+    struct TxidSet {
+        static constexpr int RING = 4;
+        Stream stream; Event ev; bool ev_set = false;
+        Event decide_ev[FABGPU_SLOTS]; bool decide_set[FABGPU_SLOTS] = {};
+        HostArray<bdev::TxidSlot> h_stage[RING]; Event stage_ev[RING]; bool stage_set[RING] = {}; unsigned seq = 0;
+        DevArray<bdev::TxidSlot> d_stage;
+        HostArray<unsigned long long> h_count; DevArray<unsigned long long> d_count;
+        bdev::TxidSlot* table = nullptr; uint64_t slots = 0;                   // table: stream-ordered allocation on `stream`
+        const uint64_t seed = txid::random_seed();
+        bool installed = false, broken = false; unsigned long long count = 0, pending = 0;
+        ~TxidSet() { if (table) cudaFree(table); }
+    } txid;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
     ~fabgpu_ctx() { if (!devs.empty()) cudaSetDevice(devs[0].id); }
 };
@@ -2012,6 +2030,169 @@ int fabgpu_key_policies_update(fabgpu_ctx* ctx, const int32_t* nodes, int n_node
     return key_policies(ctx, false, nodes, n_nodes, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, root, n);
 }
 
+// ---- committed tx-id set (fabgpu_committed_txids / _add / _info); every step below runs under slot0_mu -----------------------------
+// Brings the set's stream behind every block already submitted.  sync: the caller's thread also waits for the previous mutation; else
+// its count is taken only if it has finished.
+static int txid_begin(fabgpu_ctx* ctx, bool sync)
+{
+    auto& s = ctx->txid;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    if (!s.stream) {
+        cudaStream_t st = nullptr; cudaEvent_t ev = nullptr;
+        CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); s.stream.reset(st);
+        CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); s.ev.reset(ev);
+        for (auto& e : s.stage_ev) { cudaEvent_t x = nullptr; CK(ctx, cudaEventCreateWithFlags(&x, cudaEventDisableTiming)); e.reset(x); }
+        if (int rc = s.d_count.reserve(ctx, 8)) return rc;
+        if (int rc = s.h_count.reserve(ctx, 8)) return rc;
+    }
+    if (s.ev_set) {
+        if (sync) CK(ctx, cudaEventSynchronize(s.ev.get()));
+        const cudaError_t q = sync ? cudaSuccess : cudaEventQuery(s.ev.get());
+        if (q == cudaSuccess) { s.count = s.h_count.get()[0]; s.pending = 0; }
+        else if (q == cudaErrorNotReady) { if (cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError(); }
+        else CK(ctx, q);
+    }
+    for (int k = 0; k < FABGPU_SLOTS; k++)
+        if (s.decide_set[k]) CK(ctx, cudaStreamWaitEvent(s.stream.get(), s.decide_ev[k].get(), 0));
+    return FABGPU_OK;
+}
+
+static uint64_t txid_max_bytes()
+{
+    const char* v = getenv("FABGPU_TXID_MAX_BYTES");      // bound on the table's bytes; unset = whatever cudaMalloc grants
+    return v && *v ? strtoull(v, nullptr, 10) : ~0ull;
+}
+
+// Frees the table in stream order: the blocks that read it have been waited for (txid_begin)
+static void txid_drop_table(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->txid;
+    if (s.table) cudaFreeAsync(s.table, s.stream.get());
+    s.table = nullptr; s.slots = 0;
+}
+
+// Grows the table (doubling, to at least min_slots) so that `recs` fit at a load of at most 1/2, inserts them, and records the set event
+static int txid_insert_records(fabgpu_ctx* ctx, const std::vector<bdev::TxidSlot>& recs, uint64_t min_slots)
+{
+    auto& s = ctx->txid;
+    cudaStream_t st = s.stream.get();
+    const uint64_t want = std::max(txid::slots_for(s.count + s.pending + recs.size(), s.slots), min_slots);
+    if (want != s.slots) {
+        const uint64_t bytes = want * sizeof(bdev::TxidSlot);
+        if (bytes > txid_max_bytes() || want > (1ull << 32)) {
+            char buf[192];
+            snprintf(buf, sizeof buf, "committed tx-id table of %llu slots (%llu bytes) exceeds FABGPU_TXID_MAX_BYTES", (unsigned long long)want,
+                     (unsigned long long)bytes);
+            ctx->last_error = buf;
+            return FABGPU_E_CUDA;
+        }
+        bdev::TxidSlot* nt = nullptr;
+        CK(ctx, cudaMallocAsync(reinterpret_cast<void**>(&nt), bytes, st));
+        if (cudaMemsetAsync(nt, 0, bytes, st) != cudaSuccess) { cudaFreeAsync(nt, st); ctx->last_error = "committed tx-id table clear failed"; return FABGPU_E_CUDA; }
+        if (s.table) {
+            bdev::txid_rehash_kernel<<<(unsigned)((s.slots + 255) / 256), 256, 0, st>>>(nt, (uint32_t)(want - 1), s.seed, s.table, s.slots);
+            ctx->launches++;
+            if (cudaGetLastError() != cudaSuccess) { cudaFreeAsync(nt, st); ctx->last_error = "committed tx-id rehash launch failed"; return FABGPU_E_CUDA; }
+        }
+        txid_drop_table(ctx);
+        s.table = nt; s.slots = want;
+    }
+    const size_t n = recs.size();
+    if (n) {
+        const int r = (int)(s.seq++ % fabgpu_ctx::TxidSet::RING);
+        auto& hs = s.h_stage[r];
+        if (s.stage_set[r]) CK(ctx, cudaEventSynchronize(s.stage_ev[r].get()));     // its copy, RING mutations ago
+        const size_t bytes = n * sizeof(bdev::TxidSlot);
+        if (bytes > hs.bytes())
+            if (int rc = hs.reserve(ctx, std::max(bytes, 2 * hs.bytes()))) return rc;
+        if (bytes > s.d_stage.bytes())
+            if (int rc = s.d_stage.reserve(ctx, std::max(bytes, 2 * s.d_stage.bytes()))) return rc;
+        memcpy(hs.get(), recs.data(), bytes);
+        CK(ctx, cudaMemcpyAsync(s.d_stage.get(), hs.get(), bytes, cudaMemcpyHostToDevice, st));
+        CK(ctx, cudaEventRecord(s.stage_ev[r].get(), st));
+        s.stage_set[r] = true;
+        s.pending += n;
+        bdev::txid_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.table, (uint32_t)(s.slots - 1), s.seed, s.d_stage.get(), (uint32_t)n,
+                                                                             s.d_count.get());
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+    }
+    CK(ctx, cudaMemcpyAsync(s.h_count.get(), s.d_count.get(), 8, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaEventRecord(s.ev.get(), st));
+    s.ev_set = true;
+    return FABGPU_OK;
+}
+
+// A failed mutation may have lost ids: from here on every lookup answers "unanswerable" (254) until a replacing call succeeds
+static int txid_fail(fabgpu_ctx* ctx, int rc)
+{
+    auto& s = ctx->txid;
+    const std::string err = ctx->last_error;
+    s.broken = true;
+    if (s.stream) {
+        txid_drop_table(ctx);
+        if (cudaEventRecord(s.ev.get(), s.stream.get()) == cudaSuccess) s.ev_set = true;
+    }
+    ctx->last_error = err + " (the committed tx-id set is broken until fabgpu_committed_txids replaces it)";
+    return rc;
+}
+
+int fabgpu_committed_txids(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n, size_t capacity_hint)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::vector<bdev::TxidSlot> recs;
+    if (const char* err = txid::prepare(id_blob, id_off, kind, n, ctx->txid.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->txid;
+    int rc = drain_block_streams(ctx);                         // a replacement is rare: it simply lets the blocks in flight finish
+    if (!rc) rc = txid_begin(ctx, true);
+    if (rc) return s.installed ? txid_fail(ctx, rc) : rc;
+    txid_drop_table(ctx);
+    s.installed = s.broken = false; s.count = s.pending = 0;
+    if (n == 0 && capacity_hint == 0) {                        // removed: every flag is what it is without a set
+        CK(ctx, cudaEventRecord(s.ev.get(), s.stream.get()));
+        s.ev_set = true;
+        return FABGPU_OK;
+    }
+    s.installed = true;
+    CK(ctx, cudaMemsetAsync(s.d_count.get(), 0, 8, s.stream.get()));
+    // the hint sizes the table up front when it fits under the byte bound; the ids given must fit in any case
+    uint64_t hint_slots = txid::slots_for(capacity_hint);
+    if (hint_slots * sizeof(bdev::TxidSlot) > txid_max_bytes()) hint_slots = 0;
+    if ((rc = txid_insert_records(ctx, recs, hint_slots))) return txid_fail(ctx, rc);
+    return FABGPU_OK;
+}
+
+int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::vector<bdev::TxidSlot> recs;
+    if (const char* err = txid::prepare(id_blob, id_off, kind, n, ctx->txid.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->txid;
+    if (!s.installed) { ctx->last_error = "no committed tx-id set installed: call fabgpu_committed_txids first"; return FABGPU_E_ARG; }
+    if (s.broken) { ctx->last_error = "the committed tx-id set is broken by a failed call: replace it with fabgpu_committed_txids"; return FABGPU_E_ARG; }
+    int rc = txid_begin(ctx, false);
+    if (!rc) rc = txid_insert_records(ctx, recs, 0);
+    return rc ? txid_fail(ctx, rc) : FABGPU_OK;
+}
+
+int fabgpu_committed_txids_info(const fabgpu_ctx* cctx, unsigned long long out[2])
+{
+    if (!cctx || !out) return FABGPU_E_ARG;
+    fabgpu_ctx* ctx = const_cast<fabgpu_ctx*>(cctx);          // waits for the last mutation to read its count; changes nothing
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->txid;
+    if (s.ev_set) {
+        CK(ctx, cudaSetDevice(ctx->devs[0].id));
+        CK(ctx, cudaEventSynchronize(s.ev.get()));
+        if (s.installed && !s.broken) { s.count = s.h_count.get()[0]; s.pending = 0; }
+    }
+    out[0] = s.installed && !s.broken ? s.count : 0;
+    out[1] = s.slots;
+    return FABGPU_OK;
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -2166,10 +2347,22 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     int rc = launch_verify(ctx, dv, dm.all_slots ? MODE_CACHED : MODE_MIXED, db.d_ks.get(), db.d_qx.get(), db.d_qy.get(), db.d_dig.get(), db.d_r.get(), db.d_s.get(), J_cap, db.d_mask.get(), db.d_off.get(), st,
                            db.d_counter.get(), cnt, nullptr, db.d_idx.get(), dm.classes ? dm.classes : CLASS_GENERIC, db.d_scal.get());
     if (rc) return rc;
+    // the committed tx-id set as the mutations returned so far left it (all of them, as submitters and mutations hold slot0_mu)
+    auto& tx_set = ctx->txid;
+    bdev::TxidSetDev tsd{nullptr, 0, 0, 0};
+    if (tx_set.installed) {
+        tsd.slots = tx_set.table; tsd.mask = (uint32_t)(tx_set.slots - 1); tsd.seed = tx_set.seed; tsd.broken = tx_set.broken || !tx_set.table;
+        if (tx_set.ev_set) CK(ctx, cudaStreamWaitEvent(st, tx_set.ev.get(), 0));
+    }
     if (db.use_ev) CK(ctx, cudaEventRecord(db.ev[4].get(), st));
     bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), db.d_txs.get(), cnt, m, pol, db.d_mask.get(), db.d_gate.get(), db.d_ident.get(), db.d_dig.get(), (uint32_t)J_cap, db.d_flags.get(),
-                                                               db.d_hash.get(), db.d_seg.get(), kl, db.v13 ? db.d_counter.get() + 1 : nullptr);
+                                                               db.d_hash.get(), db.d_seg.get(), kl, db.v13 ? db.d_counter.get() + 1 : nullptr, tsd);
     ctx->launches++;
+    if (tx_set.installed) {                                   // a later mutation of the set waits for this decide stage
+        if (!tx_set.decide_ev[slot]) { cudaEvent_t ev = nullptr; CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); tx_set.decide_ev[slot].reset(ev); }
+        CK(ctx, cudaEventRecord(tx_set.decide_ev[slot].get(), st));
+        tx_set.decide_set[slot] = true;
+    }
     if (db.kl_on) {
         bdev::block_kl_resolve_kernel<<<1, 256, 0, st>>>(db.d_txs.get(), cnt, kl, db.d_flags.get());
         ctx->launches++;

@@ -209,8 +209,10 @@ int fabgpu_gate_signature(const uint8_t* sig, size_t sig_len, uint8_t r_out[32],
  * common/policies/policy.go:365-402) -- with the SHA-256 of each signed message computed on the device straight from the
  * block bytes, then replays the reference's per-transaction decision order (msgvalidation.go:248-320, v20/validator.go:
  * 300-455, cauthdsl.go:24-92, markTXIdDuplicates) and writes the TRANSACTIONS_FILTER bytes (peer.TxValidationCode).
- * Outside the pre-pass, exactly as mocked in the reference's unit tests: ledger lookups, chaincode definitions, rw-sets,
- * key-level policies.  Config transactions are flagged 254 (NOT_VALIDATED) and must be validated by the CPU validator. */
+ * The ledger's inputs come as tables the caller installs: chaincode definitions (_namespace_policies, _namespace_versions), collection
+ * and key-level policies, and the committed tx ids (fabgpu_committed_txids): once a set is installed, a transaction whose id the ledger
+ * already holds is DUPLICATE_TXID (9) as in the reference; without one the device does not look ids up in the ledger.  Config
+ * transactions are flagged 254 (NOT_VALIDATED) and must be validated by the CPU validator. */
 
 /* Installs the MSP view and the endorsement policy used by fabgpu_validate_block.
  * identities: n_ids serialized msp.SerializedIdentity byte strings (id_blob + (n_ids+1) offsets) exactly as they appear in
@@ -234,7 +236,7 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
                          const int32_t* policy_nodes, int n_nodes, const uint8_t* principal_blob, const uint32_t* principal_off,
                          int n_principals, const char* channel_id);
 /* Optional refinements of the table fabgpu_msp_configure installed (call them after it; each drains the block slots first;
- * fabgpu_msp_configure clears all four):
+ * fabgpu_msp_configure clears all four -- but not the committed tx-id set, which is ledger state, not channel configuration):
  *   _identity_groups: group[i] = de-duplication id of identity i.  The reference de-duplicates a transaction's signers on
  *       Mspid + certificate digest (common/policies/policy.go:380-386), so two byte-different serializations of ONE certificate
  *       must share a group; without this call every table entry is its own group.
@@ -328,6 +330,34 @@ int fabgpu_key_policies_update(fabgpu_ctx* ctx, const int32_t* nodes, int n_node
 enum { FABGPU_CAP_V2_0 = 0, FABGPU_CAP_V1_3 = 1 };
 int fabgpu_channel_capability(fabgpu_ctx* ctx, int cap);
 int fabgpu_namespace_versions(fabgpu_ctx* ctx, const uint8_t* ver_blob, const uint32_t* ver_off, int n_ns);
+/* The ledger's committed transaction ids, for checkTxIdDupsLedger (core/committer/txvalidator/v20/validator.go:363-372,462-491,
+ * v14/validator.go:334-345).  Ids are ChannelHeader.tx_id byte strings: id_blob with n + 1 offsets; kind[i] (kind NULL = all 0) says
+ * what the ledger's GetTransactionByID answers for id i: 0 = found (the block store indexes the id of every transaction of every
+ * committed block, whatever its flag), 1 = indexed but the lookup fails (ids imported from a snapshot, whose index value is empty).
+ *   fabgpu_committed_txids replaces the set; n = 0 with capacity_hint = 0 removes it.  capacity_hint (ids) sizes the table up front.
+ *       It drains the block slots first.
+ *   fabgpu_committed_txids_add upserts ids into the installed set without draining the slots: what a peer calls with a block's ids
+ *       right after submitting that block.  FABGPU_E_ARG when no set is installed.
+ *   An id given twice keeps the larger kind.  Only canonical ids are kept -- 64 characters of [0-9a-f], stored as 32 binary bytes: a
+ *   transaction reaches the ledger check only after CheckTxID has passed, so its id is the lowercase hex of SHA-256(nonce || creator),
+ *   and an id in any other form (uppercase, another length, empty) can never match.
+ *   Ordering: an add or replace is never seen by a block submitted before the call (its own ids do not flag it), and is seen by every
+ *   block submitted after the call returns.  The caller's arrays are not referenced after the call returns.
+ *   While a set is installed, an endorser transaction that passed the checks up to TARGET_CHAIN_NOT_FOUND (14) is DUPLICATE_TXID (9)
+ *   when its id has kind 0 and 254 when it has kind 1, before the dispatcher, the chaincode definitions and the policies decide
+ *   anything, in both validator modes.  A ledger duplicate is not VALID, so it takes no part in the in-block duplicate pass, and a later
+ *   writer of a key it metadata-writes is 254.  Config transactions stay 254.
+ *   Memory: 36 bytes per slot, a power-of-two slot count at a load of at most 1/2 (at least 1024 slots): 2^25 slots, 1.2 GB, for 10^7
+ *   ids.  The table doubles as ids are added; FABGPU_TXID_MAX_BYTES (environment) bounds its bytes.  When growing or inserting fails
+ *   (that bound, or an allocation failure) the call returns an error and the set is broken: every transaction that reaches the ledger
+ *   check is 254, and _add is refused, until a fabgpu_committed_txids call succeeds.  The device never answers "not found" from a set
+ *   that lacks ids.
+ *   FABGPU_E_ARG, with a fabgpu_last_error text and the previous set kept, for NULL arrays with n > 0, decreasing offsets and a kind
+ *   other than 0 or 1.  fabgpu_msp_configure keeps the set.
+ *   fabgpu_committed_txids_info: out[0] = distinct ids held (0 while broken or removed), out[1] = table slots. */
+int fabgpu_committed_txids(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n, size_t capacity_hint);
+int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n);
+int fabgpu_committed_txids_info(const fabgpu_ctx* ctx, unsigned long long out[2]);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
