@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FABGPU_LIB") or os.path.join(_HERE, "lib", "libfabgpu_ecdsa.so")
 SLOTS = 3
 CAP_V2_0, CAP_V1_3 = 0, 1      # fabgpu_channel_capability
+STATE_REMOVE = (2 ** 64 - 1, 2 ** 64 - 1)   # fabgpu_state_versions_update: a version that removes the key
 
 OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
 (ST_VALID, ST_INVALID, ST_ERR_NIL_KEY, ST_ERR_EMPTY_SIG, ST_ERR_EMPTY_DIGEST, ST_ERR_UNMARSHAL, ST_ERR_R_NOT_POSITIVE,
@@ -31,6 +32,7 @@ EXPORTS = [
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info",
+    "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
 ]
 
 
@@ -485,6 +487,42 @@ class Context:
         if k is not None and len(ids) and k.shape[0] != len(ids):
             raise ValueError("one kind per id")
         self._ck(fn(self._h, _p(b), _p(o), _p(k), ctypes.c_size_t(len(ids)), *extra))
+
+    def state_versions(self, entries, height, capacity=0):
+        """Replaces the world-state version table of the MVCC stage (fabgpu_state_versions).  entries: [((namespace, collection, key),
+        (block_num, tx_num))] -- collection "" for a public key, key str or bytes (the 32-byte key hash for a collection key); height:
+        committed blocks, the next block validate_mvcc checks.  capacity sizes the table for that many keys.  No entries and capacity 0
+        remove the table."""
+        self._state_versions(lib().fabgpu_state_versions, entries, height, (ctypes.c_size_t(capacity),))
+
+    def state_versions_update(self, entries, height):
+        """Upserts entries (fabgpu_state_versions_update); a version of STATE_REMOVE removes the key.  A height above the table's
+        closes a block validate_mvcc left open."""
+        self._state_versions(lib().fabgpu_state_versions_update, entries, height, ())
+
+    def state_versions_info(self):
+        """(keys held, table slots, height, keys unknown)"""
+        out = (ctypes.c_ulonglong * 4)()
+        self._ck(lib().fabgpu_state_versions_info(self._h, out))
+        return tuple(int(x) for x in out)
+
+    def validate_mvcc(self, slot, block_num, tv_flags):
+        """The MVCC stage of the block validate_wait(slot) returned (fabgpu_validate_mvcc): tv_flags are the validator's flags, the result
+        the committed ones (VALID, 11 or 254 for each VALID, the others copied).  Applies the block to the table at height block_num."""
+        tv = np.ascontiguousarray(np.asarray(tv_flags, np.uint8))
+        flags = np.zeros(max(tv.shape[0], 1), np.uint8)
+        self._ck(lib().fabgpu_validate_mvcc(self._h, ctypes.c_int(slot), ctypes.c_uint64(block_num), _p(tv if tv.size else flags), _p(flags),
+                                            ctypes.c_size_t(tv.shape[0])))
+        return flags[: tv.shape[0]]
+
+    def _state_versions(self, fn, entries, height, extra):
+        b = lambda x: x.encode() if isinstance(x, str) else bytes(x)
+        entries = list(entries)
+        nb, no = _blob([b(k[0]) for k, _ in entries])
+        cb, co = _blob([b(k[1]) for k, _ in entries])
+        kb, ko = _blob([b(k[2]) for k, _ in entries])
+        ver = np.ascontiguousarray(np.array([x for _, v in entries for x in v] or [0], np.uint64))
+        self._ck(fn(self._h, _p(nb), _p(no), _p(cb), _p(co), _p(kb), _p(ko), _p(ver), ctypes.c_size_t(len(entries)), ctypes.c_uint64(height), *extra))
 
     def block_buffer(self, nbytes, slot=0):
         """Pinned staging buffer (numpy view) for block bytes; one per slot."""

@@ -529,7 +529,9 @@ BD_HD uint32_t kl_atomic_add(uint32_t* p, uint32_t n)
 // Every write of a TxReadWriteSet as rwset.FromProtoBytes reads it, in baseEvaluator.Evaluate's terms (validator_keylevel.go:86-142):
 // on_write(namespace, collection, key, is_metadata) for each KVWrite{key = 1} and KVMetadataWrite{key = 1} of a namespace's KVRWSet and each
 // KVWriteHash{key_hash = 1} and KVMetadataWriteHash{key_hash = 1} of its collections.  false when a level does not parse.
-template <typename F>
+// Reads (the MVCC stage, stateset.cuh): on_write(namespace, collection, key, field, record) -> bool for every record instead, reads and
+// range queries included -- field 1-4 of KVRWSet, 11-13 for field 1-3 of HashedRWSet; a range query has no key; false = does not parse.
+template <bool Reads = false, typename F>
 BD_HD bool kl_scan_rwset(const uint8_t* base, Seg results, F on_write)
 {
     bool ok = true;
@@ -541,10 +543,13 @@ BD_HD bool kl_scan_rwset(const uint8_t* base, Seg results, F on_write)
         // KVMetadataWrite{key = 1, entries = 2}
         Seg none; none.off = none.len = 0;
         if (!scan_msg(base, kv, BD_F(1) | BD_F(2) | BD_F(3) | BD_F(4), 0, [&](uint32_t g, Seg w) {
-                if (!ok || (g != 3 && g != 4)) return;
+                if (!ok || (!Reads && g != 3 && g != 4)) return;
                 Seg key; key.off = key.len = 0;
-                if (!scan_msg(base, w, g == 3 ? BD_F(1) | BD_F(3) : BD_F(1) | BD_F(2), g == 3 ? BD_F(2) : 0, [&](uint32_t h, Seg k) { if (h == 1) key = k; })) { ok = false; return; }
-                on_write(name, none, key, g == 4);
+                // KVRead{key = 1, version = 2} (Reads); a RangeQueryInfo is handed over unparsed
+                if ((!Reads || g != 2) &&
+                    !scan_msg(base, w, g == 3 ? BD_F(1) | BD_F(3) : BD_F(1) | BD_F(2), g == 3 ? BD_F(2) : 0, [&](uint32_t h, Seg k) { if (h == 1) key = k; })) { ok = false; return; }
+                if constexpr (Reads) { if (!on_write(name, none, key, g, w)) ok = false; }
+                else on_write(name, none, key, g == 4);
             })) ok = false;
         if (!ok) return;
         scan_msg(base, nsb, BD_F(3), 0, [&](uint32_t, Seg cb) {          // CollectionHashedReadWriteSet{collection_name = 1, hashed_rwset = 2, pvt_rwset_hash = 3}
@@ -554,10 +559,11 @@ BD_HD bool kl_scan_rwset(const uint8_t* base, Seg results, F on_write)
             // HashedRWSet{hashed_reads = 1, hashed_writes = 2, metadata_writes = 3}; KVWriteHash{key_hash = 1, is_delete = 2, value_hash = 3,
             // is_purge = 4}, KVMetadataWriteHash{key_hash = 1, entries = 2}
             if (!scan_msg(base, hashed, BD_F(1) | BD_F(2) | BD_F(3), 0, [&](uint32_t g, Seg w) {
-                    if (!ok || (g != 2 && g != 3)) return;
-                    Seg key; key.off = key.len = 0;
+                    if (!ok || (!Reads && g != 2 && g != 3)) return;
+                    Seg key; key.off = key.len = 0;                   // KVReadHash{key_hash = 1, version = 2} (Reads)
                     if (!scan_msg(base, w, g == 2 ? BD_F(1) | BD_F(3) : BD_F(1) | BD_F(2), g == 2 ? BD_F(2) | BD_F(4) : 0, [&](uint32_t h, Seg k) { if (h == 1) key = k; })) { ok = false; return; }
-                    on_write(name, cname, key, g == 3);
+                    if constexpr (Reads) { if (!on_write(name, cname, key, 10 + g, w)) ok = false; }
+                    else on_write(name, cname, key, g == 3);
                 })) ok = false;
         });
     });

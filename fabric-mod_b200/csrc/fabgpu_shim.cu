@@ -28,6 +28,7 @@
 #include "blockdev_kernels.cuh"
 #include "keypolicy.hpp"
 #include "txidset.hpp"
+#include "stateset.hpp"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -254,6 +255,7 @@ struct fabgpu_ctx {
         DevArray<bdev::WriteRec> d_w; DevArray<uint64_t> d_md_hash; DevArray<unsigned long long> d_md_min; DevArray<uint32_t> d_md_sum, d_clist; DevArray<uint8_t> d_conf;
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
         bool busy = false, on_device = false, use_ev = false, kl_on = false, v13 = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
+        bool mvcc_ready = false;                 // fabgpu_validate_wait returned the block and its bytes are still on the device
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
@@ -276,6 +278,23 @@ struct fabgpu_ctx {
         bool installed = false, broken = false; unsigned long long count = 0, pending = 0;
         ~TxidSet() { if (table) cudaFree(table); }
     } txid;
+    // fabgpu_state_versions: the world state's key versions on device 0 (stateset.cuh); ledger state, so fabgpu_msp_configure keeps it.
+    // Every call runs under slot0_mu and returns with its stream synchronised -- replace and update on `stream`, fabgpu_validate_mvcc on
+    // the slot's stream -- so `count` is exact between calls and growth is decided on it plus the keys one call may add.  Blocks in
+    // flight never read the table.
+    struct StateSet {
+        Stream stream;
+        HostArray<bdev::StateSlot> h_stage; DevArray<bdev::StateSlot> d_stage;
+        HostArray<unsigned long long> h_count; DevArray<unsigned long long> d_count;   // [0..2]: StateSetDev::count, [3]: a failed upsert
+        bdev::StateSlot* table = nullptr; uint64_t slots = 0;                            // stream-ordered allocation
+        const uint64_t seed = txid::random_seed();
+        bool installed = false, broken = false, open = false; uint64_t height = 0; unsigned long long count[3] = {0, 0, 0};
+        // the MVCC stage's arrays (one stage runs at a time)
+        DevArray<bdev::MvccRec> d_rec; DevArray<uint32_t> d_first, d_n, d_mlist, d_ctr; DevArray<uint8_t> d_info, d_tv, d_flags;
+        DevArray<bdev::MvccKey> d_key; HostArray<uint8_t> h_flags; HostArray<uint32_t> h_ctr;
+        uint32_t rec_hint = 8;                                                           // records per transaction the arrays are sized for
+        ~StateSet() { if (table) cudaFree(table); }
+    } sv;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
     ~fabgpu_ctx() { if (!devs.empty()) cudaSetDevice(devs[0].id); }
 };
@@ -2193,6 +2212,260 @@ int fabgpu_committed_txids_info(const fabgpu_ctx* cctx, unsigned long long out[2
     return FABGPU_OK;
 }
 
+// ---- world-state version table and the MVCC stage (fabgpu_state_versions / _update / _info, fabgpu_validate_mvcc); under slot0_mu ----
+static int sv_begin(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->sv;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    if (!s.stream) {
+        cudaStream_t st = nullptr;
+        CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); s.stream.reset(st);
+        if (int rc = s.d_count.reserve(ctx, 32)) return rc;
+        if (int rc = s.h_count.reserve(ctx, 32)) return rc;
+        if (int rc = s.d_ctr.reserve(ctx, 16)) return rc;
+        if (int rc = s.h_ctr.reserve(ctx, 16)) return rc;
+    }
+    return FABGPU_OK;
+}
+
+static uint64_t sv_max_bytes()
+{
+    const char* v = getenv("FABGPU_STATE_MAX_BYTES");     // bound on the table's bytes; unset = whatever cudaMalloc grants
+    return v && *v ? strtoull(v, nullptr, 10) : ~0ull;
+}
+
+static bdev::StateSetDev sv_dev(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->sv;
+    bdev::StateSetDev d{s.table, (uint32_t)(s.slots - 1), s.broken ? 1u : 0u, s.seed, s.d_count.get()};
+    return d;
+}
+
+// Makes room for `more` further claimed slots at a load of at most 1/2 (and at least min_slots): a rehash into a fresh table on `st`,
+// which drops removed keys.  The old table is freed in stream order.
+static int sv_reserve(fabgpu_ctx* ctx, uint64_t more, uint64_t min_slots, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    if (s.table && s.slots >= min_slots && s.count[1] + more <= s.slots / 2) return FABGPU_OK;
+    const uint64_t want = std::max(stateset::slots_for(s.count[0] + more, s.slots), min_slots);
+    const uint64_t bytes = want * sizeof(bdev::StateSlot);
+    if (bytes > sv_max_bytes() || want > (1ull << 32)) {
+        char buf[192];
+        snprintf(buf, sizeof buf, "state version table of %llu slots (%llu bytes) exceeds FABGPU_STATE_MAX_BYTES", (unsigned long long)want,
+                 (unsigned long long)bytes);
+        ctx->last_error = buf;
+        return FABGPU_E_CUDA;
+    }
+    bdev::StateSlot* nt = nullptr;
+    CK(ctx, cudaMallocAsync(reinterpret_cast<void**>(&nt), bytes, st));
+    if (cudaMemsetAsync(nt, 0, bytes, st) != cudaSuccess || cudaMemsetAsync(s.d_count.get(), 0, 24, st) != cudaSuccess) {
+        cudaFreeAsync(nt, st); ctx->last_error = "state version table clear failed"; return FABGPU_E_CUDA;
+    }
+    bdev::StateSlot* old = s.table; const uint64_t n_old = s.slots;
+    s.table = nt; s.slots = want;
+    if (old) {
+        bdev::sv_rehash_kernel<<<(unsigned)((n_old + 255) / 256), 256, 0, st>>>(sv_dev(ctx), old, n_old, reinterpret_cast<int*>(s.d_count.get() + 3));
+        ctx->launches++;
+        const cudaError_t e = cudaGetLastError();
+        cudaFreeAsync(old, st);
+        if (e != cudaSuccess) { ctx->last_error = "state version rehash launch failed"; return FABGPU_E_CUDA; }
+    }
+    s.count[1] = s.count[0];
+    return FABGPU_OK;
+}
+
+// Upserts `recs` on `st` (room already made)
+static int sv_insert(fabgpu_ctx* ctx, const std::vector<bdev::StateSlot>& recs, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    const size_t n = recs.size();
+    if (!n) return FABGPU_OK;
+    const size_t bytes = n * sizeof(bdev::StateSlot);
+    if (bytes > s.h_stage.bytes())
+        if (int rc = s.h_stage.reserve(ctx, std::max(bytes, 2 * s.h_stage.bytes()))) return rc;
+    if (bytes > s.d_stage.bytes())
+        if (int rc = s.d_stage.reserve(ctx, std::max(bytes, 2 * s.d_stage.bytes()))) return rc;
+    memcpy(s.h_stage.get(), recs.data(), bytes);
+    CK(ctx, cudaMemcpyAsync(s.d_stage.get(), s.h_stage.get(), bytes, cudaMemcpyHostToDevice, st));
+    bdev::sv_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(sv_dev(ctx), s.d_stage.get(), (uint32_t)n, reinterpret_cast<int*>(s.d_count.get() + 3));
+    ctx->launches++;
+    CK(ctx, cudaGetLastError());
+    return FABGPU_OK;
+}
+
+// Waits for `st` and takes the table's counts; a failed upsert (no free slot) is an error
+static int sv_finish(fabgpu_ctx* ctx, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    CK(ctx, cudaMemcpyAsync(s.h_count.get(), s.d_count.get(), 32, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    for (int k = 0; k < 3; k++) s.count[k] = s.h_count.get()[k];
+    if (*reinterpret_cast<const int*>(s.h_count.get() + 3)) { ctx->last_error = "state version table: no free slot"; return FABGPU_E_CUDA; }
+    return FABGPU_OK;
+}
+
+// FABGPU_OK, or the error text of a failed CUDA call that may have left the table half changed (the caller then breaks it, sv_fail)
+static int sv_cuda(fabgpu_ctx* ctx, cudaError_t e, const char* what)
+{
+    if (e == cudaSuccess) return FABGPU_OK;
+    ctx->last_error = std::string(what) + " failed: " + cudaGetErrorString(e);
+    return FABGPU_E_CUDA;
+}
+
+// A failed call may have lost versions: every VALID transaction is 254 and nothing is applied until a replacing call succeeds
+static int sv_fail(fabgpu_ctx* ctx, int rc, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    const std::string err = ctx->last_error;
+    s.broken = true;
+    if (st) cudaStreamSynchronize(st);
+    if (s.table) cudaFree(s.table);
+    s.table = nullptr; s.slots = 0; s.count[0] = s.count[1] = s.count[2] = 0;
+    ctx->last_error = err + " (the state version table is broken until fabgpu_state_versions replaces it)";
+    return rc;
+}
+
+int fabgpu_state_versions(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                          const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::vector<bdev::StateSlot> recs;
+    if (const char* err = stateset::prepare(ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, ctx->sv.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    int rc = drain_block_streams(ctx);                         // the stage of a slot's block may still be running: let it finish
+    if (!rc) rc = sv_begin(ctx);
+    if (rc) return s.installed ? sv_fail(ctx, rc, nullptr) : rc;
+    cudaStream_t st = s.stream.get();
+    if (s.table) cudaFreeAsync(s.table, st);
+    s.table = nullptr; s.slots = 0; s.count[0] = s.count[1] = s.count[2] = 0;
+    s.installed = s.broken = s.open = false; s.height = 0;
+    if (n == 0 && capacity_hint == 0) { CK(ctx, cudaStreamSynchronize(st)); return FABGPU_OK; }
+    s.installed = true; s.height = height;
+    uint64_t hint_slots = stateset::slots_for(capacity_hint);
+    if (hint_slots * sizeof(bdev::StateSlot) > sv_max_bytes()) hint_slots = 0;
+    if ((rc = sv_cuda(ctx, cudaMemsetAsync(s.d_count.get(), 0, 32, st), "state version count clear")) ||
+        (rc = sv_reserve(ctx, recs.size(), hint_slots, st)) || (rc = sv_insert(ctx, recs, st)) || (rc = sv_finish(ctx, st)))
+        return sv_fail(ctx, rc, st);
+    return FABGPU_OK;
+}
+
+int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                                 const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::vector<bdev::StateSlot> recs;
+    if (const char* err = stateset::prepare(ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, ctx->sv.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    if (!s.installed) { ctx->last_error = "no state version table installed: call fabgpu_state_versions first"; return FABGPU_E_ARG; }
+    if (s.broken) { ctx->last_error = "the state version table is broken by a failed call: replace it with fabgpu_state_versions"; return FABGPU_E_ARG; }
+    if (height < s.height) { ctx->last_error = "state version height below the table's height"; return FABGPU_E_ARG; }
+    int rc = sv_begin(ctx);
+    if (rc) return rc;
+    cudaStream_t st = s.stream.get();
+    if ((rc = sv_reserve(ctx, recs.size(), 0, st)) || (rc = sv_insert(ctx, recs, st)) || (rc = sv_finish(ctx, st))) return sv_fail(ctx, rc, st);
+    if (height > s.height) { s.height = height; s.open = false; }
+    return FABGPU_OK;
+}
+
+int fabgpu_state_versions_info(const fabgpu_ctx* cctx, unsigned long long out[4])
+{
+    if (!cctx || !out) return FABGPU_E_ARG;
+    fabgpu_ctx* ctx = const_cast<fabgpu_ctx*>(cctx);          // takes slot0_mu; changes nothing
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    const bool on = s.installed && !s.broken;
+    out[0] = on ? s.count[0] : 0; out[1] = s.slots; out[2] = s.height; out[3] = on ? s.count[2] : 0;
+    return FABGPU_OK;
+}
+
+// The MVCC stage of the slot's block, on the slot's stream after its last kernel:
+//   mv_scan_kernel (per transaction: read / write records with key digests) -> host reads the record count (grows the arrays and runs
+//   the scan again on overflow) -> mv_key_kernel (per record: the block's key table, the committed table's answer) -> mv_check_kernel
+//   -> mv_mark_kernel (per transaction: flags of the independent ones) -> mv_walk_kernel (one thread: the dependent ones in order)
+//   -> growth of the table for the block's keys -> mv_apply_kernel (per key: its final state at (block_num, tx)) -> D2H flags.
+int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* tv_flags, uint8_t* flags, size_t n)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    if (n && (!tv_flags || !flags)) { ctx->last_error = "flag arrays missing"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv; auto& db = ctx->dbs[slot];
+    if (!s.installed) { ctx->last_error = "no state version table installed: call fabgpu_state_versions first"; return FABGPU_E_ARG; }
+    if (s.open) { ctx->last_error = "the previous block is open: fabgpu_state_versions_update(..., height = block_num + 1) first"; return FABGPU_E_ARG; }
+    if (block_num != s.height) { ctx->last_error = "block_num is not the table's height"; return FABGPU_E_ARG; }
+    if (db.busy || !db.mvcc_ready) { ctx->last_error = "the slot holds no finished block: fabgpu_validate_wait first"; return FABGPU_E_ARG; }
+    if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
+    if (s.broken) {                                            // nothing can be decided or applied
+        for (size_t t = 0; t < n; t++) flags[t] = tv_flags[t] == bdev::TXC_VALID ? bdev::TXC_NOT_VALIDATED : tv_flags[t];
+        return FABGPU_OK;
+    }
+    int rc = sv_begin(ctx);
+    if (rc) return rc;
+    const uint32_t T = (uint32_t)n;
+    if (T == 0) { db.mvcc_ready = false; s.height = block_num + 1; return FABGPU_OK; }
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    Grow grow{ctx};
+    grow(s.d_first, 4 * (size_t)T); grow(s.d_n, 4 * (size_t)T); grow(s.d_mlist, 4 * (size_t)T); grow(s.d_info, T); grow(s.d_tv, T); grow(s.d_flags, T);
+    grow(s.h_flags, T);
+    if (grow.rc) return grow.rc;
+    memcpy(s.h_flags.get(), tv_flags, n);
+    CK(ctx, cudaMemcpyAsync(s.d_tv.get(), s.h_flags.get(), n, cudaMemcpyHostToDevice, st));
+    bdev::MvccArrays a;
+    uint32_t R = 0;
+    for (;;) {
+        const size_t R_cap = (size_t)T * s.rec_hint;
+        if (R_cap > UINT32_MAX) { ctx->last_error = "block has too many read and write records"; return FABGPU_E_ARG; }
+        if (R_cap * sizeof(bdev::MvccRec) > s.d_rec.bytes())
+            if (int r2 = s.d_rec.reserve(ctx, R_cap * sizeof(bdev::MvccRec))) return r2;
+        uint32_t* hc = s.h_ctr.get();
+        hc[0] = 0; hc[1] = 0; hc[2] = UINT32_MAX; hc[3] = 0;
+        CK(ctx, cudaMemcpyAsync(s.d_ctr.get(), hc, 16, cudaMemcpyHostToDevice, st));
+        a.rec = s.d_rec.get(); a.R_cap = (uint32_t)R_cap; a.first_rec = s.d_first.get(); a.n_rec = s.d_n.get(); a.info = s.d_info.get();
+        a.key = nullptr; a.K_size = 0; a.ctr = s.d_ctr.get(); a.mlist = s.d_mlist.get();
+        bdev::mv_scan_kernel<<<(T + 63) / 64, 64, 0, st>>>(ctx->bbs[slot].d_block.get(), db.d_txs.get(), T, s.d_tv.get(), a);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(hc, s.d_ctr.get(), 16, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        R = hc[0];
+        if (R <= R_cap) break;
+        s.rec_hint = (uint32_t)((R + T - 1) / T) + 1;            // later blocks are sized for it too
+    }
+    uint32_t K = 64;
+    while (K < 2 * (uint64_t)R) K <<= 1;
+    if ((size_t)K * sizeof(bdev::MvccKey) > s.d_key.bytes())
+        if (int r2 = s.d_key.reserve(ctx, (size_t)K * sizeof(bdev::MvccKey))) return r2;
+    a.key = s.d_key.get(); a.K_size = K;
+    CK(ctx, cudaMemsetAsync(a.key, 0, (size_t)K * sizeof(bdev::MvccKey), st));
+    if (R) {
+        bdev::mv_key_kernel<<<(R + 255) / 256, 256, 0, st>>>(a, sv_dev(ctx), R);
+        bdev::mv_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(a, R);
+        ctx->launches += 2;
+    }
+    bdev::mv_mark_kernel<<<(T + 127) / 128, 128, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T);
+    bdev::mv_walk_kernel<<<1, 256, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T);
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    if ((rc = sv_reserve(ctx, R, 0, st))) return sv_fail(ctx, rc, st);
+    bdev::mv_apply_kernel<<<(K + 255) / 256, 256, 0, st>>>(a, s.d_flags.get(), sv_dev(ctx), (unsigned long long)block_num,
+                                                          reinterpret_cast<int*>(s.d_count.get() + 3));
+    ctx->launches++;
+    // from the apply on the table is changed: a failure leaves it broken
+    if ((rc = sv_cuda(ctx, cudaGetLastError(), "mv_apply_kernel launch")) ||
+        (rc = sv_cuda(ctx, cudaMemcpyAsync(s.h_flags.get(), s.d_flags.get(), n, cudaMemcpyDeviceToHost, st), "MVCC flag copy")) ||
+        (rc = sv_cuda(ctx, cudaMemcpyAsync(s.h_ctr.get(), s.d_ctr.get(), 16, cudaMemcpyDeviceToHost, st), "MVCC counter copy")) ||
+        (rc = sv_finish(ctx, st)))
+        return sv_fail(ctx, rc, st);
+    memcpy(flags, s.h_flags.get(), n);
+    const uint32_t* hc = s.h_ctr.get();
+    db.mvcc_ready = false;
+    if (hc[1] || hc[2] != UINT32_MAX) s.open = true;           // two keys shared a tag, or a write set could not be enumerated
+    else s.height = block_num + 1;
+    return FABGPU_OK;
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -2445,6 +2718,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     auto& db = ctx->dbs[slot];
     if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
+    db.mvcc_ready = false;
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
     int rc;
     {
@@ -2470,7 +2744,7 @@ int fabgpu_validate_envelopes_async(fabgpu_ctx* ctx, int slot, const uint8_t* bl
         std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
         auto& db = ctx->dbs[slot];
         if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-        db.T = 0; db.on_device = false; db.busy = true;
+        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false;
         return FABGPU_OK;
     }
     return validate_submit(ctx, slot, blob, env_off[n_env], env_off, n_env);
@@ -2489,8 +2763,9 @@ int fabgpu_validate_wait(fabgpu_ctx* ctx, int slot, uint8_t* flags, size_t flags
         ctx->last_error = "flags buffer too small";
         return FABGPU_E_ARG;
     }
-    if (db.on_device) return block_finish(ctx, slot, flags);
-    return FABGPU_OK;                                         // an empty envelope list: nothing ran
+    const int rc = db.on_device ? block_finish(ctx, slot, flags) : FABGPU_OK;      // (an empty envelope list: nothing ran)
+    db.mvcc_ready = rc == FABGPU_OK;
+    return rc;
 }
 
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out)

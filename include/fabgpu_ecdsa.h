@@ -358,6 +358,42 @@ int fabgpu_namespace_versions(fabgpu_ctx* ctx, const uint8_t* ver_blob, const ui
 int fabgpu_committed_txids(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n, size_t capacity_hint);
 int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n);
 int fabgpu_committed_txids_info(const fabgpu_ctx* ctx, unsigned long long out[2]);
+/* The ledger's MVCC check (core/ledger/kvledger/txmgmt/validation/validator.go:82-281), an opt-in stage after the validator, over a
+ * device-resident table of the world state's committed key versions with LevelDB semantics (CouchDB's key and value checks are not
+ * restated).  Entry i of a call is (namespace, collection, key) -> (ver[2i], ver[2i+1]) = (block_num, tx_num): three blobs with n + 1
+ * offsets each; the collection is empty for a public key, and for a private-data key the key is its 32-byte key hash.
+ *   fabgpu_state_versions replaces the table; `height` is the ledger height (committed blocks), so the next block to check is block
+ *       `height`.  capacity_hint (keys) sizes the table up front.  n = 0 with capacity_hint = 0 removes it.  It drains the block slots.
+ *   fabgpu_state_versions_update upserts entries; a version of (UINT64_MAX, UINT64_MAX) removes the key.  height must be >= the table's;
+ *       a larger one closes a block the device left open.
+ *   fabgpu_state_versions_info: out[0] = keys held (present or unknown), out[1] = table slots, out[2] = height, out[3] = keys unknown;
+ *       keys and unknown keys are 0 while broken or removed.
+ *   fabgpu_validate_mvcc checks block `block_num` (= the table's height) held by `slot` after fabgpu_validate_wait returned it and before
+ *       the slot's next submit.  tv_flags are the validator's n flags (the device's own, or with some 254s settled by the CPU validator);
+ *       flags receives the committed ones: a VALID transaction becomes VALID, MVCC_READ_CONFLICT (11) or 254, every other flag is copied.
+ *       254 is given to a transaction with a range query (phantom reads are not checked), one that reads a key an undetermined earlier
+ *       transaction of the block writes or that the table marks unknown, one after a transaction whose write set cannot be enumerated,
+ *       and one whose applyWriteSet would put a nil value, where the reference panics: a write without a value, or the metadata path
+ *       (tx_ops.go adds the operations' flags per key, so two writes or two deletes of one key also take it) on a key an earlier
+ *       transaction of the block deleted or an undetermined one wrote.
+ *       Then the block is applied at (block_num, tx index): the writes of every transaction left VALID; the keys written by a
+ *       transaction left at 254 become unknown, and a later read of an unknown key is 254 until _update gives it a version or removes
+ *       it.  When some VALID or 254 transaction's write set cannot be enumerated (no ChaincodeAction.results reached, a non-endorser
+ *       transaction) the block stays open: the height does not advance, and the next call is refused until
+ *       _update(..., height = block_num + 1) supplies those writes.  Otherwise the height becomes block_num + 1.
+ *   FABGPU_E_ARG, with a fabgpu_last_error text and nothing changed, for no table installed, block_num other than the height, an open
+ *   block, a slot without a finished block, n other than the block's transaction count, NULL arrays with n > 0, decreasing offsets, and
+ *   a key given twice in one call.
+ *   Memory: 56 bytes per slot, a power-of-two slot count at a load of at most 1/2 (at least 1024 slots).  FABGPU_STATE_MAX_BYTES
+ *   (environment) bounds the table; when growing or inserting fails the call returns an error and the table is broken: every VALID
+ *   transaction is 254 and nothing is applied, until a fabgpu_state_versions call succeeds.  fabgpu_msp_configure keeps the table.
+ *   The table lives on device 0; blocks in flight on other slots never read it. */
+int fabgpu_state_versions(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                          const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint);
+int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                                 const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height);
+int fabgpu_state_versions_info(const fabgpu_ctx* ctx, unsigned long long out[4]);
+int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* tv_flags, uint8_t* flags, size_t n);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
