@@ -33,6 +33,7 @@ EXPORTS = [
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
+    "fabgpu_state_versions_indexed", "fabgpu_state_index_info",
 ]
 
 
@@ -494,6 +495,17 @@ class Context:
         committed blocks, the next block validate_mvcc checks.  capacity sizes the table for that many keys.  No entries and capacity 0
         remove the table."""
         self._state_versions(lib().fabgpu_state_versions, entries, height, (ctypes.c_size_t(capacity),))
+
+    def state_versions_indexed(self, entries, height, capacity=0):
+        """state_versions, and an ordered index of the public keys (fabgpu_state_versions_indexed): while it is installed validate_mvcc
+        decides range queries (phantom reads) instead of giving them 254.  state_versions drops the index."""
+        self._state_versions(lib().fabgpu_state_versions_indexed, entries, height, (ctypes.c_size_t(capacity),))
+
+    def state_index_info(self):
+        """(index entries the table holds, entries including dead ones, index bytes on the device); zeros without an index"""
+        out = (ctypes.c_ulonglong * 3)()
+        self._ck(lib().fabgpu_state_index_info(self._h, out))
+        return tuple(int(x) for x in out)
 
     def state_versions_update(self, entries, height):
         """Upserts entries (fabgpu_state_versions_update); a version of STATE_REMOVE removes the key.  A height above the table's

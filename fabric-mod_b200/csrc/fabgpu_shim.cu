@@ -293,6 +293,14 @@ struct fabgpu_ctx {
         DevArray<bdev::MvccRec> d_rec; DevArray<uint32_t> d_first, d_n, d_mlist, d_ctr; DevArray<uint8_t> d_info, d_tv, d_flags;
         DevArray<bdev::MvccKey> d_key; HostArray<uint8_t> h_flags; HostArray<uint32_t> h_ctr;
         uint32_t rec_hint = 8;                                                           // records per transaction the arrays are sized for
+        // the ordered index of the public keys (fabgpu_state_versions_indexed, stateindex.cuh): base and delta runs, the delta's next
+        // form, a maintenance step's new run and flags, the key bytes; icnt as StateIndexDev documents, h_icnt its copy after each call
+        bool indexed = false;
+        DevArray<bdev::IndexEntry> ix_base, ix_delta, ix_delta2, ix_fresh; DevArray<uint8_t> ix_heap; DevArray<uint32_t> ix_flag;
+        DevArray<unsigned long long> d_icnt; HostArray<unsigned long long> h_icnt; unsigned long long icnt[5] = {0, 0, 0, 0, 0};
+        DevArray<bdev::MvccRange> d_rng; DevArray<bdev::MerkleState> d_mk; DevArray<uint32_t> d_first_rng, d_n_rng; DevArray<bdev::WrittenKey> d_wk, d_wk2, d_cand;
+        DevArray<uint8_t> d_cand_bytes;
+        uint32_t rng_hint = 1;                                                           // range records per transaction
         ~StateSet() { if (table) cudaFree(table); }
     } sv;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
@@ -2222,8 +2230,10 @@ static int sv_begin(fabgpu_ctx* ctx)
         CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); s.stream.reset(st);
         if (int rc = s.d_count.reserve(ctx, 32)) return rc;
         if (int rc = s.h_count.reserve(ctx, 32)) return rc;
-        if (int rc = s.d_ctr.reserve(ctx, 16)) return rc;
-        if (int rc = s.h_ctr.reserve(ctx, 16)) return rc;
+        if (int rc = s.d_ctr.reserve(ctx, 32)) return rc;
+        if (int rc = s.h_ctr.reserve(ctx, 32)) return rc;
+        if (int rc = s.d_icnt.reserve(ctx, 64)) return rc;
+        if (int rc = s.h_icnt.reserve(ctx, 64)) return rc;
     }
     return FABGPU_OK;
 }
@@ -2232,6 +2242,28 @@ static uint64_t sv_max_bytes()
 {
     const char* v = getenv("FABGPU_STATE_MAX_BYTES");     // bound on the table's bytes; unset = whatever cudaMalloc grants
     return v && *v ? strtoull(v, nullptr, 10) : ~0ull;
+}
+
+// Bytes the index holds on the device (they count toward FABGPU_STATE_MAX_BYTES with the table's)
+static uint64_t ix_bytes(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->sv;
+    return s.ix_base.bytes() + s.ix_delta.bytes() + s.ix_delta2.bytes() + s.ix_fresh.bytes() + s.ix_heap.bytes() + s.ix_flag.bytes();
+}
+
+static void ix_drop(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->sv;
+    s.indexed = false;
+    s.ix_base = {}; s.ix_delta = {}; s.ix_delta2 = {}; s.ix_fresh = {}; s.ix_heap = {}; s.ix_flag = {};
+    for (auto& c : s.icnt) c = 0;
+}
+
+static bdev::StateIndexDev ix_dev(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->sv;
+    bdev::StateIndexDev d{s.ix_base.get(), s.ix_delta.get(), s.ix_heap.get(), s.icnt[0], s.icnt[1], s.indexed ? 1u : 0u};
+    return d;
 }
 
 static bdev::StateSetDev sv_dev(fabgpu_ctx* ctx)
@@ -2249,7 +2281,7 @@ static int sv_reserve(fabgpu_ctx* ctx, uint64_t more, uint64_t min_slots, cudaSt
     if (s.table && s.slots >= min_slots && s.count[1] + more <= s.slots / 2) return FABGPU_OK;
     const uint64_t want = std::max(stateset::slots_for(s.count[0] + more, s.slots), min_slots);
     const uint64_t bytes = want * sizeof(bdev::StateSlot);
-    if (bytes > sv_max_bytes() || want > (1ull << 32)) {
+    if (bytes + ix_bytes(ctx) > sv_max_bytes() || want > (1ull << 32)) {
         char buf[192];
         snprintf(buf, sizeof buf, "state version table of %llu slots (%llu bytes) exceeds FABGPU_STATE_MAX_BYTES", (unsigned long long)want,
                  (unsigned long long)bytes);
@@ -2321,12 +2353,115 @@ static int sv_fail(fabgpu_ctx* ctx, int rc, cudaStream_t st)
     if (st) cudaStreamSynchronize(st);
     if (s.table) cudaFree(s.table);
     s.table = nullptr; s.slots = 0; s.count[0] = s.count[1] = s.count[2] = 0;
+    ix_drop(ctx);
     ctx->last_error = err + " (the state version table is broken until fabgpu_state_versions replaces it)";
     return rc;
 }
 
-int fabgpu_state_versions(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
-                          const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint)
+// Makes room in the index for a step adding at most `n_new` entries with at most `bytes_new` key bytes: the new run, its flags, the delta's
+// next form (the merge writes it, then it becomes the delta), and the heap (grown with its contents kept)
+static int ix_room(fabgpu_ctx* ctx, uint64_t n_new, uint64_t bytes_new, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    const uint64_t E = sizeof(bdev::IndexEntry);
+    const uint64_t want_fresh = std::max<uint64_t>(n_new, 1) * E, want_delta = (s.icnt[1] + std::max<uint64_t>(n_new, 1)) * E;
+    const uint64_t want_heap = s.icnt[3] + bytes_new;
+    uint64_t grow = 0;
+    if (want_fresh > s.ix_fresh.bytes()) grow += 2 * want_fresh - s.ix_fresh.bytes();
+    if (want_fresh / E * 4 > s.ix_flag.bytes()) grow += 2 * (want_fresh / E * 4);
+    if (want_delta > s.ix_delta2.bytes()) grow += 2 * want_delta - s.ix_delta2.bytes();
+    if (want_heap > s.ix_heap.bytes()) grow += 2 * want_heap;
+    if (s.slots * sizeof(bdev::StateSlot) + ix_bytes(ctx) + grow > sv_max_bytes()) {
+        ctx->last_error = "state key index exceeds FABGPU_STATE_MAX_BYTES";
+        return FABGPU_E_CUDA;
+    }
+    Grow g{ctx};
+    if (want_fresh > s.ix_fresh.bytes()) g(s.ix_fresh, 2 * want_fresh);
+    if (want_fresh / E * 4 > s.ix_flag.bytes()) g(s.ix_flag, 2 * (want_fresh / E * 4));
+    if (want_delta > s.ix_delta2.bytes()) g(s.ix_delta2, 2 * want_delta);
+    if (g.rc) return g.rc;
+    if (want_heap > s.ix_heap.bytes()) {
+        DevArray<uint8_t> h;
+        if (int rc = h.reserve(ctx, std::max<uint64_t>(2 * want_heap, 4096))) return rc;
+        if (s.icnt[3]) CK(ctx, cudaMemcpyAsync(h.get(), s.ix_heap.get(), s.icnt[3], cudaMemcpyDeviceToDevice, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        std::swap(h, s.ix_heap);
+    }
+    return FABGPU_OK;
+}
+
+// Adds to the index the candidates (sorted, at most n_ub of them, n_p: their device count, or n) that the table now holds and the
+// index lacks: flags, the new run, its merge with the delta.  Room already made.  The counts are settled by ix_finish.
+static int ix_insert(fabgpu_ctx* ctx, const bdev::WrittenKey* cand, uint32_t n, const uint32_t* n_p, uint64_t n_ub, const uint8_t* src, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    if (!n_ub) return FABGPU_OK;
+    const unsigned g1 = (unsigned)((n_ub + 255) / 256);
+    bdev::ix_flag_kernel<<<g1, 256, 0, st>>>(cand, n, n_p, src, ix_dev(ctx), sv_dev(ctx), s.ix_flag.get());
+    bdev::ix_compact_kernel<<<1, 1024, 0, st>>>(cand, n, n_p, src, s.ix_flag.get(), s.ix_heap.get(), s.ix_fresh.get(), s.d_icnt.get());
+    bdev::ix_merge_kernel<<<(unsigned)((s.icnt[1] + n_ub + 255) / 256), 256, 0, st>>>(s.ix_delta.get(), s.d_icnt.get() + 1, s.ix_fresh.get(),
+                                                                                     s.d_icnt.get() + 2, s.ix_heap.get(), s.ix_delta2.get());
+    bdev::ix_fin_kernel<<<1, 1, 0, st>>>(s.d_icnt.get(), 0);
+    ctx->launches += 4;
+    CK(ctx, cudaGetLastError());
+    std::swap(s.ix_delta, s.ix_delta2);
+    return FABGPU_OK;
+}
+
+// Waits for `st`, takes the index's counts, and folds the delta into the base once it passes stateset::index_fold_at
+static int ix_finish(fabgpu_ctx* ctx, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    CK(ctx, cudaMemcpyAsync(s.h_icnt.get(), s.d_icnt.get(), 40, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    for (int k = 0; k < 5; k++) s.icnt[k] = s.h_icnt.get()[k];
+    if (s.icnt[1] <= stateset::index_fold_at(s.icnt[0])) return FABGPU_OK;
+    const uint64_t n = s.icnt[0] + s.icnt[1], E = sizeof(bdev::IndexEntry);
+    if (s.slots * sizeof(bdev::StateSlot) + ix_bytes(ctx) + n * E > sv_max_bytes()) {
+        ctx->last_error = "state key index exceeds FABGPU_STATE_MAX_BYTES";
+        return FABGPU_E_CUDA;
+    }
+    DevArray<bdev::IndexEntry> nb;
+    if (int rc = nb.reserve(ctx, n * E)) return rc;
+    bdev::ix_merge_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.ix_base.get(), s.d_icnt.get(), s.ix_delta.get(), s.d_icnt.get() + 1,
+                                                                      s.ix_heap.get(), nb.get());
+    bdev::ix_fin_kernel<<<1, 1, 0, st>>>(s.d_icnt.get(), 1);
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaStreamSynchronize(st));
+    std::swap(nb, s.ix_base);
+    s.icnt[0] = n; s.icnt[1] = 0;
+    return FABGPU_OK;
+}
+
+// Installs the index over the call's public keys (sorted on the host), on `st`
+static int ix_install(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint32_t* coll_off, const uint8_t* key_blob,
+                      const uint32_t* key_off, const uint64_t* ver, size_t n, const std::vector<bdev::StateSlot>& recs, cudaStream_t st)
+{
+    auto& s = ctx->sv;
+    std::vector<bdev::WrittenKey> keys; std::vector<uint8_t> blob;
+    stateset::index_keys(ns_blob, ns_off, coll_off, key_blob, key_off, ver, n, recs, keys, blob);
+    std::vector<bdev::IndexEntry> ent(keys.size());
+    for (size_t i = 0; i < keys.size(); i++) {
+        ent[i].off = keys[i].ns_off; ent[i].nl = keys[i].nl; ent[i].kl = keys[i].kl;
+        for (int k = 0; k < 8; k++) ent[i].w[k] = keys[i].w[k];
+    }
+    const uint64_t E = sizeof(bdev::IndexEntry), eb = std::max<uint64_t>(ent.size(), 1) * E, hb = std::max<uint64_t>(blob.size(), 4096);
+    if (s.slots * sizeof(bdev::StateSlot) + eb + hb > sv_max_bytes()) { ctx->last_error = "state key index exceeds FABGPU_STATE_MAX_BYTES"; return FABGPU_E_CUDA; }
+    Grow g{ctx};
+    g(s.ix_base, eb); g(s.ix_heap, hb);
+    if (g.rc) return g.rc;
+    if (!ent.empty()) CK(ctx, cudaMemcpyAsync(s.ix_base.get(), ent.data(), ent.size() * E, cudaMemcpyHostToDevice, st));
+    if (!blob.empty()) CK(ctx, cudaMemcpyAsync(s.ix_heap.get(), blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+    unsigned long long* hc = s.h_icnt.get();
+    hc[0] = ent.size(); hc[1] = 0; hc[2] = 0; hc[3] = blob.size(); hc[4] = 0;
+    CK(ctx, cudaMemcpyAsync(s.d_icnt.get(), hc, 40, cudaMemcpyHostToDevice, st));
+    s.indexed = true;
+    return ix_finish(ctx, st);
+}
+
+static int sv_replace(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                      const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint, bool indexed)
 {
     if (!ctx) return FABGPU_E_ARG;
     std::vector<bdev::StateSlot> recs;
@@ -2340,14 +2475,28 @@ int fabgpu_state_versions(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_
     if (s.table) cudaFreeAsync(s.table, st);
     s.table = nullptr; s.slots = 0; s.count[0] = s.count[1] = s.count[2] = 0;
     s.installed = s.broken = s.open = false; s.height = 0;
+    if (s.indexed) { CK(ctx, cudaStreamSynchronize(st)); ix_drop(ctx); }
     if (n == 0 && capacity_hint == 0) { CK(ctx, cudaStreamSynchronize(st)); return FABGPU_OK; }
     s.installed = true; s.height = height;
     uint64_t hint_slots = stateset::slots_for(capacity_hint);
     if (hint_slots * sizeof(bdev::StateSlot) > sv_max_bytes()) hint_slots = 0;
     if ((rc = sv_cuda(ctx, cudaMemsetAsync(s.d_count.get(), 0, 32, st), "state version count clear")) ||
-        (rc = sv_reserve(ctx, recs.size(), hint_slots, st)) || (rc = sv_insert(ctx, recs, st)) || (rc = sv_finish(ctx, st)))
+        (rc = sv_reserve(ctx, recs.size(), hint_slots, st)) || (rc = sv_insert(ctx, recs, st)) || (rc = sv_finish(ctx, st)) ||
+        (indexed && (rc = ix_install(ctx, ns_blob, ns_off, coll_off, key_blob, key_off, ver, n, recs, st))))
         return sv_fail(ctx, rc, st);
     return FABGPU_OK;
+}
+
+int fabgpu_state_versions(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                          const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint)
+{
+    return sv_replace(ctx, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, height, capacity_hint, false);
+}
+
+int fabgpu_state_versions_indexed(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                                  const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint)
+{
+    return sv_replace(ctx, ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, height, capacity_hint, true);
 }
 
 int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
@@ -2365,7 +2514,44 @@ int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const 
     if (rc) return rc;
     cudaStream_t st = s.stream.get();
     if ((rc = sv_reserve(ctx, recs.size(), 0, st)) || (rc = sv_insert(ctx, recs, st)) || (rc = sv_finish(ctx, st))) return sv_fail(ctx, rc, st);
+    if (s.indexed) {                                           // the index gains the public keys it lacks
+        std::vector<bdev::WrittenKey> keys; std::vector<uint8_t> blob;
+        stateset::index_keys(ns_blob, ns_off, coll_off, key_blob, key_off, ver, n, recs, keys, blob);
+        if (!keys.empty()) {
+            Grow g{ctx};
+            g(s.d_cand, keys.size() * sizeof(bdev::WrittenKey)); g(s.d_cand_bytes, std::max<size_t>(blob.size(), 1));
+            if (g.rc) return sv_fail(ctx, g.rc, st);
+            if ((rc = sv_cuda(ctx, cudaMemcpyAsync(s.d_cand.get(), keys.data(), keys.size() * sizeof(bdev::WrittenKey), cudaMemcpyHostToDevice, st), "index copy")) ||
+                (!blob.empty() && (rc = sv_cuda(ctx, cudaMemcpyAsync(s.d_cand_bytes.get(), blob.data(), blob.size(), cudaMemcpyHostToDevice, st), "index copy"))) ||
+                (rc = ix_room(ctx, keys.size(), blob.size(), st)) ||
+                (rc = ix_insert(ctx, s.d_cand.get(), (uint32_t)keys.size(), nullptr, keys.size(), s.d_cand_bytes.get(), st)) || (rc = ix_finish(ctx, st)))
+                return sv_fail(ctx, rc, st);
+        }
+    }
     if (height > s.height) { s.height = height; s.open = false; }
+    return FABGPU_OK;
+}
+
+int fabgpu_state_index_info(const fabgpu_ctx* cctx, unsigned long long out[3])
+{
+    if (!cctx || !out) return FABGPU_E_ARG;
+    fabgpu_ctx* ctx = const_cast<fabgpu_ctx*>(cctx);          // takes slot0_mu; changes nothing the stage reads
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    out[0] = out[1] = out[2] = 0;
+    if (!s.indexed || !s.installed || s.broken) return FABGPU_OK;
+    if (int rc = sv_begin(ctx)) return rc;
+    cudaStream_t st = s.stream.get();
+    const uint64_t n = s.icnt[0] + s.icnt[1];
+    CK(ctx, cudaMemsetAsync(s.d_icnt.get() + 4, 0, 8, st));
+    if (n) {
+        bdev::ix_live_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ix_dev(ctx), sv_dev(ctx), s.d_icnt.get());
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+    }
+    CK(ctx, cudaMemcpyAsync(s.h_icnt.get(), s.d_icnt.get(), 40, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    out[0] = s.h_icnt.get()[4]; out[1] = n; out[2] = ix_bytes(ctx);
     return FABGPU_OK;
 }
 
@@ -2385,6 +2571,9 @@ int fabgpu_state_versions_info(const fabgpu_ctx* cctx, unsigned long long out[4]
 //   the scan again on overflow) -> mv_key_kernel (per record: the block's key table, the committed table's answer) -> mv_check_kernel
 //   -> mv_mark_kernel (per transaction: flags of the independent ones) -> mv_walk_kernel (one thread: the dependent ones in order)
 //   -> growth of the table for the block's keys -> mv_apply_kernel (per key: its final state at (block_num, tx)) -> D2H flags.
+// With an index installed the scan also emits range records, and before mv_mark_kernel: mv_written_kernel (the block's written public
+// keys) -> mv_sort_kernel (one launch per merge pass) -> mv_range_kernel (per range record: marking and the committed answer); after the
+// apply the index gains the block's new keys (ix_insert), and the delta is folded into the base when due (ix_finish).
 int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* tv_flags, uint8_t* flags, size_t n)
 {
     if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -2412,27 +2601,41 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     if (grow.rc) return grow.rc;
     memcpy(s.h_flags.get(), tv_flags, n);
     CK(ctx, cudaMemcpyAsync(s.d_tv.get(), s.h_flags.get(), n, cudaMemcpyHostToDevice, st));
+    const bool ix = s.indexed;
+    if (ix) {
+        grow(s.d_first_rng, 4 * (size_t)T); grow(s.d_n_rng, 4 * (size_t)T);
+        if (grow.rc) return grow.rc;
+    }
+    const uint8_t* blk = ctx->bbs[slot].d_block.get();
     bdev::MvccArrays a;
-    uint32_t R = 0;
+    uint32_t R = 0, G = 0;
     for (;;) {
-        const size_t R_cap = (size_t)T * s.rec_hint;
-        if (R_cap > UINT32_MAX) { ctx->last_error = "block has too many read and write records"; return FABGPU_E_ARG; }
+        const size_t R_cap = (size_t)T * s.rec_hint, G_cap = ix ? (size_t)T * s.rng_hint : 0;
+        if (R_cap > UINT32_MAX || G_cap > UINT32_MAX) { ctx->last_error = "block has too many read and write records"; return FABGPU_E_ARG; }
         if (R_cap * sizeof(bdev::MvccRec) > s.d_rec.bytes())
             if (int r2 = s.d_rec.reserve(ctx, R_cap * sizeof(bdev::MvccRec))) return r2;
+        if (G_cap * sizeof(bdev::MvccRange) > s.d_rng.bytes())
+            if (int r2 = s.d_rng.reserve(ctx, G_cap * sizeof(bdev::MvccRange))) return r2;
         uint32_t* hc = s.h_ctr.get();
-        hc[0] = 0; hc[1] = 0; hc[2] = UINT32_MAX; hc[3] = 0;
-        CK(ctx, cudaMemcpyAsync(s.d_ctr.get(), hc, 16, cudaMemcpyHostToDevice, st));
+        hc[0] = 0; hc[1] = 0; hc[2] = UINT32_MAX; hc[3] = 0; hc[4] = 0; hc[5] = 0; hc[6] = 0; hc[7] = 0;
+        CK(ctx, cudaMemcpyAsync(s.d_ctr.get(), hc, 32, cudaMemcpyHostToDevice, st));
         a.rec = s.d_rec.get(); a.R_cap = (uint32_t)R_cap; a.first_rec = s.d_first.get(); a.n_rec = s.d_n.get(); a.info = s.d_info.get();
         a.key = nullptr; a.K_size = 0; a.ctr = s.d_ctr.get(); a.mlist = s.d_mlist.get();
-        bdev::mv_scan_kernel<<<(T + 63) / 64, 64, 0, st>>>(ctx->bbs[slot].d_block.get(), db.d_txs.get(), T, s.d_tv.get(), a);
+        if (ix) {
+            a.indexed = 1; a.block = block_num; a.rng = s.d_rng.get(); a.G_cap = (uint32_t)G_cap; a.first_rng = s.d_first_rng.get();
+            a.n_rng = s.d_n_rng.get(); a.ix = ix_dev(ctx);
+        }
+        bdev::mv_scan_kernel<<<(T + 63) / 64, 64, 0, st>>>(blk, db.d_txs.get(), T, s.d_tv.get(), a);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
-        CK(ctx, cudaMemcpyAsync(hc, s.d_ctr.get(), 16, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaMemcpyAsync(hc, s.d_ctr.get(), 32, cudaMemcpyDeviceToHost, st));
         CK(ctx, cudaStreamSynchronize(st));
-        R = hc[0];
-        if (R <= R_cap) break;
-        s.rec_hint = (uint32_t)((R + T - 1) / T) + 1;            // later blocks are sized for it too
+        R = hc[0]; G = hc[4];
+        if (R <= R_cap && G <= G_cap) break;
+        if (R > R_cap) s.rec_hint = (uint32_t)((R + T - 1) / T) + 1;            // later blocks are sized for it too
+        if (G > G_cap) s.rng_hint = (uint32_t)((G + T - 1) / T) + 1;
     }
+    const uint64_t key_bytes = s.h_ctr.get()[6];
     uint32_t K = 64;
     while (K < 2 * (uint64_t)R) K <<= 1;
     if ((size_t)K * sizeof(bdev::MvccKey) > s.d_key.bytes())
@@ -2444,19 +2647,44 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
         bdev::mv_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(a, R);
         ctx->launches += 2;
     }
+    if (ix && (R || G)) {                                      // the block's written public keys, sorted (at most R of them)
+        Grow g2{ctx};
+        g2(s.d_wk, (size_t)std::max(R, 1u) * sizeof(bdev::WrittenKey)); g2(s.d_wk2, (size_t)std::max(R, 1u) * sizeof(bdev::WrittenKey));
+        if (g2.rc) return g2.rc;
+        a.wk = s.d_wk.get();
+        bdev::mv_written_kernel<<<(K + 255) / 256, 256, 0, st>>>(a);
+        ctx->launches++;
+        bdev::WrittenKey* in = s.d_wk.get(); bdev::WrittenKey* out = s.d_wk2.get();
+        for (uint32_t width = 1; width < R; width <<= 1) {
+            bdev::mv_sort_kernel<<<(R + 255) / 256, 256, 0, st>>>(in, out, a.ctr, width, blk);
+            ctx->launches++;
+            std::swap(in, out);
+        }
+        a.wk = in;
+        if (G) {
+            if ((size_t)G * sizeof(bdev::MerkleState) > s.d_mk.bytes())
+                if (int r2 = s.d_mk.reserve(ctx, (size_t)G * sizeof(bdev::MerkleState))) return r2;
+            a.mk = s.d_mk.get();
+            bdev::mv_range_kernel<<<(G + 127) / 128, 128, 0, st>>>(blk, a, sv_dev(ctx), G);
+            ctx->launches++;
+        }
+    }
     bdev::mv_mark_kernel<<<(T + 127) / 128, 128, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T);
-    bdev::mv_walk_kernel<<<1, 256, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T);
+    if (ix) bdev::mv_walk_kernel<true><<<1, 256, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T, blk, sv_dev(ctx));
+    else bdev::mv_walk_kernel<false><<<1, 256, 0, st>>>(s.d_tv.get(), a, s.d_flags.get(), T, blk, sv_dev(ctx));
     ctx->launches += 2;
     CK(ctx, cudaGetLastError());
     if ((rc = sv_reserve(ctx, R, 0, st))) return sv_fail(ctx, rc, st);
+    if (ix && R && (rc = ix_room(ctx, R, key_bytes, st))) return sv_fail(ctx, rc, st);
     bdev::mv_apply_kernel<<<(K + 255) / 256, 256, 0, st>>>(a, s.d_flags.get(), sv_dev(ctx), (unsigned long long)block_num,
                                                           reinterpret_cast<int*>(s.d_count.get() + 3));
     ctx->launches++;
     // from the apply on the table is changed: a failure leaves it broken
+    if (ix && R && (rc = ix_insert(ctx, a.wk, 0, a.ctr + 5, R, blk, st))) return sv_fail(ctx, rc, st);
     if ((rc = sv_cuda(ctx, cudaGetLastError(), "mv_apply_kernel launch")) ||
         (rc = sv_cuda(ctx, cudaMemcpyAsync(s.h_flags.get(), s.d_flags.get(), n, cudaMemcpyDeviceToHost, st), "MVCC flag copy")) ||
         (rc = sv_cuda(ctx, cudaMemcpyAsync(s.h_ctr.get(), s.d_ctr.get(), 16, cudaMemcpyDeviceToHost, st), "MVCC counter copy")) ||
-        (rc = sv_finish(ctx, st)))
+        (rc = sv_finish(ctx, st)) || (ix && R && (rc = ix_finish(ctx, st))))
         return sv_fail(ctx, rc, st);
     memcpy(flags, s.h_flags.get(), n);
     const uint32_t* hc = s.h_ctr.get();

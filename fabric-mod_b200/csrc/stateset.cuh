@@ -7,6 +7,9 @@
 // public key; for a private key the key is its 32-byte hash).  The table is open addressing over 56-byte slots (digest, state, version)
 // at a load of at most 1/2; the first probe is txid_mix of the digest with the context's seed, since key bytes are chosen by submitters.
 // A removed key keeps its slot as SV_REMOVED (probes continue past it; an upsert of the same key takes it back).
+//
+// Range queries (RangeQueryInfo) are decided only while an ordered index of the public keys is installed (stateindex.cuh,
+// fabgpu_state_versions_indexed); without one a VALID transaction with a range query is 254 (MV_RANGE).
 #pragma once
 #include "blockdev.cuh"
 #if defined(__CUDACC__)
@@ -167,6 +170,12 @@ BD_HD uint32_t sv_lookup(const StateSetDev& t, const uint32_t w[8], unsigned lon
     return SV_EMPTY;
 }
 
+} }  // namespace fabgpu::bdev
+
+#include "stateindex.cuh"
+
+namespace fabgpu { namespace bdev {
+
 // ---- the MVCC stage over one block -----------------------------------------------------------------------------------------------
 // record kinds: a read (public or hashed), a write, a deleting write, a metadata write with entries (metadataUpdate) and one without
 // (metadataDelete); MvccRec::has_ver is a read's Version, a write's value (or value hash)
@@ -174,7 +183,7 @@ enum : uint8_t { MR_READ = 0, MR_PUT = 1, MR_DEL = 2, MR_META = 3, MR_MDEL = 4 }
 // MvccRec::c -- reads: the committed comparison; writes: the key's committed existence
 enum : uint8_t { MC_OK = 0, MC_FAIL = 1, MC_UNDET = 2, MC_ABSENT = 0, MC_EXISTS = 1 };
 // per-transaction info bits
-#define MV_RANGE 1u                // a RangeQueryInfo: phantom reads are not checked here
+#define MV_RANGE 1u                // a RangeQueryInfo while no index is installed: phantom reads are not checked
 #define MV_OPEN 2u                 // its write set cannot be enumerated (no ChaincodeAction.results, a non-endorser transaction, no parse)
 #define MV_MARKED 4u               // touches a key that another transaction of the block writes first: the sequential walk decides it
 // the walk's running state of a key in `updates` (validator.go:176-193)
@@ -184,7 +193,22 @@ struct MvccRec {
     uint32_t w[8];
     uint32_t tx, key;              // transaction; entry of the block's key table
     unsigned long long blk, txn;   // a read's version
-    uint8_t kind, has_ver, c, pad;
+    uint8_t kind, has_ver, c, pub; // pub: a key of a KVRWSet (not a hashed one)
+    Seg ns, k;                     // the namespace and key bytes in the block
+};
+
+// One RangeQueryInfo of a VALID transaction (while an index is installed).  form: RF_NONE neither raw_reads nor reads_merkle_hashes
+// (no reads), RF_RAW raw_reads (body: QueryReads), RF_MERKLE reads_merkle_hashes (body: QueryReadsMerkleSummary), RF_BAD a wire form
+// not decided here.  lo, hi: the in-range slice of the block's sorted written public keys; endk: the end key's entry of the block's key
+// table + 1 (0: the block does not write it).  c: the answer against the committed state alone; marked: an earlier transaction of the
+// block writes a key of the range (or its end key, when served), so the walk decides it.  ib, id: the range's first positions in the
+// index's base and delta, found once before the walk.
+enum : uint8_t { RF_NONE = 0, RF_RAW = 1, RF_MERKLE = 2, RF_BAD = 3 };
+struct MvccRange {
+    uint32_t tx; Seg ns, start, end, body;
+    uint32_t lo, hi, endk, degree, level;
+    uint8_t exhausted, form, c, marked;
+    unsigned long long ib, id;
 };
 
 // One entry per distinct key the block reads or writes.  tag: txid_mix of the digest (0 = empty), claimed by CAS; w written by the claimer.
@@ -194,14 +218,22 @@ struct MvccKey {
     uint32_t nfirst, nw, lastr;         // UINT32_MAX - earliest writer (0 none: the table starts zeroed), write records, latest reader + 1 (0 none)
     uint32_t wrec;                      // some write record (the only one when nw == 1)
     uint32_t rs, rs_tx, op_tx, op;      // the walk: running state, its writer, and the combined operation of transaction op_tx - 1
+    uint32_t rng;                       // a later transaction's range covers the key after one of its writers: the walk tracks it
 };
 
 struct MvccArrays {
     MvccRec* rec; uint32_t R_cap;
     uint32_t* first_rec; uint32_t* n_rec; uint8_t* info;   // per transaction
     MvccKey* key; uint32_t K_size;                         // power of two >= 2 R
-    uint32_t* ctr;                 // [0] records handed out (> R_cap: overflow), [1] alias, [2] first open transaction (UINT32_MAX none), [3] marked
+    uint32_t* ctr;                 // [0] records handed out (> R_cap: overflow), [1] alias, [2] first open transaction (UINT32_MAX none), [3] marked,
+                                   // [4] range records handed out (> G_cap: overflow), [5] written public keys, [6] their bytes (an upper bound)
     uint32_t* mlist;               // the marked transactions in index order
+    // range queries, while an index is installed (indexed = 1); without one these members are not read
+    uint32_t indexed = 0; unsigned long long block = 0;
+    MvccRange* rng = nullptr; uint32_t G_cap = 0; uint32_t* first_rng = nullptr; uint32_t* n_rng = nullptr;   // per transaction
+    WrittenKey* wk = nullptr;                                                 // the block's written public keys, sorted (ctr[5] of them)
+    MerkleState* mk = nullptr;                                                // per range record: its Merkle state (global scratch)
+    StateIndexDev ix = {nullptr, nullptr, nullptr, 0, 0, 0};
 };
 
 BD_HD uint32_t mv_atomic_min(uint32_t* p, uint32_t v)
@@ -239,20 +271,19 @@ BD_HD bool mv_reached(const TxDev& tx)
 }
 
 // Every read, hashed read and write of a TxReadWriteSet, through kl_scan_rwset's parser with its reads enabled.
-// on_rec(ns, coll, key, kind, has_ver, blk, txn); *range = a RangeQueryInfo is present.  false when a level does not parse.
-template <typename F>
-BD_HD bool mv_scan(const uint8_t* base, Seg results, bool* range, F on_rec)
+// on_rec(ns, coll, key, kind, has_ver, blk, txn, pub); on_range(ns, RangeQueryInfo).  false when a level does not parse.
+template <typename F, typename G>
+BD_HD bool mv_scan(const uint8_t* base, Seg results, F on_rec, G on_range)
 {
-    *range = false;
     return kl_scan_rwset<true>(base, results, [&](Seg ns, Seg coll, Seg key, uint32_t g, Seg body) {
         // g: the field of the record in its set -- KVRWSet 1 read, 2 range query, 3 write, 4 metadata write;
         // HashedRWSet 11 hashed read, 12 hashed write, 13 hashed metadata write (kl_scan_rwset adds 10)
-        if (g == 2) { *range = true; return true; }
+        if (g == 2) { on_range(ns, body); return true; }
         if (g == 1 || g == 11) {
             // KVRead{key = 1, version = 2}, KVReadHash{key_hash = 1, version = 2}: an absent version is nil, an empty one (0, 0)
             bool has = false; unsigned long long blk = 0, txn = 0; bool ok = true;
             if (!scan_msg(base, body, BD_F(1) | BD_F(2), 0, [&](uint32_t h, Seg v) { if (h == 2) { has = true; ok = ok && mv_version(base, v, blk, txn); } }) || !ok) return false;
-            on_rec(ns, coll, key, (uint8_t)MR_READ, has, blk, txn);
+            on_rec(ns, coll, key, (uint8_t)MR_READ, has, blk, txn, g < 10);
             return true;
         }
         // KVWrite{key = 1, is_delete = 2, value = 3}, KVWriteHash{key_hash = 1, is_delete = 2, value_hash = 3, is_purge = 4};
@@ -266,34 +297,89 @@ BD_HD bool mv_scan(const uint8_t* base, Seg results, bool* range, F on_rec)
             if (!md && f == 2 && wt == 0) del = x != 0;
             if (f == (md ? 2u : 3u)) has = true;
         }
-        on_rec(ns, coll, key, (uint8_t)(md ? (has ? MR_META : MR_MDEL) : del ? MR_DEL : MR_PUT), has, 0ull, 0ull);
+        on_rec(ns, coll, key, (uint8_t)(md ? (has ? MR_META : MR_MDEL) : del ? MR_DEL : MR_PUT), has, 0ull, 0ull, g < 10);
         return true;
     });
 }
 
-// Stage 1, one thread per transaction: the records of a transaction tv_flags leaves VALID or 254, with their key digests
+// RangeQueryInfo{start_key = 1, end_key = 2, itr_exhausted = 3, oneof {raw_reads = 4, reads_merkle_hashes = 5}} (kv_rwset.proto, as
+// recalled: the file is not in the reference tree); QueryReads{kv_reads = 1}; QueryReadsMerkleSummary{max_degree = 1, max_level = 2,
+// max_level_hashes = 3}.  A scalar or string field given twice: the last wins, as proto.Unmarshal does.  RF_BAD: the message or its reads
+// do not parse, both oneof fields are present, a oneof field is repeated, or max_degree / max_level does not fit 32 bits -- shapes whose
+// decoding this stage does not restate.
+BD_HD void mv_range_parse(const uint8_t* base, Seg info, MvccRange& g)
+{
+    g.start.off = g.start.len = g.end.off = g.end.len = g.body.off = g.body.len = 0;
+    g.exhausted = 0; g.form = RF_NONE; g.degree = g.level = 0;
+    Reader r; r.base = base; r.pos = info.off; r.end = info.off + info.len; r.ok = true;
+    uint32_t f, wt, n4 = 0, n5 = 0; uint64_t x = 0; Seg b; b.off = b.len = 0;
+    while (r.next(f, wt, x, b)) {
+        if (f == 3) { if (wt != 0) { g.form = RF_BAD; return; } g.exhausted = x != 0; }
+        else if (f == 1 || f == 2 || f == 4 || f == 5) {
+            if (wt != 2) { g.form = RF_BAD; return; }
+            if (f == 1) g.start = b; else if (f == 2) g.end = b; else { g.body = b; (f == 4 ? n4 : n5)++; }
+        }
+    }
+    if (!r.ok || n4 + n5 > 1) { g.form = RF_BAD; return; }
+    if (n4) {
+        g.form = RF_RAW;
+        bool ok = true;
+        if (!scan_msg(base, g.body, BD_F(1), 0, [&](uint32_t, Seg kv) {
+                unsigned long long blk = 0, txn = 0;
+                if (!scan_msg(base, kv, BD_F(1) | BD_F(2), 0, [&](uint32_t h, Seg v) { if (h == 2) ok = ok && mv_version(base, v, blk, txn); })) ok = false;
+            }) || !ok) g.form = RF_BAD;
+    } else if (n5) {
+        g.form = RF_MERKLE;
+        Reader m; m.base = base; m.pos = g.body.off; m.end = g.body.off + g.body.len; m.ok = true;
+        while (m.next(f, wt, x, b)) {
+            if (f == 1 || f == 2) { if (wt != 0 || x > 0xffffffffull) { g.form = RF_BAD; return; } if (f == 1) g.degree = (uint32_t)x; else g.level = (uint32_t)x; }
+            else if (f == 3 && wt != 2) { g.form = RF_BAD; return; }
+        }
+        if (!m.ok) g.form = RF_BAD;
+    }
+}
+
+// Stage 1, one thread per transaction: the records of a transaction tv_flags leaves VALID or 254, with their key digests, and (index
+// installed) the range records of a VALID one
 BD_HD void mv_scan_tx(const uint8_t* base, const TxDev& tx, uint32_t t, uint8_t tv, MvccArrays& a)
 {
     a.first_rec[t] = 0; a.n_rec[t] = 0; a.info[t] = 0;
+    if (a.indexed) { a.first_rng[t] = 0; a.n_rng[t] = 0; }
     if (tv != TXC_VALID && tv != TXC_NOT_VALIDATED) return;
-    bool range = false;
-    uint32_t n = 0;
-    if (!mv_reached(tx) || !mv_scan(base, tx.results, &range, [&](Seg, Seg, Seg, uint8_t, bool, unsigned long long, unsigned long long) { n++; })) {
+    uint32_t n = 0, n_range = 0;
+    if (!mv_reached(tx) || !mv_scan(base, tx.results, [&](Seg, Seg, Seg, uint8_t, bool, unsigned long long, unsigned long long, bool) { n++; },
+                                    [&](Seg, Seg) { n_range++; })) {
         a.info[t] = MV_OPEN;
         mv_atomic_min(a.ctr + 2, t);                                   // later VALID transactions may read its writes
         return;
     }
-    a.info[t] = range ? MV_RANGE : 0;
+    const bool ranges = a.indexed && tv == TXC_VALID;
+    a.info[t] = n_range && !a.indexed ? MV_RANGE : 0;
+    if (ranges && n_range) {
+        const uint32_t b = kl_atomic_add(a.ctr + 4, n_range);
+        if (b + n_range <= a.G_cap && b + n_range >= b) {
+            a.first_rng[t] = b; a.n_rng[t] = n_range;
+            uint32_t q = b;
+            mv_scan(base, tx.results, [&](Seg, Seg, Seg, uint8_t, bool, unsigned long long, unsigned long long, bool) {}, [&](Seg ns, Seg info) {
+                MvccRange& g = a.rng[q++];
+                g.tx = t; g.ns = ns; g.lo = g.hi = g.endk = 0; g.c = MC_OK; g.marked = 0; g.ib = g.id = 0;
+                mv_range_parse(base, info, g);
+            });
+        }
+    }
     if (n == 0) return;
     const uint32_t b = kl_atomic_add(a.ctr, n);
     if (b + n > a.R_cap || b + n < b) return;                        // overflow: the host grows the arrays and runs the stage again
     a.first_rec[t] = b; a.n_rec[t] = n;
-    uint32_t q = b;
-    mv_scan(base, tx.results, &range, [&](Seg ns, Seg coll, Seg key, uint8_t kind, bool has, unsigned long long blk, unsigned long long txn) {
+    uint32_t q = b, bytes = 0;
+    mv_scan(base, tx.results, [&](Seg ns, Seg coll, Seg key, uint8_t kind, bool has, unsigned long long blk, unsigned long long txn, bool pub) {
         MvccRec& r = a.rec[q++];
         sv_key(base + ns.off, ns.len, base + coll.off, coll.len, base + key.off, key.len, r.w);
-        r.tx = t; r.key = 0; r.blk = blk; r.txn = txn; r.kind = kind; r.has_ver = has ? 1 : 0; r.c = 0; r.pad = 0;
-    });
+        r.tx = t; r.key = 0; r.blk = blk; r.txn = txn; r.kind = kind; r.has_ver = has ? 1 : 0; r.c = 0; r.pub = pub ? 1 : 0;
+        r.ns = ns; r.k = key;
+        if (pub && kind != MR_READ) bytes += ns.len + key.len;
+    }, [&](Seg, Seg) {});
+    if (a.indexed && bytes) kl_atomic_add(a.ctr + 6, bytes);
 }
 
 // Stage 2, one thread per record: its entry in the block's key table, and the committed table's answer
@@ -347,7 +433,192 @@ BD_HD uint32_t mv_first(const MvccKey& e) { return UINT32_MAX - e.nfirst; }
 // Some transaction's outcome depends on another's write of the key: two write records, or a read after the first write
 BD_HD bool mv_contended(const MvccKey& e)
 {
-    return e.nw >= 2 || (e.nw >= 1 && e.lastr > mv_first(e) + 1);
+    return e.nw >= 2 || (e.nw >= 1 && e.lastr > mv_first(e) + 1) || (e.nw >= 1 && e.rng);
+}
+
+// ---- range queries (index installed) --------------------------------------------------------------------------------------------
+// The entry of the block's key table holding digest w, or UINT32_MAX
+BD_HD uint32_t mv_find_key(const MvccArrays& a, uint64_t seed, const uint32_t w[8])
+{
+    unsigned long long tag = txid_mix(w, seed ^ 0x9e3779b97f4a7c15ull);
+    if (tag == 0) tag = 1;
+    uint32_t pos = (uint32_t)tag & (a.K_size - 1);
+    for (uint32_t probe = 0; probe < a.K_size; probe++, pos = (pos + 1) & (a.K_size - 1)) {
+        const MvccKey& e = a.key[pos];
+        if (e.tag == 0) return UINT32_MAX;
+        if (e.tag == tag && txid_equal(e.w, w)) return pos;
+    }
+    return UINT32_MAX;
+}
+
+// One thread per entry of the block's key table: a public key some record writes joins the list the range records search (unsorted)
+BD_HD void mv_written_key(uint32_t k, MvccArrays& a)
+{
+    const MvccKey& e = a.key[k];
+    if (!e.tag || !e.nw) return;
+    const MvccRec& r = a.rec[e.wrec];
+    if (!r.pub) return;
+    WrittenKey& o = a.wk[kl_atomic_add(a.ctr + 5, 1)];
+    o.ns_off = r.ns.off; o.nl = r.ns.len; o.key_off = r.k.off; o.kl = r.k.len; o.k = k;
+    for (int j = 0; j < 8; j++) o.w[j] = e.w[j];
+}
+
+// The combined iterator (combined_iterator.go) of one range over the committed state and -- in the walk -- `updates`, the running state
+// of the block's keys that earlier VALID or 254 transactions wrote.  Candidates come in key order from the index (base and delta merged)
+// and from the block's in-range written keys; where both hold a key the block's state wins.  A committed candidate the table does not
+// hold is skipped (a dead index entry); a deleted key is skipped.  When itr_exhausted is false the end key is served once, after
+// everything else: from the block's state, else from the table, not at all when absent or deleted.
+struct RangeIt {
+    const uint8_t* base; const MvccRange* g; const StateSetDev* set; const StateIndexDev* ix; const MvccArrays* a;
+    bool use_block; uint64_t ib, id; uint32_t j; bool end_served;
+};
+
+BD_HD void rq_begin(RangeIt& it, const uint8_t* base, const MvccRange& g, const StateSetDev& set, const MvccArrays& a, bool use_block)
+{
+    it.base = base; it.g = &g; it.set = &set; it.ix = &a.ix; it.a = &a; it.use_block = use_block; it.end_served = false; it.j = g.lo;
+    it.ib = g.ib; it.id = g.id;
+}
+
+BD_HD int rq_state(uint32_t rs, uint32_t rs_tx, unsigned long long block, unsigned long long& blk, unsigned long long& txn)
+{
+    if (rs == RS_PUT) { blk = block; txn = rs_tx; return 1; }
+    return rs == RS_DEL ? 0 : 2;
+}
+
+// The next result: 1 (key bytes, version), 0 none left, 2 a candidate whose state is unknown (the answer is 254)
+BD_HD int rq_next(RangeIt& it, const uint8_t*& key, uint32_t& kl, unsigned long long& blk, unsigned long long& txn)
+{
+    const MvccRange& g = *it.g; const StateIndexDev& x = *it.ix; const MvccArrays& a = *it.a;
+    const KeyRef bound = key_ref(it.base + g.ns.off, g.ns.len, it.base + g.end.off, g.end.len);
+    if (it.set->broken) return 2;
+    for (;;) {
+        const bool hb = it.ib < x.nb && ri_below_end(key_ref(x.heap, x.base[it.ib]), bound);
+        const bool hd = it.id < x.nd && ri_below_end(key_ref(x.heap, x.delta[it.id]), bound);
+        const IndexEntry* c = nullptr; bool from_base = false;
+        if (hb && (!hd || key_cmp(key_ref(x.heap, x.base[it.ib]), key_ref(x.heap, x.delta[it.id])) < 0)) { c = x.base + it.ib; from_base = true; }
+        else if (hd) c = x.delta + it.id;
+        while (it.use_block && it.j < g.hi && a.key[a.wk[it.j].k].rs == RS_NONE) it.j++;
+        const WrittenKey* u = it.use_block && it.j < g.hi ? a.wk + it.j : nullptr;
+        if (!c && !u) break;
+        const int cmp = !c ? 1 : !u ? -1 : key_cmp(key_ref(x.heap, *c), key_ref(it.base, *u));
+        if (cmp <= 0) { if (from_base) it.ib++; else it.id++; }
+        if (cmp >= 0) it.j++;
+        if (cmp < 0) {
+            const uint32_t st = sv_lookup(*it.set, c->w, blk, txn);
+            if (st == SV_EMPTY) continue;
+            if (st == SV_UNKNOWN) return 2;
+            key = x.heap + c->off + c->nl; kl = c->kl;
+            return 1;
+        }
+        const MvccKey& e = a.key[u->k];
+        const int r = rq_state(e.rs, e.rs_tx, a.block, blk, txn);
+        if (r == 0) continue;
+        key = it.base + u->key_off; kl = u->kl;
+        return r;
+    }
+    if (g.exhausted || it.end_served) return 0;
+    it.end_served = true;
+    key = it.base + g.end.off; kl = g.end.len;
+    if (it.use_block && g.endk && a.key[g.endk - 1].rs != RS_NONE) {
+        const MvccKey& e = a.key[g.endk - 1];
+        return rq_state(e.rs, e.rs_tx, a.block, blk, txn);
+    }
+    uint32_t w[8];
+    sv_key(it.base + g.ns.off, g.ns.len, nullptr, 0, it.base + g.end.off, g.end.len, w);
+    const uint32_t st = sv_lookup(*it.set, w, blk, txn);
+    return st == SV_PRESENT ? 1 : st == SV_UNKNOWN ? 2 : 0;
+}
+
+// validateRangeQuery (validator.go:216-237) over the iterator: MC_OK, MC_FAIL or MC_UNDET.  Results are drawn as the reference's
+// validators draw them, so a candidate of unknown state past the point where the answer is settled is never reached.
+// Raw reads (rangeQueryResultsValidator): the results must equal the recorded KVReads, key and version, with none left over.  A read
+// without a Version that is reached with a result of its key is 254: convertToVersionHeight dereferences the nil Version and the
+// reference panics (a read with a mismatching key returns false first).
+// Merkle summary (rangeQueryHashValidator): the loop's early exits are restated after every result (mk_early) -- false, or 254 where the
+// reference indexes MaxLevelHashes out of range and panics -- and at the end the summary Done() builds is compared with the recorded
+// one.  The state lives in global scratch `m`, not on the thread's stack.
+BD_HD uint8_t rq_eval(const uint8_t* base, const MvccRange& g, const StateSetDev& set, const MvccArrays& a, bool use_block, MerkleState* m)
+{
+    if (g.form == RF_BAD || (g.form == RF_MERKLE && g.degree < 2)) return MC_UNDET;   // newMerkleTree fails: the reference fails the commit
+    RangeIt it;
+    rq_begin(it, base, g, set, a, use_block);
+    const uint8_t* key = nullptr; uint32_t kl = 0; unsigned long long blk = 0, txn = 0;
+    if (g.form == RF_MERKLE) {
+        mk_init(*m, base, g.body, g.degree, g.level);
+        for (;;) {
+            const int r = rq_next(it, key, kl, blk, txn);
+            if (r == 2) return MC_UNDET;
+            if (r == 0) break;
+            mk_add(*m, key, kl, blk, txn);
+            if (m->overflow) return MC_UNDET;
+            const int e = mk_early(*m);
+            if (e) return e == 1 ? MC_FAIL : MC_UNDET;
+        }
+        const int d = mk_done(*m, g.degree);
+        return d < 0 ? MC_UNDET : d ? MC_OK : MC_FAIL;
+    }
+    int r = rq_next(it, key, kl, blk, txn);
+    if (r == 2) return MC_UNDET;
+    bool fail = false, panic = false;
+    if (g.form == RF_RAW)
+        scan_msg(base, g.body, BD_F(1), 0, [&](uint32_t, Seg kv) {
+            if (fail || panic || r == 2) return;
+            Seg rk; rk.off = rk.len = 0; unsigned long long rb = 0, rt = 0; bool hv = false;
+            scan_msg(base, kv, BD_F(1) | BD_F(2), 0, [&](uint32_t h, Seg v) { if (h == 1) rk = v; else { hv = true; mv_version(base, v, rb, rt); } });
+            if (r == 0 || bytes_cmp(key, kl, base + rk.off, rk.len) != 0) { fail = true; return; }
+            if (!hv) { panic = true; return; }
+            if (blk != rb || txn != rt) { fail = true; return; }
+            r = rq_next(it, key, kl, blk, txn);
+        });
+    if (panic) return MC_UNDET;
+    if (fail) return MC_FAIL;
+    if (r == 2) return MC_UNDET;
+    return r == 0 ? MC_OK : MC_FAIL;
+}
+
+// One thread per range record, before the walk: its slice of the block's sorted written public keys, whether an earlier transaction
+// writes in it (those keys, and a written end key that will be served, count as contended from here on), and its answer against the
+// committed state alone.
+BD_HD void mv_range_rec(uint32_t q, const uint8_t* base, MvccArrays& a, const StateSetDev& set)
+{
+    MvccRange& g = a.rng[q];
+    if (g.form == RF_BAD || (g.form == RF_MERKLE && g.degree < 2)) { g.c = MC_UNDET; return; }
+    const uint32_t W = a.ctr[5];
+    const KeyRef s = key_ref(base + g.ns.off, g.ns.len, base + g.start.off, g.start.len);
+    const KeyRef bound = key_ref(base + g.ns.off, g.ns.len, base + g.end.off, g.end.len);
+    g.lo = (uint32_t)ri_lower(a.wk, 0, W, base, s);
+    uint32_t lo = g.lo, hi = W;                                       // the first key past the range: ri_below_end turns false once
+    while (lo < hi) { const uint32_t mid = lo + (hi - lo) / 2; if (ri_below_end(key_ref(base, a.wk[mid]), bound)) lo = mid + 1; else hi = mid; }
+    g.hi = lo;
+    bool marked = false;
+    for (uint32_t j = g.lo; j < g.hi; j++) {
+        MvccKey& e = a.key[a.wk[j].k];
+        if (mv_first(e) < g.tx) { marked = true; e.rng = 1; }
+    }
+    if (!g.exhausted) {
+        uint32_t w[8];
+        sv_key(base + g.ns.off, g.ns.len, nullptr, 0, base + g.end.off, g.end.len, w);
+        const uint32_t k = mv_find_key(a, set.seed, w);
+        if (k != UINT32_MAX && a.key[k].nw) {
+            g.endk = k + 1;
+            if (mv_first(a.key[k]) < g.tx) { marked = true; a.key[k].rng = 1; }
+        }
+    }
+    g.marked = marked ? 1 : 0;
+    g.ib = ri_lower(a.ix.base, 0, a.ix.nb, a.ix.heap, s);
+    g.id = ri_lower(a.ix.delta, 0, a.ix.nd, a.ix.heap, s);
+    g.c = rq_eval(base, g, set, a, false, a.mk + q);
+}
+
+// In the walk: the answer of a marked range record against the running state; the committed answer stands when no key of the range (nor
+// the end key) has entered `updates` yet
+BD_HD uint8_t mv_range_walk(const uint8_t* base, uint32_t q, const StateSetDev& set, const MvccArrays& a)
+{
+    const MvccRange& g = a.rng[q];
+    if (!g.marked) return g.c;                                     // (a form not decoded is never marked)
+    bool moved = g.endk && a.key[g.endk - 1].rs != RS_NONE;
+    for (uint32_t j = g.lo; j < g.hi && !moved; j++) moved = a.key[a.wk[j].k].rs != RS_NONE;
+    return moved ? rq_eval(base, g, set, a, true, a.mk + q) : g.c;
 }
 
 // A write's keyOpsFlag: upsertVal 1, metadataUpdate 2, metadataDelete 4, keyDelete 8 (tx_ops.go:162-169).  prepareTxOps ADDS them per
@@ -384,6 +655,12 @@ BD_HD void mv_mark_tx(uint32_t t, const uint8_t* tv, MvccArrays& a, uint8_t* fla
             nil_put = nil_put || (r.kind == MR_PUT && !r.has_ver);    // one write per key here: PutValAndMetadata of a nil value panics
         }
     }
+    if (a.indexed)
+        for (uint32_t q = a.first_rng[t]; q < a.first_rng[t] + a.n_rng[t]; q++) {
+            const MvccRange& g = a.rng[q];
+            marked = marked || g.marked;
+            fail = fail || g.c == MC_FAIL; undet = undet || g.c == MC_UNDET;
+        }
     if (marked) { a.info[t] |= MV_MARKED; return; }
     if (f != TXC_VALID) return;
     flags[t] = (a.info[t] & (MV_RANGE | MV_OPEN)) || t > a.ctr[2] || undet ? TXC_NOT_VALIDATED : fail ? 11 : nil_put ? TXC_NOT_VALIDATED : TXC_VALID;
@@ -391,7 +668,10 @@ BD_HD void mv_mark_tx(uint32_t t, const uint8_t* tv, MvccArrays& a, uint8_t* fla
 
 // Stage 5, one thread, the marked transactions in index order: a VALID one is decided against the running state of the keys earlier
 // transactions wrote, then the writes of every one left VALID or 254 enter that state.  Costs the transaction's own records.
-BD_HD void mv_walk_step(uint32_t t, const uint8_t* tv, MvccArrays& a, uint8_t* flags)
+// Indexed: the stage decides range records (base, set: the block and the table they read); the plain instantiation is the stage without
+// an index, compiled without the range code
+template <bool Indexed = false>
+BD_HD void mv_walk_step(uint32_t t, const uint8_t* tv, MvccArrays& a, uint8_t* flags, const uint8_t* base = nullptr, const StateSetDev* set = nullptr)
 {
     const uint32_t b = a.first_rec[t], end = b + a.n_rec[t];
     uint8_t f = tv[t];
@@ -420,6 +700,11 @@ BD_HD void mv_walk_step(uint32_t t, const uint8_t* tv, MvccArrays& a, uint8_t* f
                 nil_put = nil_put || (cls == MR_PUT && (e.op & 0x100u)) || (cls == MR_META && (e.rs == RS_DEL || e.rs == RS_UNDET));
             }
         }
+        if constexpr (Indexed)
+            for (uint32_t q = a.first_rng[t]; q < a.first_rng[t] + a.n_rng[t]; q++) {
+                const uint8_t c = mv_range_walk(base, q, *set, a);
+                fail = fail || c == MC_FAIL; undet = undet || c == MC_UNDET;
+            }
         f = (a.info[t] & (MV_RANGE | MV_OPEN)) || t > a.ctr[2] || undet ? TXC_NOT_VALIDATED : fail ? 11 : nil_put ? TXC_NOT_VALIDATED : TXC_VALID;
         flags[t] = f;
     }
@@ -464,6 +749,25 @@ BD_HD void mv_apply_key(uint32_t k, MvccArrays& a, const uint8_t* flags, const S
     }
     if (state == SV_EMPTY) return;
     if (sv_upsert(set, e.w, state, state == SV_PRESENT ? block : 0ull, txn) < 0) *full = 1;
+}
+
+// ---- index maintenance (fabgpu_state_versions_update, and the stage after its apply) -----------------------------------------------
+// One thread per candidate (sorted, keys distinct): flag[i] = 1 for a key the table now holds (present or unknown) that the index lacks,
+// so a later range sees it -- and answers 254 for an unknown one
+BD_HD void ix_flag(uint32_t i, const WrittenKey* c, const uint8_t* src, const StateIndexDev& x, const StateSetDev& set, uint32_t* flag)
+{
+    unsigned long long b = 0, t = 0;
+    const uint32_t st = set.broken ? SV_EMPTY : sv_lookup(set, c[i].w, b, t);
+    flag[i] = (st == SV_PRESENT || st == SV_UNKNOWN) && !ri_contains(x, key_ref(src, c[i])) ? 1u : 0u;
+}
+
+// A flagged candidate becomes entry `out` of the new run, its bytes at heap + at
+BD_HD void ix_emit(const WrittenKey& c, const uint8_t* src, uint8_t* heap, unsigned long long at, IndexEntry& out)
+{
+    for (uint32_t k = 0; k < c.nl; k++) heap[at + k] = src[c.ns_off + k];
+    for (uint32_t k = 0; k < c.kl; k++) heap[at + c.nl + k] = src[c.key_off + k];
+    out.off = at; out.nl = c.nl; out.kl = c.kl;
+    for (int k = 0; k < 8; k++) out.w[k] = c.w[k];
 }
 
 #if defined(__CUDACC__)
@@ -519,10 +823,34 @@ mv_mark_kernel(const uint8_t* __restrict__ tv, MvccArrays a, uint8_t* __restrict
     if (t < T) mv_mark_tx(t, tv, a, flags);
 }
 
-// One CTA: the marked transactions are compacted by a block-wide scan (as in block_kl_resolve_kernel), then one thread walks them in
-// index order
+// Range queries: the block's written public keys (one thread per entry of the key table), their merge sort (one launch per pass, runs of
+// `width`), then one thread per range record
 __global__ void __launch_bounds__(256)
-mv_walk_kernel(const uint8_t* __restrict__ tv, MvccArrays a, uint8_t* __restrict__ flags, uint32_t T)
+mv_written_kernel(MvccArrays a)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < a.K_size && !a.ctr[1] && a.ctr[0] <= a.R_cap) mv_written_key(k, a);
+}
+
+__global__ void __launch_bounds__(256)
+mv_sort_kernel(const WrittenKey* __restrict__ in, WrittenKey* __restrict__ out, const uint32_t* __restrict__ ctr, uint32_t width, const uint8_t* __restrict__ block)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < ctr[5]) ri_sort_one(in, i, ctr[5], width, block, out);
+}
+
+__global__ void __launch_bounds__(128)
+mv_range_kernel(const uint8_t* __restrict__ block, MvccArrays a, StateSetDev set, uint32_t G)
+{
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < G && !a.ctr[1] && a.ctr[0] <= a.R_cap) mv_range_rec(q, block, a, set);
+}
+
+// One CTA: the marked transactions are compacted by a block-wide scan (as in block_kl_resolve_kernel), then one thread walks them in
+// index order.  mv_walk_kernel<false> is the stage without an index; <true> also decides the marked range records.
+template <bool Indexed>
+__global__ void __launch_bounds__(256)
+mv_walk_kernel(const uint8_t* __restrict__ tv, MvccArrays a, uint8_t* __restrict__ flags, uint32_t T, const uint8_t* __restrict__ block, StateSetDev set)
 {
     __shared__ uint32_t warp_sum[32];
     if (a.ctr[1] || a.ctr[0] > a.R_cap) return;
@@ -546,7 +874,7 @@ mv_walk_kernel(const uint8_t* __restrict__ tv, MvccArrays a, uint8_t* __restrict
     __syncthreads();
     if (tid != 0) return;
     a.ctr[3] = total;
-    for (uint32_t k = 0; k < total; k++) mv_walk_step(a.mlist[k], tv, a, flags);
+    for (uint32_t k = 0; k < total; k++) mv_walk_step<Indexed>(a.mlist[k], tv, a, flags, block, &set);
 }
 
 __global__ void __launch_bounds__(256)
@@ -554,6 +882,78 @@ mv_apply_kernel(MvccArrays a, const uint8_t* __restrict__ flags, StateSetDev set
 {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k < a.K_size) mv_apply_key(k, a, flags, set, block, full);
+}
+
+// Index maintenance over n sorted candidates (n_p: a device count instead): flags, then one CTA writes the flagged ones, in order, as the
+// new run (icnt[2] entries) with their bytes appended to the heap (icnt[3]); the run merges with the delta; ix_fin_kernel settles the counts
+__global__ void __launch_bounds__(256)
+ix_flag_kernel(const WrittenKey* __restrict__ c, uint32_t n, const uint32_t* __restrict__ n_p, const uint8_t* __restrict__ src, StateIndexDev x,
+               StateSetDev set, uint32_t* __restrict__ flag)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < (n_p ? *n_p : n)) ix_flag(i, c, src, x, set, flag);
+}
+
+__global__ void __launch_bounds__(1024)
+ix_compact_kernel(const WrittenKey* __restrict__ c, uint32_t n, const uint32_t* __restrict__ n_p, const uint8_t* __restrict__ src,
+                  const uint32_t* __restrict__ flag, uint8_t* __restrict__ heap, IndexEntry* __restrict__ out, unsigned long long* __restrict__ icnt)
+{
+    __shared__ unsigned long long sn[32], sb[32];
+    if (n_p) n = *n_p;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, per = (n + blockDim.x - 1) / blockDim.x;
+    const uint32_t lo = min(n, tid * per), hi = min(n, lo + per);
+    unsigned long long cn = 0, cb = 0;
+    for (uint32_t i = lo; i < hi; i++) if (flag[i]) { cn++; cb += c[i].nl + c[i].kl; }
+    unsigned long long xn = cn, xb = cb;
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const unsigned long long yn = __shfl_up_sync(0xffffffffu, xn, d), yb = __shfl_up_sync(0xffffffffu, xb, d);
+        if (lane >= d) { xn += yn; xb += yb; }
+    }
+    if (lane == 31) { sn[warp] = xn; sb[warp] = xb; }
+    __syncthreads();
+    if (warp == 0) {
+        unsigned long long vn = lane < blockDim.x / 32 ? sn[lane] : 0, vb = lane < blockDim.x / 32 ? sb[lane] : 0;
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const unsigned long long yn = __shfl_up_sync(0xffffffffu, vn, d), yb = __shfl_up_sync(0xffffffffu, vb, d);
+            if (lane >= d) { vn += yn; vb += yb; }
+        }
+        sn[lane] = vn; sb[lane] = vb;
+    }
+    __syncthreads();
+    const unsigned long long h0 = icnt[3];
+    unsigned long long off = xn - cn + (warp ? sn[warp - 1] : 0), at = h0 + xb - cb + (warp ? sb[warp - 1] : 0);
+    for (uint32_t i = lo; i < hi; i++)
+        if (flag[i]) { ix_emit(c[i], src, heap, at, out[off]); off++; at += c[i].nl + c[i].kl; }
+    __syncthreads();
+    if (tid == 0) { icnt[2] = sn[31]; icnt[3] = h0 + sb[31]; }
+}
+
+// out = merge of the sorted runs A (*na entries) and B (*nb), keys disjoint; one thread per entry of either
+__global__ void __launch_bounds__(256)
+ix_merge_kernel(const IndexEntry* __restrict__ A, const unsigned long long* __restrict__ na, const IndexEntry* __restrict__ B,
+                const unsigned long long* __restrict__ nb, const uint8_t* __restrict__ heap, IndexEntry* __restrict__ out)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, n_a = *na, n_b = *nb;
+    if (i < n_a) ri_merge_one(A, i, B, n_b, heap, out, 0);
+    else if (i < n_a + n_b) ri_merge_one(B, i - n_a, A, n_a, heap, out, 0);
+}
+
+// fold = 0: the new run joined the delta; 1: the delta joined the base
+__global__ void ix_fin_kernel(unsigned long long* icnt, int fold)
+{
+    if (fold) { icnt[0] += icnt[1]; icnt[1] = 0; }
+    else { icnt[1] += icnt[2]; icnt[2] = 0; }
+}
+
+// fabgpu_state_index_info: icnt[4] = entries the table holds (present or unknown)
+__global__ void __launch_bounds__(256)
+ix_live_kernel(StateIndexDev x, StateSetDev set, unsigned long long* __restrict__ icnt)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= x.nb + x.nd) return;
+    const IndexEntry& e = i < x.nb ? x.base[i] : x.delta[i - x.nb];
+    unsigned long long b = 0, t = 0;
+    if (!set.broken && sv_lookup(set, e.w, b, t) != SV_EMPTY) atomicAdd(icnt + 4, 1ull);
 }
 #endif
 

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "stateset.cuh"
@@ -42,6 +43,36 @@ inline const char* prepare(const uint8_t* ns_blob, const uint32_t* ns_off, const
             if (bdev::txid_equal(out[index[h]].w, out[i].w)) return "state version key given twice in one call";
         }
     return nullptr;
+}
+
+// The public keys of a call that are not removals (collection empty, version not (UINT64_MAX, UINT64_MAX)), sorted by (namespace, key)
+// bytewise: the index's install form and an update's insertions.  blob holds each key's namespace then key; recs: prepare's output.
+inline void index_keys(const uint8_t* ns_blob, const uint32_t* ns_off, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off,
+                       const uint64_t* ver, size_t n, const std::vector<bdev::StateSlot>& recs, std::vector<bdev::WrittenKey>& out,
+                       std::vector<uint8_t>& blob)
+{
+    out.clear(); blob.clear();
+    for (size_t i = 0; i < n; i++) {
+        if (coll_off[i + 1] != coll_off[i] || (ver[2 * i] == UINT64_MAX && ver[2 * i + 1] == UINT64_MAX)) continue;
+        bdev::WrittenKey c;
+        c.nl = ns_off[i + 1] - ns_off[i]; c.kl = key_off[i + 1] - key_off[i]; c.k = 0;
+        c.ns_off = (uint32_t)blob.size(); c.key_off = c.ns_off + c.nl;
+        blob.insert(blob.end(), ns_blob + ns_off[i], ns_blob + ns_off[i + 1]);
+        blob.insert(blob.end(), key_blob + key_off[i], key_blob + key_off[i + 1]);
+        for (int k = 0; k < 8; k++) c.w[k] = recs[i].w[k];
+        out.push_back(c);
+    }
+    const uint8_t* b = blob.data();
+    std::sort(out.begin(), out.end(), [b](const bdev::WrittenKey& x, const bdev::WrittenKey& y) {
+        return bdev::key_cmp(bdev::key_ref(b, x), bdev::key_ref(b, y)) < 0;
+    });
+}
+
+// The delta is folded into the base when it holds more than this many entries
+inline uint64_t index_fold_at(uint64_t base)
+{
+    const uint64_t f = std::min<uint64_t>(base / 8, 1u << 18);
+    return std::max<uint64_t>(f, 4096);
 }
 
 // Slots for `keys` claimed slots at a load of at most 1/2: the smallest power of two >= max(2 keys, MIN_SLOTS), at least `have`

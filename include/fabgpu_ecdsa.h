@@ -371,7 +371,7 @@ int fabgpu_committed_txids_info(const fabgpu_ctx* ctx, unsigned long long out[2]
  *   fabgpu_validate_mvcc checks block `block_num` (= the table's height) held by `slot` after fabgpu_validate_wait returned it and before
  *       the slot's next submit.  tv_flags are the validator's n flags (the device's own, or with some 254s settled by the CPU validator);
  *       flags receives the committed ones: a VALID transaction becomes VALID, MVCC_READ_CONFLICT (11) or 254, every other flag is copied.
- *       254 is given to a transaction with a range query (phantom reads are not checked), one that reads a key an undetermined earlier
+ *       254 is given to a transaction with a range query while no index is installed (see fabgpu_state_versions_indexed), one that reads a key an undetermined earlier
  *       transaction of the block writes or that the table marks unknown, one after a transaction whose write set cannot be enumerated,
  *       and one whose applyWriteSet would put a nil value, where the reference panics: a write without a value, or the metadata path
  *       (tx_ops.go adds the operations' flags per key, so two writes or two deletes of one key also take it) on a key an earlier
@@ -394,6 +394,35 @@ int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const 
                                  const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height);
 int fabgpu_state_versions_info(const fabgpu_ctx* ctx, unsigned long long out[4]);
 int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* tv_flags, uint8_t* flags, size_t n);
+/* Range queries (phantom reads) in fabgpu_validate_mvcc, opt-in: an ordered index of the table's public keys (entries with an empty
+ * collection), in bytewise (namespace, key) order, each with its key's digest.  The index only says which keys of a range may exist;
+ * presence and version always come from the table, so a removed key may stay in the index as a dead entry until the next install.
+ *   fabgpu_state_versions_indexed takes fabgpu_state_versions' arguments, replaces the table the same way, and installs the index over
+ *       the call's public keys.  A plain fabgpu_state_versions call drops the index; so does a failure that breaks the table.
+ *   While an index is installed, fabgpu_state_versions_update and fabgpu_validate_mvcc add to it every public key the table comes to hold
+ *       (present, or unknown after a 254 writer) that it lacks; later insertions go to a small sorted delta, folded into the sorted base
+ *       once it passes max(4096, min(base / 8, 2^18)) entries.
+ *   fabgpu_validate_mvcc then gives a VALID transaction with range queries VALID, 11 or 254 by validateRangeQuery (validator.go:216-237,
+ *       LevelDB): the results of [start_key, end_key) -- an empty end_key is the rest of the namespace -- over the committed state and
+ *       the writes of the block's earlier VALID transactions (theirs win; a deleted key is skipped; a metadata write on a present key
+ *       re-puts it at (block, tx)), and, when itr_exhausted is false, the end key served once after everything else (from those writes,
+ *       else from the table, not at all when absent or deleted; also when start_key > end_key or end_key is empty).
+ *       raw_reads (or neither oneof field: no reads) must equal the results exactly, key and version, with none left over.
+ *       reads_merkle_hashes must equal the summary RangeQueryResultsHelper(max_degree).Done() builds over the results; max_degree or
+ *       fewer results give no summary, hence 11.  Results are drawn as the reference's validators draw them, early exits included.
+ *       254 where the reference panics: a raw read without a Version reached with a result of its key, and rangeQueryHashValidator's
+ *       early-exit loop indexing the top level out of range (the top level rising after its first matched hash).
+ *       254 for max_degree < 2 (the reference fails the commit), a result candidate whose state is unknown (the table marks it, or an
+ *       undetermined earlier transaction of the block writes it), and a RangeQueryInfo this stage does not decode: one that does not
+ *       parse, both oneof fields present, a oneof field repeated, a max_degree or max_level beyond 32 bits.
+ *       Without an index every entry point behaves as above, range queries included (254).
+ *   fabgpu_state_index_info: out[0] = index entries the table holds (present or unknown), out[1] = entries including dead ones,
+ *       out[2] = the index's device bytes; all 0 without an index.
+ *   Memory: 48 bytes per entry plus the key bytes, with room for growth; the index counts toward FABGPU_STATE_MAX_BYTES, and a failed
+ *   growth or insert breaks the table (and drops the index) as a failed table growth does. */
+int fabgpu_state_versions_indexed(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
+                                  const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint);
+int fabgpu_state_index_info(const fabgpu_ctx* ctx, unsigned long long out[3]);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
