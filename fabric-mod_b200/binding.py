@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FABGPU_LIB") or os.path.join(_HERE, "lib", "libfabgpu_ecdsa.so")
 SLOTS = 3
 CAP_V2_0, CAP_V1_3 = 0, 1      # fabgpu_channel_capability
+STATEDB_LEVELDB, STATEDB_COUCHDB = 0, 1             # fabgpu_state_database
 STATE_REMOVE = (2 ** 64 - 1, 2 ** 64 - 1)   # fabgpu_state_versions_update: a version that removes the key
 
 OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
@@ -33,7 +34,7 @@ EXPORTS = [
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
-    "fabgpu_state_versions_indexed", "fabgpu_state_index_info",
+    "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
 ]
 
 
@@ -506,6 +507,19 @@ class Context:
         out = (ctypes.c_ulonglong * 3)()
         self._ck(lib().fabgpu_state_index_info(self._h, out))
         return tuple(int(x) for x in out)
+
+    def state_database(self, kind):
+        """The state database validate_mvcc restates (fabgpu_state_database): STATEDB_LEVELDB (the default) or STATEDB_COUCHDB, which
+        adds CouchDB's key and value checks (INVALID_WRITESET, 24) and makes the install calls refuse public keys CouchDB cannot hold."""
+        self._ck(lib().fabgpu_state_database(self._h, ctypes.c_int(kind)))
+
+    def test_couch_values(self, values, path=0):
+        """The device's verdict bits of CouchDB's value check on each of the byte strings (fabgpu_test_couch_values): path 0 chooses
+        the scan by length as validate_mvcc does, 1 forces the one-thread scan, 2 the CTA scan"""
+        b, o = _blob([bytes(v) for v in values])
+        out = np.zeros(max(len(values), 1), np.uint32)
+        self._ck(lib().fabgpu_test_couch_values(self._h, _p(b), _p(o), ctypes.c_size_t(len(values)), ctypes.c_int(path), _p(out)))
+        return out[: len(values)]
 
     def state_versions_update(self, entries, height):
         """Upserts entries (fabgpu_state_versions_update); a version of STATE_REMOVE removes the key.  A height above the table's

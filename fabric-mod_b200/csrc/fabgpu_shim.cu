@@ -29,6 +29,7 @@
 #include "keypolicy.hpp"
 #include "txidset.hpp"
 #include "stateset.hpp"
+#include "couchval.cuh"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -301,6 +302,10 @@ struct fabgpu_ctx {
         DevArray<bdev::MvccRange> d_rng; DevArray<bdev::MerkleState> d_mk; DevArray<uint32_t> d_first_rng, d_n_rng; DevArray<bdev::WrittenKey> d_wk, d_wk2, d_cand;
         DevArray<uint8_t> d_cand_bytes;
         uint32_t rng_hint = 1;                                                           // range records per transaction
+        // the state database the stage restates (fabgpu_state_database); CouchDB adds the key and value pre-pass (couchval.cuh)
+        bool couch = false;
+        DevArray<bdev::CvWrite> d_cvw; DevArray<uint32_t> d_cv_first, d_cv_n; DevArray<uint8_t> d_cv_undet, d_cv_code; DevArray<uint32_t> d_cv_long;
+        uint32_t cv_hint = 4;                                                            // public writes per transaction
         ~StateSet() { if (table) cudaFree(table); }
     } sv;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
@@ -2460,6 +2465,19 @@ static int ix_install(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* n
     return ix_finish(ctx, st);
 }
 
+// CouchDB: every public key the call gives a version is one CouchDB can hold (validateKey); false with the error text otherwise.  A
+// removal passes: the stage marks unknown the keys a 254 transaction writes, such a key among them, and the caller settles it by removal.
+static bool cv_keys_ok(fabgpu_ctx* ctx, const uint32_t* coll_off, const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n)
+{
+    for (size_t i = 0; i < n; i++)
+        if (coll_off[i + 1] == coll_off[i] && !(ver[2 * i] == UINT64_MAX && ver[2 * i + 1] == UINT64_MAX) &&
+            !bdev::cv_key_ok(key_blob + key_off[i], key_off[i + 1] - key_off[i])) {
+            ctx->last_error = "a public key CouchDB cannot hold (empty, starting with '_', or not UTF-8) under FABGPU_STATEDB_COUCHDB";
+            return false;
+        }
+    return true;
+}
+
 static int sv_replace(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
                       const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint, bool indexed)
 {
@@ -2468,6 +2486,7 @@ static int sv_replace(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* n
     if (const char* err = stateset::prepare(ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, ctx->sv.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& s = ctx->sv;
+    if (s.couch && !cv_keys_ok(ctx, coll_off, key_blob, key_off, ver, n)) return FABGPU_E_ARG;
     int rc = drain_block_streams(ctx);                         // the stage of a slot's block may still be running: let it finish
     if (!rc) rc = sv_begin(ctx);
     if (rc) return s.installed ? sv_fail(ctx, rc, nullptr) : rc;
@@ -2509,6 +2528,7 @@ int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const 
     auto& s = ctx->sv;
     if (!s.installed) { ctx->last_error = "no state version table installed: call fabgpu_state_versions first"; return FABGPU_E_ARG; }
     if (s.broken) { ctx->last_error = "the state version table is broken by a failed call: replace it with fabgpu_state_versions"; return FABGPU_E_ARG; }
+    if (s.couch && !cv_keys_ok(ctx, coll_off, key_blob, key_off, ver, n)) return FABGPU_E_ARG;
     if (height < s.height) { ctx->last_error = "state version height below the table's height"; return FABGPU_E_ARG; }
     int rc = sv_begin(ctx);
     if (rc) return rc;
@@ -2566,11 +2586,63 @@ int fabgpu_state_versions_info(const fabgpu_ctx* cctx, unsigned long long out[4]
     return FABGPU_OK;
 }
 
+int fabgpu_state_database(fabgpu_ctx* ctx, int kind)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    if (kind != FABGPU_STATEDB_LEVELDB && kind != FABGPU_STATEDB_COUCHDB) { ctx->last_error = "unknown state database kind"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    ctx->sv.couch = kind == FABGPU_STATEDB_COUCHDB;
+    return FABGPU_OK;
+}
+
+// CouchDB's pre-pass on `st`, before the stage reads d_tv: cv_scan_kernel (per transaction: the public writes of the VALID ones, and
+// the read / range rules) -> host reads the write count (grows the arrays and runs the scan again on overflow) -> cv_check_kernel (per
+// write: key, and a value of at most CV_SHORT_MAX bytes) -> cv_long_kernel (one CTA per longer value) -> cv_flag_kernel (per transaction: VALID -> 24 or 254 in d_tv)
+static int cv_prepass(fabgpu_ctx* ctx, cudaStream_t st, const uint8_t* blk, const bdev::TxDev* txs, uint32_t T)
+{
+    auto& s = ctx->sv;
+    Grow grow{ctx};
+    grow(s.d_cv_first, 4 * (size_t)T); grow(s.d_cv_n, 4 * (size_t)T); grow(s.d_cv_undet, T);
+    if (grow.rc) return grow.rc;
+    bdev::CvArrays c;
+    uint32_t W = 0;
+    for (;;) {
+        const size_t W_cap = (size_t)T * s.cv_hint;
+        if (W_cap > UINT32_MAX) { ctx->last_error = "block has too many writes"; return FABGPU_E_ARG; }
+        Grow g2{ctx};
+        g2(s.d_cvw, W_cap * sizeof(bdev::CvWrite)); g2(s.d_cv_code, W_cap); g2(s.d_cv_long, 4 * W_cap);
+        if (g2.rc) return g2.rc;
+        uint32_t* hc = s.h_ctr.get();
+        hc[0] = hc[1] = 0;
+        CK(ctx, cudaMemcpyAsync(s.d_ctr.get(), hc, 8, cudaMemcpyHostToDevice, st));
+        c.w = s.d_cvw.get(); c.W_cap = (uint32_t)W_cap; c.first_w = s.d_cv_first.get(); c.n_w = s.d_cv_n.get(); c.undet = s.d_cv_undet.get();
+        c.code = s.d_cv_code.get(); c.lng = s.d_cv_long.get(); c.ctr = s.d_ctr.get();
+        bdev::cv_scan_kernel<<<(T + 63) / 64, 64, 0, st>>>(blk, txs, T, s.d_tv.get(), c);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(hc, s.d_ctr.get(), 4, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        W = hc[0];
+        if (W <= W_cap) break;
+        s.cv_hint = (uint32_t)((W + T - 1) / T) + 1;
+    }
+    if (W) {                                                   // the long values: one CTA each, as many as there are (at most 264 CTAs)
+        bdev::cv_check_kernel<<<(W + 127) / 128, 128, 0, st>>>(blk, c, W);
+        bdev::cv_long_kernel<<<std::min(W, 264u), bdev::CV_LT_THREADS, 0, st>>>(blk, c);
+        ctx->launches += 2;
+    }
+    bdev::cv_flag_kernel<<<(T + 127) / 128, 128, 0, st>>>(c, s.d_tv.get(), T);
+    ctx->launches++;
+    CK(ctx, cudaGetLastError());
+    return FABGPU_OK;
+}
+
 // The MVCC stage of the slot's block, on the slot's stream after its last kernel:
 //   mv_scan_kernel (per transaction: read / write records with key digests) -> host reads the record count (grows the arrays and runs
 //   the scan again on overflow) -> mv_key_kernel (per record: the block's key table, the committed table's answer) -> mv_check_kernel
 //   -> mv_mark_kernel (per transaction: flags of the independent ones) -> mv_walk_kernel (one thread: the dependent ones in order)
 //   -> growth of the table for the block's keys -> mv_apply_kernel (per key: its final state at (block_num, tx)) -> D2H flags.
+// Under CouchDB, cv_prepass runs first and turns VALID flags of d_tv into 24 or 254, so a 24 transaction drops out of the stage.
 // With an index installed the scan also emits range records, and before mv_mark_kernel: mv_written_kernel (the block's written public
 // keys) -> mv_sort_kernel (one launch per merge pass) -> mv_range_kernel (per range record: marking and the committed answer); after the
 // apply the index gains the block's new keys (ix_insert), and the delta is folded into the base when due (ix_finish).
@@ -2601,12 +2673,13 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     if (grow.rc) return grow.rc;
     memcpy(s.h_flags.get(), tv_flags, n);
     CK(ctx, cudaMemcpyAsync(s.d_tv.get(), s.h_flags.get(), n, cudaMemcpyHostToDevice, st));
+    const uint8_t* blk = ctx->bbs[slot].d_block.get();
+    if (s.couch && (rc = cv_prepass(ctx, st, blk, db.d_txs.get(), T))) return rc;
     const bool ix = s.indexed;
     if (ix) {
         grow(s.d_first_rng, 4 * (size_t)T); grow(s.d_n_rng, 4 * (size_t)T);
         if (grow.rc) return grow.rc;
     }
-    const uint8_t* blk = ctx->bbs[slot].d_block.get();
     bdev::MvccArrays a;
     uint32_t R = 0, G = 0;
     for (;;) {
@@ -3060,6 +3133,28 @@ int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t
     ctx->launches++;
     CK(ctx, cudaGetLastError());
     CK(ctx, cudaMemcpy(out, dout.get(), 32 * n, cudaMemcpyDeviceToHost));
+    return FABGPU_OK;
+}
+
+int fabgpu_test_couch_values(fabgpu_ctx* ctx, const uint8_t* blob, const uint32_t* off, size_t n, int path, uint32_t* out)
+{
+    if (!ctx || (n && (!blob || !off || !out)) || n > UINT32_MAX || path < 0 || path > 2) return FABGPU_E_ARG;
+    for (size_t i = 0; i < n; i++) if (off[i + 1] < off[i]) { ctx->last_error = "decreasing offsets"; return FABGPU_E_ARG; }
+    if (n == 0) return FABGPU_OK;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    const size_t bytes = std::max<size_t>(off[n], 1);
+    DevArray<uint8_t> d_b; DevArray<uint32_t> d_o, d_out;
+    Grow grow{ctx};
+    grow(d_b, bytes); grow(d_o, 4 * (n + 1)); grow(d_out, 4 * n);
+    if (grow.rc) return grow.rc;
+    CK(ctx, cudaMemcpy(d_b.get(), blob, off[n], cudaMemcpyHostToDevice));
+    CK(ctx, cudaMemcpy(d_o.get(), off, 4 * (n + 1), cudaMemcpyHostToDevice));
+    bdev::cv_test_kernel<<<(unsigned)((n + 127) / 128), 128>>>(d_b.get(), d_o.get(), (uint32_t)n, path, d_out.get());
+    bdev::cv_test_long_kernel<<<(unsigned)std::min<size_t>(n, 1024), bdev::CV_LT_THREADS>>>(d_b.get(), d_o.get(), (uint32_t)n, path, d_out.get());
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpy(out, d_out.get(), 4 * n, cudaMemcpyDeviceToHost));
     return FABGPU_OK;
 }
 

@@ -359,8 +359,8 @@ int fabgpu_committed_txids(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32
 int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n);
 int fabgpu_committed_txids_info(const fabgpu_ctx* ctx, unsigned long long out[2]);
 /* The ledger's MVCC check (core/ledger/kvledger/txmgmt/validation/validator.go:82-281), an opt-in stage after the validator, over a
- * device-resident table of the world state's committed key versions with LevelDB semantics (CouchDB's key and value checks are not
- * restated).  Entry i of a call is (namespace, collection, key) -> (ver[2i], ver[2i+1]) = (block_num, tx_num): three blobs with n + 1
+ * device-resident table of the world state's committed key versions with LevelDB semantics (CouchDB's key and value checks: see
+ * fabgpu_state_database).  Entry i of a call is (namespace, collection, key) -> (ver[2i], ver[2i+1]) = (block_num, tx_num): three blobs with n + 1
  * offsets each; the collection is empty for a public key, and for a private-data key the key is its 32-byte key hash.
  *   fabgpu_state_versions replaces the table; `height` is the ledger height (committed blocks), so the next block to check is block
  *       `height`.  capacity_hint (keys) sizes the table up front.  n = 0 with capacity_hint = 0 removes it.  It drains the block slots.
@@ -423,6 +423,28 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
 int fabgpu_state_versions_indexed(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob, const uint32_t* coll_off,
                                   const uint8_t* key_blob, const uint32_t* key_off, const uint64_t* ver, size_t n, uint64_t height, size_t capacity_hint);
 int fabgpu_state_index_info(const fabgpu_ctx* ctx, unsigned long long out[3]);
+/* The state database fabgpu_validate_mvcc restates, a context property: FABGPU_STATEDB_LEVELDB (the default) or FABGPU_STATEDB_COUCHDB;
+ * FABGPU_E_ARG for any other kind.  It changes only what later fabgpu_validate_mvcc calls do; fabgpu_state_versions* and
+ * fabgpu_msp_configure keep it.  While CouchDB is set:
+ *   fabgpu_validate_mvcc first runs validateWriteset (batch_preparer.go:317-330) with CouchDB's ValidateKeyValue (statecouchdb.go:427,
+ *       couchdoc_conv.go:37-57,278-297) over every transaction tv_flags leaves VALID and whose write set the stage enumerates: each public
+ *       KVWrite's key, and its value when the field is present (a delete's too); hashed and metadata writes are not checked.
+ *       A key is invalid when it is empty, starts with '_', or is not valid UTF-8 (utf8.ValidString).  A value is invalid when Go 1.14's
+ *       json.Unmarshal into a map[string]interface{} succeeds -- RFC 8259 grammar as encoding/json's scanner reads it, a top-level object
+ *       (or null, which has no fields), no number whose float64 overflows -- and a top-level member name, unescaped, is "~version" or
+ *       starts with '_'.  A transaction with an invalid write is INVALID_WRITESET (24): it drops out before the MVCC check, its reads
+ *       unchecked and its writes neither applied nor made unknown.  Otherwise it is 254 when some write is undecided: a value nested
+ *       deeper than 128 containers, or one holding a reserved name
+ *       and a number within the 40 leading digits of the overflow bound or with an exponent of 10000 or more.  It is also 254 when it
+ *       reads a public key CouchDB cannot hold, has a range whose start or end key is not UTF-8, or has a range with itr_exhausted false
+ *       whose end key CouchDB cannot hold.  Other ranges are decided as with LevelDB, over bytewise key order.  254s then take the
+ *       stage's undetermined-writer path.
+ *       A value of at most 16384 bytes is scanned by one thread, a longer one by one CTA; both give the same verdict.
+ *   fabgpu_state_versions, _indexed and _update refuse, with FABGPU_E_ARG and nothing changed, a version for a public key CouchDB cannot
+ *       hold.  A removal of one is accepted: a key a 254 transaction writes becomes unknown, and one CouchDB cannot hold is settled by
+ *       removing it. */
+enum { FABGPU_STATEDB_LEVELDB = 0, FABGPU_STATEDB_COUCHDB = 1 };
+int fabgpu_state_database(fabgpu_ctx* ctx, int kind);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
@@ -459,6 +481,12 @@ int fabgpu_test_fieldop(fabgpu_ctx* ctx, int op, const uint8_t* a, const uint8_t
  * [1, 2^w)); key_slot <= -2: a small handle from fabgpu_keys_register_small (w and the window count from fabgpu_small_table_info,
  * digit in [1, 2^(w-1)]), FABGPU_E_ARG when the handle is stale.  Reads a small table only after its build has finished. */
 int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* window, const uint32_t* digit, size_t n, uint8_t* out);
+/* The verdict of fabgpu_state_database's CouchDB value check on each of n values (blob with n + 1 offsets): out[i] holds bits
+ * 1 the scanner accepts it, 2 the top-level value is an object, 4 a number overflows float64, 8 a number is undecided, 16 a top-level
+ * name is reserved; or 32 (with 2 when the top-level value is an object) when a container deeper than 128 opens before any syntax
+ * error, as fabric-mod_b200/csrc/couchval.cuh.  path 0 scans as fabgpu_validate_mvcc does (one thread for a value of at most 16384
+ * bytes, one CTA for a longer one); 1 forces the one-thread scan, 2 the CTA scan; FABGPU_E_ARG for any other path. */
+int fabgpu_test_couch_values(fabgpu_ctx* ctx, const uint8_t* blob, const uint32_t* off, size_t n, int path, uint32_t* out);
 /* Phase times of the last fabgpu_bccsp_verify_batch call, microseconds: [0] key-table lookup/registration,
  * [1] staging copy into pinned memory (host gates + packing on the host-gated path), [2] H2D + kernels + D2H (enqueue to
  * completion), [3] status copy-out.  For metrics export
