@@ -32,7 +32,7 @@ EXPORTS = [
     "fabgpu_peer_mask_create", "fabgpu_peer_mask_open", "fabgpu_peer_mask_close", "fabgpu_verify_p256_device_keyed_allgather",
     "fabgpu_validate_block_async", "fabgpu_validate_envelopes_async", "fabgpu_validate_wait", "fabgpu_block_buffer_slot",
     "fabgpu_keys_register_small", "fabgpu_small_slot_capacity", "fabgpu_key_table_stats", "fabgpu_small_table_info",
-    "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info",
+    "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info", "fabgpu_committed_txids_add_block",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
 ]
@@ -475,6 +475,11 @@ class Context:
         """Upserts ids into the installed set (fabgpu_committed_txids_add) without draining the blocks in flight: seen by every block
         submitted after this returns, by none submitted before."""
         self._committed_txids(lib().fabgpu_committed_txids_add, ids, kinds, ())
+
+    def committed_txids_add_block(self, slot):
+        """Upserts the ids the block store indexes for the block submitted on `slot` (fabgpu_committed_txids_add_block), extracted on the
+        device: call it after validate_*_async(slot) (or a blocking validate_* call, slot 0) and before the slot's next submit."""
+        self._ck(lib().fabgpu_committed_txids_add_block(self._h, ctypes.c_int(slot)))
 
     def committed_txids_info(self):
         """(distinct ids held, table slots)"""

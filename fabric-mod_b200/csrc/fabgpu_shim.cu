@@ -26,6 +26,7 @@
 #include "cuda_owned.hpp"
 #include "sha256.cuh"
 #include "blockdev_kernels.cuh"
+#include "txidblock.cuh"
 #include "keypolicy.hpp"
 #include "txidset.hpp"
 #include "stateset.hpp"
@@ -257,6 +258,7 @@ struct fabgpu_ctx {
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
         bool busy = false, on_device = false, use_ev = false, kl_on = false, v13 = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
         bool mvcc_ready = false;                 // fabgpu_validate_wait returned the block and its bytes are still on the device
+        uint8_t txid_block = 0;                  // fabgpu_committed_txids_add_block: 0 no block submitted, 1 submitted, 2 its ids added
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
@@ -277,6 +279,10 @@ struct fabgpu_ctx {
         bdev::TxidSlot* table = nullptr; uint64_t slots = 0;                   // table: stream-ordered allocation on `stream`
         const uint64_t seed = txid::random_seed();
         bool installed = false, broken = false; unsigned long long count = 0, pending = 0;
+        // fabgpu_committed_txids_add_block: the block's id records and its de-duplication index (one add runs at a time on `stream`);
+        // read_ev[slot] follows the last kernel that reads the slot's block and envelope table, and the slot's next submit waits for it
+        DevArray<bdev::TxidSlot> d_brec; DevArray<uint32_t> d_dd;
+        Event read_ev[FABGPU_SLOTS]; bool read_set[FABGPU_SLOTS] = {};
         ~TxidSet() { if (table) cudaFree(table); }
     } txid;
     // fabgpu_state_versions: the world state's key versions on device 0 (stateset.cuh); ledger state, so fabgpu_msp_configure keeps it.
@@ -2103,12 +2109,12 @@ static void txid_drop_table(fabgpu_ctx* ctx)
     s.table = nullptr; s.slots = 0;
 }
 
-// Grows the table (doubling, to at least min_slots) so that `recs` fit at a load of at most 1/2, inserts them, and records the set event
-static int txid_insert_records(fabgpu_ctx* ctx, const std::vector<bdev::TxidSlot>& recs, uint64_t min_slots)
+// Grows the table (doubling, to at least min_slots) so that `n` more ids fit at a load of at most 1/2
+static int txid_room(fabgpu_ctx* ctx, uint64_t n, uint64_t min_slots)
 {
     auto& s = ctx->txid;
     cudaStream_t st = s.stream.get();
-    const uint64_t want = std::max(txid::slots_for(s.count + s.pending + recs.size(), s.slots), min_slots);
+    const uint64_t want = std::max(txid::slots_for(s.count + s.pending + n, s.slots), min_slots);
     if (want != s.slots) {
         const uint64_t bytes = want * sizeof(bdev::TxidSlot);
         if (bytes > txid_max_bytes() || want > (1ull << 32)) {
@@ -2129,6 +2135,26 @@ static int txid_insert_records(fabgpu_ctx* ctx, const std::vector<bdev::TxidSlot
         txid_drop_table(ctx);
         s.table = nt; s.slots = want;
     }
+    return FABGPU_OK;
+}
+
+// Records the set event after the count's copy: later submits wait for it, and the next call takes the count once it has passed
+static int txid_publish(fabgpu_ctx* ctx)
+{
+    auto& s = ctx->txid;
+    cudaStream_t st = s.stream.get();
+    CK(ctx, cudaMemcpyAsync(s.h_count.get(), s.d_count.get(), 8, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaEventRecord(s.ev.get(), st));
+    s.ev_set = true;
+    return FABGPU_OK;
+}
+
+// Grows the table so that `recs` fit, inserts them, and records the set event
+static int txid_insert_records(fabgpu_ctx* ctx, const std::vector<bdev::TxidSlot>& recs, uint64_t min_slots)
+{
+    auto& s = ctx->txid;
+    cudaStream_t st = s.stream.get();
+    if (int rc = txid_room(ctx, recs.size(), min_slots)) return rc;
     const size_t n = recs.size();
     if (n) {
         const int r = (int)(s.seq++ % fabgpu_ctx::TxidSet::RING);
@@ -2149,10 +2175,7 @@ static int txid_insert_records(fabgpu_ctx* ctx, const std::vector<bdev::TxidSlot
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
-    CK(ctx, cudaMemcpyAsync(s.h_count.get(), s.d_count.get(), 8, cudaMemcpyDeviceToHost, st));
-    CK(ctx, cudaEventRecord(s.ev.get(), st));
-    s.ev_set = true;
-    return FABGPU_OK;
+    return txid_publish(ctx);
 }
 
 // A failed mutation may have lost ids: from here on every lookup answers "unanswerable" (254) until a replacing call succeeds
@@ -2206,6 +2229,49 @@ int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const ui
     if (s.broken) { ctx->last_error = "the committed tx-id set is broken by a failed call: replace it with fabgpu_committed_txids"; return FABGPU_E_ARG; }
     int rc = txid_begin(ctx, false);
     if (!rc) rc = txid_insert_records(ctx, recs, 0);
+    return rc ? txid_fail(ctx, rc) : FABGPU_OK;
+}
+
+// The slot's block, on the set's stream after every slot's last decide stage (txid_begin): growth for T more ids, then
+// txid_block_id_kernel (reads the slot's block and envelope table; read_ev follows it) and txid_block_insert_kernel (txidblock.cuh)
+static int txid_insert_block(fabgpu_ctx* ctx, int slot)
+{
+    auto& s = ctx->txid; auto& db = ctx->dbs[slot];
+    cudaStream_t st = s.stream.get();
+    const uint32_t T = (uint32_t)db.T;
+    if (int rc = txid_room(ctx, T, 0)) return rc;
+    uint32_t dd = 64;
+    while (dd < 2 * (uint64_t)T) dd <<= 1;
+    Grow grow{ctx};
+    grow(s.d_brec, sizeof(bdev::TxidSlot) * (size_t)T); grow(s.d_dd, 4 * (size_t)dd);
+    if (grow.rc) return grow.rc;
+    if (!s.read_ev[slot]) { cudaEvent_t ev = nullptr; CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); s.read_ev[slot].reset(ev); }
+    CK(ctx, cudaMemsetAsync(s.d_dd.get(), 0, 4 * (size_t)dd, st));
+    bdev::txid_block_id_kernel<<<(T + 127) / 128, 128, 0, st>>>(ctx->bbs[slot].d_block.get(), db.d_env_off.get(), T, s.d_brec.get());
+    CK(ctx, cudaEventRecord(s.read_ev[slot].get(), st));
+    s.read_set[slot] = true;
+    bdev::txid_block_insert_kernel<<<(T + 255) / 256, 256, 0, st>>>(s.table, (uint32_t)(s.slots - 1), s.seed, s.d_brec.get(), T, s.d_dd.get(), dd - 1,
+                                                                    s.d_count.get());
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    s.pending += T;
+    return txid_publish(ctx);
+}
+
+int fabgpu_committed_txids_add_block(fabgpu_ctx* ctx, int slot)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->txid; auto& db = ctx->dbs[slot];
+    if (!s.installed) { ctx->last_error = "no committed tx-id set installed: call fabgpu_committed_txids first"; return FABGPU_E_ARG; }
+    if (s.broken) { ctx->last_error = "the committed tx-id set is broken by a failed call: replace it with fabgpu_committed_txids"; return FABGPU_E_ARG; }
+    if (db.txid_block == 0) { ctx->last_error = "the slot holds no submitted block"; return FABGPU_E_ARG; }
+    if (db.txid_block == 2) { ctx->last_error = "the slot's block was already added"; return FABGPU_E_ARG; }
+    db.txid_block = 2;
+    if (db.T == 0) return FABGPU_OK;
+    int rc = txid_begin(ctx, false);
+    if (!rc) rc = txid_insert_block(ctx, slot);
     return rc ? txid_fail(ctx, rc) : FABGPU_OK;
 }
 
@@ -2826,9 +2892,19 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
             CK(ctx, cudaMemcpy(dm.key_slot.get(), raw.data(), 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
         }
     }
+    // The slot's last fabgpu_committed_txids_add_block may still be reading its block and envelope table (TxidSet::read_ev): a buffer
+    // is reallocated only after that kernel has finished, and the copies below are enqueued behind it.
+    auto& tx_set = ctx->txid;
+    auto txid_read_done = [&]() -> int {
+        if (tx_set.read_set[slot]) CK(ctx, cudaEventSynchronize(tx_set.read_ev[slot].get()));
+        tx_set.read_set[slot] = false;
+        return FABGPU_OK;
+    };
     // slack: word-wise readers (bytes_equal, the SHA loader) touch the aligned words past the end.  An empty block needs no buffer.
-    if (block_len && block_len + 64 > bb.d_block.bytes())
+    if (block_len && block_len + 64 > bb.d_block.bytes()) {
+        if (int rc = txid_read_done()) return rc;
         if (int rc = bb.d_block.reserve(ctx, block_len + (block_len >> 2) + 64)) return rc;
+    }
     const char* evs = getenv("FABGPU_BLOCK_EVENTS");          // "1": time the device stages with CUDA events (diagnostics)
     db.use_ev = evs && evs[0] == '1';
     if (db.use_ev) for (auto& e : db.ev) if (!e) { cudaEvent_t ev = nullptr; CK(ctx, cudaEventCreate(&ev)); e.reset(ev); }
@@ -2847,6 +2923,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     if (T == 0) return FABGPU_OK;
     const size_t J_cap = T * (1 + BD_ENDS_HINT);
     if (T > db.tx_cap()) {
+        if (int rc = txid_read_done()) return rc;
         const size_t tc = T + (T >> 2) + 256, jc = tc * (1 + BD_ENDS_HINT);
         Grow grow{ctx};
         grow(db.d_env_off, 8 * (tc + 1)); grow(db.d_txs, sizeof(bdev::TxDev) * tc);
@@ -2867,6 +2944,10 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
         db.h_env_off.get()[2 * i + 1] = env_off ? env_off[i + 1] : split[2 * i + 1];
     }
     cudaStream_t st = ds.stream.get();
+    if (tx_set.read_set[slot]) {
+        CK(ctx, cudaStreamWaitEvent(st, tx_set.read_ev[slot].get(), 0));
+        tx_set.read_set[slot] = false;
+    }
     CK(ctx, cudaMemcpyAsync(db.d_env_off.get(), db.h_env_off.get(), 8 * T, cudaMemcpyHostToDevice, st));
     CK(ctx, cudaMemsetAsync(db.d_counter.get(), 0, 16, st));
     bdev::MspDev m; m.id_blob = dm.id_blob.get(); m.id_off = dm.id_off.get(); m.key_slot = dm.key_slot.get(); m.valid = dm.valid.get(); m.msp_code = dm.msp_code.get(); m.group = dm.group.get();
@@ -2922,7 +3003,6 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
                            db.d_counter.get(), cnt, nullptr, db.d_idx.get(), dm.classes ? dm.classes : CLASS_GENERIC, db.d_scal.get());
     if (rc) return rc;
     // the committed tx-id set as the mutations returned so far left it (all of them, as submitters and mutations hold slot0_mu)
-    auto& tx_set = ctx->txid;
     bdev::TxidSetDev tsd{nullptr, 0, 0, 0};
     if (tx_set.installed) {
         tsd.slots = tx_set.table; tsd.mask = (uint32_t)(tx_set.slots - 1); tsd.seed = tx_set.seed; tsd.broken = tx_set.broken || !tx_set.table;
@@ -3019,7 +3099,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     auto& db = ctx->dbs[slot];
     if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-    db.mvcc_ready = false;
+    db.mvcc_ready = false; db.txid_block = 0;
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
     int rc;
     {
@@ -3028,7 +3108,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
         if (rc) { cudaStreamSynchronize(ctx->devs[0].slot[slot].stream.get()); return rc; }
         db.on_device = true;
     }
-    db.busy = true;
+    db.busy = true; db.txid_block = 1;
     return FABGPU_OK;
 }
 
@@ -3045,7 +3125,7 @@ int fabgpu_validate_envelopes_async(fabgpu_ctx* ctx, int slot, const uint8_t* bl
         std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
         auto& db = ctx->dbs[slot];
         if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false;
+        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false; db.txid_block = 1;
         return FABGPU_OK;
     }
     return validate_submit(ctx, slot, blob, env_off[n_env], env_off, n_env);

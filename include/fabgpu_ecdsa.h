@@ -354,10 +354,20 @@ int fabgpu_namespace_versions(fabgpu_ctx* ctx, const uint8_t* ver_blob, const ui
  *   that lacks ids.
  *   FABGPU_E_ARG, with a fabgpu_last_error text and the previous set kept, for NULL arrays with n > 0, decreasing offsets and a kind
  *   other than 0 or 1.  fabgpu_msp_configure keeps the set.
- *   fabgpu_committed_txids_info: out[0] = distinct ids held (0 while broken or removed), out[1] = table slots. */
+ *   fabgpu_committed_txids_info: out[0] = distinct ids held (0 while broken or removed), out[1] = table slots.
+ *   fabgpu_committed_txids_add_block upserts, with kind 0, the ids the block store indexes for the block of `slot`: the id
+ *       protoutil.GetOrComputeTxIDFromEnvelope gives for every envelope, whatever its flag -- a non-empty ChannelHeader.tx_id (kept only
+ *       when canonical), else hex(SHA-256(nonce || creator)) of its SignatureHeader; nothing for an envelope, payload, header or channel
+ *       header that does not unmarshal, a payload without a header, or (with an empty tx_id) a signature header that does not.  The ids
+ *       are extracted and inserted on the device: the host neither parses the block nor waits.  Call it after
+ *       fabgpu_validate_{block,envelopes}_async(slot) (or a blocking fabgpu_validate_block / _envelopes, slot 0) has returned and before
+ *       the slot's next submit; ordering is that of _add.  The slot's next submit waits on the device for the add to have read the
+ *       slot's block.  FABGPU_E_ARG, nothing enqueued, when no set is installed, the set is broken, the slot holds no submitted block,
+ *       or its block was already added.  Growth is decided on the ids held plus those sent since plus the block's transactions. */
 int fabgpu_committed_txids(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n, size_t capacity_hint);
 int fabgpu_committed_txids_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* kind, size_t n);
 int fabgpu_committed_txids_info(const fabgpu_ctx* ctx, unsigned long long out[2]);
+int fabgpu_committed_txids_add_block(fabgpu_ctx* ctx, int slot);
 /* The ledger's MVCC check (core/ledger/kvledger/txmgmt/validation/validator.go:82-281), an opt-in stage after the validator, over a
  * device-resident table of the world state's committed key versions with LevelDB semantics (CouchDB's key and value checks: see
  * fabgpu_state_database).  Entry i of a call is (namespace, collection, key) -> (ver[2i], ver[2i+1]) = (block_num, tx_num): three blobs with n + 1
