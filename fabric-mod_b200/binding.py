@@ -19,7 +19,7 @@ OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
 
 # every symbol include/fabgpu_ecdsa.h declares (tests/test_abi.py checks the header against this and the .so)
 EXPORTS = [
-    "fabgpu_init", "fabgpu_destroy", "fabgpu_last_error", "fabgpu_device_count", "fabgpu_max_batch",
+    "fabgpu_init", "fabgpu_init_shared", "fabgpu_destroy", "fabgpu_last_error", "fabgpu_device_count", "fabgpu_max_batch",
     "fabgpu_host_buffers", "fabgpu_verify_p256", "fabgpu_verify_p256_async", "fabgpu_wait", "fabgpu_verify_p256_host",
     "fabgpu_verify_p256_device", "fabgpu_bccsp_verify_batch", "fabgpu_bccsp_verify", "fabgpu_gate_signature",
     "fabgpu_test_fieldop", "fabgpu_test_table_entries", "fabgpu_launch_count",
@@ -68,6 +68,7 @@ def lib():
         L.fabgpu_max_batch.argtypes = [ctypes.c_void_p]
         L.fabgpu_launch_count.restype = ctypes.c_ulonglong
         L.fabgpu_launch_count.argtypes = [ctypes.c_void_p]
+        L.fabgpu_init_shared.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
         L.fabgpu_destroy.argtypes = [ctypes.c_void_p]
         L.fabgpu_destroy.restype = None
         L.fabgpu_device_count.argtypes = [ctypes.c_void_p]
@@ -159,12 +160,17 @@ def gate_signature(sig: bytes):
 
 
 class Context:
-    """fabgpu_ctx owner.  device_ids=None -> CUDA device 0."""
+    """fabgpu_ctx owner.  device_ids=None -> CUDA device 0.  share_tables_with=<Context>: a context on that context's devices that shares
+    its point tables and key caches (fabgpu_init_shared; device_ids must then be None), e.g. one per channel of a peer."""
 
-    def __init__(self, max_batch=65536, device_ids=None):
+    def __init__(self, max_batch=65536, device_ids=None, share_tables_with=None):
         L = lib()
         self._h = ctypes.c_void_p()
-        if device_ids:
+        if share_tables_with is not None:
+            if device_ids:
+                raise ValueError("a context that shares tables runs on the devices of the context it shares with")
+            rc = L.fabgpu_init_shared(share_tables_with._h, ctypes.c_size_t(max_batch), ctypes.byref(self._h))
+        elif device_ids:
             arr = (ctypes.c_int * len(device_ids))(*device_ids)
             rc = L.fabgpu_init(arr, ctypes.c_int(len(device_ids)), ctypes.c_size_t(max_batch), ctypes.byref(self._h))
         else:

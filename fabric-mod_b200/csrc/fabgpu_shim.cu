@@ -53,11 +53,11 @@ struct DevSlot {
     DevArray<uint4> d_scal;         // 4 x dev_cap: scalars u1, u2 of the key-table kernel (ecdsa_prep_kernel)
 };
 
-// Members go in reverse order of declaration, with this device current (~Device).
-struct Device {
+// The point tables of one device, shared by every context of a group (KeyTables).  Members go in reverse order of declaration, with
+// this device current (~DevTables).
+struct DevTables {
     int id = 0;
     DevArray<aff> gtab;
-    int sms = 132;            // multiprocessors (launch shapes; read from the device at fabgpu_init)
     DevArray<aff> qtab;       // key_slots tables of FAB_G_WINDOWS * FAB_G_ENTRIES points (per-key fixed-base tables)
     // small key tables (FAB_S_POINTS points each): the pool, the build scratch (grown on demand) and the build stream.  Every
     // enqueue that may read a small table first makes its stream wait for s_ev (the last build): builds are ordered among
@@ -66,6 +66,58 @@ struct Device {
     DevArray<uint8_t> s_keys; DevArray<int32_t> s_slots; DevArray<aff> s_bases;
     size_t s_cap() const { return s_bases.bytes() / (FAB_S_WINDOWS * sizeof(aff)); }
     Stream s_stream; Event s_ev; bool s_ev_set = false;
+    ~DevTables() { cudaSetDevice(id); }
+};
+
+// What does not depend on the channel: the device tables and the key caches that map keys to them.  fabgpu_init makes a group of one
+// context, fabgpu_init_shared adds a context to it; the last context of the group to go frees this.
+//
+// Locks, in this order (a path may skip any, never reverse two, and never holds one context's lock while taking another's):
+//   tab_mu (shared / exclusive) -> a context's fabgpu_ctx::mu -> mu.
+// Whoever turns handles into raw slot numbers and then enqueues kernels that read those slots' tables holds tab_mu SHARED from the
+// resolution to the last enqueue, in whichever context it enqueues.  fabgpu_keys_register and the small tier hold it EXCLUSIVE while
+// they recycle slots (after draining every stream of the device), so no context of the group sits between "resolved" and
+// "enqueued" when a slot changes hands.  The maps, slot owners, generations, the free list, the build counters, s_ev / s_ev_set
+// and the table contents change only under tab_mu exclusive AND mu; the LRU ticks and the seen counters change under mu (with
+// tab_mu shared or exclusive).  A reader holds mu, or tab_mu for what changes only under it exclusively.
+struct KeyTables {
+    std::vector<DevTables> devs;           // the group's devices, in the contexts' device order
+    std::shared_mutex tab_mu;
+    std::mutex mu;
+    // per-key table cache (fabgpu_keys_register): 64-byte X||Y -> slot, least-recently-used eviction
+    int key_slots = 0;
+    std::unordered_map<std::string, int> key_map;
+    std::vector<std::string> slot_key;
+    std::vector<unsigned long long> slot_tick;
+    std::vector<uint32_t> slot_gen;          // bumped whenever a slot is recycled: handles carry the generation they were issued under
+    unsigned long long tick = 0;
+    int key_min_uses = 256;
+    // small-table cache (fabgpu_keys_register_small): same protocol as the big tables, least-recently-used eviction in bulk.  A small
+    // handle is -2 - ((generation & 0x3ff) << 20 | slot); on the device the code is -2 - slot.
+    int small_slots = 0;
+    // Cumulative signatures of a key (over all calls) before it earns a small table; < 0: tier off.  A table costs about as much GPU time as a few dozen
+    // generic verifications and saves most of one per later signature: 32 is the rent-or-buy point -- by then the key has cost as much on the
+    // generic kernel as its table does, so building is at most twice the optimum whatever the key does next, and a block full of one-off keys is
+    // not slowed down by thousands of useless builds.
+    int small_min_uses = 32;
+    struct Key64 { uint8_t b[64]; bool operator==(const Key64& o) const { return memcmp(b, o.b, 64) == 0; } };
+    struct Key64Hash { size_t operator()(const Key64& k) const { uint64_t h; memcpy(&h, k.b + 8, 8); return (size_t)(h * 0x9E3779B97F4A7C15ull); } };
+    std::unordered_map<Key64, int, Key64Hash> small_map;
+    std::vector<Key64> small_key; std::vector<char> small_used;
+    std::vector<unsigned long long> small_tick;
+    std::vector<uint32_t> small_gen;
+    std::vector<int> small_free;
+    unsigned long long small_built = 0, small_recycled = 0;     // fabgpu_key_table_stats
+    // Keys without any table: signatures seen so far.  Buckets of four (tag, count) entries indexed by a hash of the key bytes -- no allocation
+    // on the batch path; a full bucket gives up its least used entry, which only delays that key's table (resolve_key_tables).
+    std::vector<uint64_t> seen_tag; std::vector<uint32_t> seen_cnt;
+};
+
+// A context's own part of a device.  Members go in reverse order of declaration, with this device current (~Device).
+struct Device {
+    int id = 0;
+    DevTables* tab = nullptr;  // the group's tables on this device
+    int sms = 132;            // multiprocessors (launch shapes; read from the device at fabgpu_init)
     DevSlot slot[FABGPU_SLOTS];
     // Stream-ordered scratch for launches on a caller's stream (fabgpu_verify_p256_device_keyed*), which own no slot: allocated and
     // freed in the launch's stream order, so concurrent callers on different streams never share a buffer and never wait for
@@ -150,49 +202,19 @@ private:
 };
 
 struct fabgpu_ctx {
+    std::shared_ptr<KeyTables> kt;     // the group's tables and key caches (first: they go after this context's devices and streams)
     std::vector<Device> devs;
     std::unique_ptr<GatePool> pool;
     HostSlot hslot[FABGPU_SLOTS];
     size_t max_batch = 0;      // per slot, whole context
     size_t dev_cap = 0;        // per device per slot (multiple of 32)
     std::string last_error;
-    std::mutex mu;         // guards enqueue and the key-table bookkeeping
-    // Key-table slots: whoever turns handles into raw slot numbers and then enqueues kernels that read those slots' tables holds this
-    // SHARED from the resolution to the last enqueue; fabgpu_keys_register holds it EXCLUSIVE while it recycles slots (it then drains
-    // every stream before rebuilding a table), so a slot cannot change hands between "resolved" and "enqueued".  Order: tab_mu, then mu.
-    std::shared_mutex tab_mu;
+    std::mutex mu;         // guards this context's enqueue state; lock order: kt->tab_mu, mu, kt->mu (KeyTables)
     std::mutex sync_mu;    // one synchronous fabgpu_bccsp_verify_batch at a time
     std::mutex sync_blk_mu;   // one synchronous fabgpu_validate_block / _envelopes at a time
     std::mutex slot0_mu;   // serialises the composite calls that stage through slot 0's pinned buffers
     std::atomic<unsigned long long> launches{0};
-    // per-key table cache (fabgpu_keys_register): 64-byte X||Y -> slot, least-recently-used eviction
-    int key_slots = 0;
-    std::unordered_map<std::string, int> key_map;
-    std::vector<std::string> slot_key;
-    std::vector<unsigned long long> slot_tick;
-    std::vector<uint32_t> slot_gen;          // bumped whenever a slot is recycled: handles carry the generation they were issued under
-    unsigned long long tick = 0;
-    int key_min_uses = 256;
-    // small-table cache (fabgpu_keys_register_small): same protocol as the big tables (tab_mu / mu), least-recently-used eviction
-    // in bulk.  A small handle is -2 - ((generation & 0x3ff) << 20 | slot); on the device the code is -2 - slot.
-    int small_slots = 0;
     int small_threads_env = 0;                // FABGPU_SMALL_THREADS: CTA width of ecdsa_verify_small_kernel (0 = by batch size)
-    // Cumulative signatures of a key (over all calls) before it earns a small table; < 0: tier off.  A table costs about as much GPU time as a few dozen
-    // generic verifications and saves most of one per later signature: 32 is the rent-or-buy point -- by then the key has cost as much on the
-    // generic kernel as its table does, so building is at most twice the optimum whatever the key does next, and a block full of one-off keys is
-    // not slowed down by thousands of useless builds.
-    int small_min_uses = 32;
-    struct Key64 { uint8_t b[64]; bool operator==(const Key64& o) const { return memcmp(b, o.b, 64) == 0; } };
-    struct Key64Hash { size_t operator()(const Key64& k) const { uint64_t h; memcpy(&h, k.b + 8, 8); return (size_t)(h * 0x9E3779B97F4A7C15ull); } };
-    std::unordered_map<Key64, int, Key64Hash> small_map;
-    std::vector<Key64> small_key; std::vector<char> small_used;
-    std::vector<unsigned long long> small_tick;
-    std::vector<uint32_t> small_gen;
-    std::vector<int> small_free;
-    unsigned long long small_built = 0, small_recycled = 0;     // fabgpu_key_table_stats
-    // Keys without any table: signatures seen so far.  Buckets of four (tag, count) entries indexed by a hash of the key bytes -- no allocation
-    // on the batch path; a full bucket gives up its least used entry, which only delays that key's table (resolve_key_tables).
-    std::vector<uint64_t> seen_tag; std::vector<uint32_t> seen_cnt;
     // key-table kernel (FABGPU_CACHED_KERNEL): 0 "jac" = Jacobian chain, one signature per thread (ecdsa_verify_cached_kernel) -- the DEFAULT; the
     // others stay selectable for comparison (tools/kbench.py); 1 "ba" = batch-affine with CTA-shared inversions, 3 "ba2" = batch-affine, two
     // signatures per thread, 2 / 4 "l2" / "l4" = the Jacobian chain split over 2 / 4 lanes.  The alternatives stay selectable: they are the measurements.
@@ -314,7 +336,8 @@ struct fabgpu_ctx {
         uint32_t cv_hint = 4;                                                            // public writes per transaction
         ~StateSet() { if (table) cudaFree(table); }
     } sv;
-    // The members above go in reverse order of declaration -- block slots and MSP copy first, devices last -- with device 0 current.
+    // The members above go in reverse order of declaration -- block slots and MSP copy first, then devices, then the group's tables if
+    // this context was the last to hold them -- with device 0 current.
     ~fabgpu_ctx() { if (!devs.empty()) cudaSetDevice(devs[0].id); }
 };
 
@@ -419,11 +442,11 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         if (n_dev) { ctx->last_error = "peer exchange needs a host-known batch size"; return FABGPU_E_ARG; }
     }
     if (n == 0 && !peer) return FABGPU_OK;
-    if ((mode == MODE_MIXED || mode == MODE_SMALL) && dv.s_ev_set) CK(ctx, cudaStreamWaitEvent(st, dv.s_ev.get(), 0));   // small tables still being built
+    if ((mode == MODE_MIXED || mode == MODE_SMALL) && dv.tab->s_ev_set) CK(ctx, cudaStreamWaitEvent(st, dv.tab->s_ev.get(), 0));   // small tables still being built
     if (mode == MODE_SMALL && n > 0) {
         const unsigned sthreads = small_threads(ctx, dv, n, false);
         ecdsa_verify_small_kernel<<<(unsigned)((n + sthreads - 1) / sthreads), sthreads, 0, st>>>(
-            nullptr, nullptr, 0u, key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.stab.get(), mask, off);
+            nullptr, nullptr, 0u, key_slot, e, r, s, (uint32_t)n, dv.tab->gtab.get(), dv.tab->stab.get(), mask, off);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -437,16 +460,16 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
             const unsigned sigs = FAB_LANES_THREADS / (unsigned)ctx->cached_kernel, blocks = (unsigned)((n + sigs - 1) / sigs);
             uint32_t nn = (uint32_t)n;
             if (n_dev) { ctx->last_error = "the lane-split kernel has no device-side batch size"; return FABGPU_E_ARG; }
-            if (ctx->cached_kernel == 2) ecdsa_verify_lanes_kernel<2><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab.get(), dv.qtab.get(), mask, off);
-            else ecdsa_verify_lanes_kernel<4><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.gtab.get(), dv.qtab.get(), mask, off);
+            if (ctx->cached_kernel == 2) ecdsa_verify_lanes_kernel<2><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.tab->gtab.get(), dv.tab->qtab.get(), mask, off);
+            else ecdsa_verify_lanes_kernel<4><<<blocks, FAB_LANES_THREADS, 0, st>>>(key_slot, e, r, s, nn, dv.tab->gtab.get(), dv.tab->qtab.get(), mask, off);
         } else if (ctx->cached_kernel == 3 && !n_dev && !fused_peer) {
             // batch-affine, two signatures per thread, no CTA exchange
             const unsigned per = 2 * FAB_BA2_THREADS, blocks = (unsigned)((n + per - 1) / per);
-            ecdsa_verify_ba2_kernel<<<blocks, FAB_BA2_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off);
+            ecdsa_verify_ba2_kernel<<<blocks, FAB_BA2_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.tab->gtab.get(), dv.tab->qtab.get(), mask, off);
         } else if (ctx->cached_kernel == 1 || ctx->cached_kernel == 3) {
             // batch-affine accumulation with CTA-shared inversions (ecdsa_batchaffine.cuh): fixed CTA width
             const unsigned blocks = (unsigned)((n + FAB_BA_THREADS - 1) / FAB_BA_THREADS);
-            ecdsa_verify_ba_kernel<<<blocks, FAB_BA_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off, n_dev, n_base, po);
+            ecdsa_verify_ba_kernel<<<blocks, FAB_BA_THREADS, 0, st>>>(key_slot, e, r, s, (uint32_t)n, dv.tab->gtab.get(), dv.tab->qtab.get(), mask, off, n_dev, n_base, po);
         } else {
         // the scalars (ecdsa_prep_kernel), then the chain.  scal: 64 bytes per signature from the caller's slot, or stream-ordered from
         // the device's pool when the launch has no slot
@@ -458,7 +481,7 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         const size_t sms = (size_t)dv.sms;
         if (!n_dev && n > sms * 384) threads = (n <= sms * FAB_CACHED_THREADS) ? FAB_CACHED_THREADS : 256;
         const unsigned blocks = (unsigned)((n + threads - 1) / threads);
-        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, scal, r, (uint32_t)n, dv.gtab.get(), dv.qtab.get(), mask, off, n_dev, n_base, po);
+        ecdsa_verify_cached_kernel<<<blocks, threads, 0, st>>>(key_slot, scal, r, (uint32_t)n, dv.tab->gtab.get(), dv.tab->qtab.get(), mask, off, n_dev, n_base, po);
         if (own) CK(ctx, cudaFreeAsync(scal, st));
         }
         ctx->launches++;
@@ -472,17 +495,17 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         if (classes & CLASS_SMALL) {
             const unsigned sthreads = small_threads(ctx, dv, n, true);
             ecdsa_verify_small_kernel<<<(unsigned)((n + sthreads - 1) / sthreads), sthreads, 0, st>>>(
-                scratch_idx, scratch_idx + n + 1, (uint32_t)n, key_slot, e, r, s, (uint32_t)n, dv.gtab.get(), dv.stab.get(), mask, off);
+                scratch_idx, scratch_idx + n + 1, (uint32_t)n, key_slot, e, r, s, (uint32_t)n, dv.tab->gtab.get(), dv.tab->stab.get(), mask, off);
         }
         if (classes & CLASS_GENERIC)
             ecdsa_verify_indexed_kernel<<<(unsigned)((n + FAB_INDEXED_THREADS - 1) / FAB_INDEXED_THREADS), FAB_INDEXED_THREADS, 0, st>>>(
-                scratch_idx, scratch_idx + n, qx, qy, e, r, s, dv.gtab.get(), mask, off);
+                scratch_idx, scratch_idx + n, qx, qy, e, r, s, dv.tab->gtab.get(), mask, off);
         ctx->launches += 1 + ((classes & CLASS_SMALL) ? 1 : 0) + ((classes & CLASS_GENERIC) ? 1 : 0);
         CK(ctx, cudaGetLastError());
     } else if (mode == MODE_MIXED && n > 0) {
         // no scratch (launches on a caller's stream): the generic kernel filters on key_slot itself
         const unsigned gthreads = 128, blocks = (unsigned)((n + gthreads - 1) / gthreads);
-        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(key_slot, qx, qy, e, r, s, (uint32_t)n, dv.gtab.get(), mask, off, n_dev, n_base);
+        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(key_slot, qx, qy, e, r, s, (uint32_t)n, dv.tab->gtab.get(), mask, off, n_dev, n_base);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -492,7 +515,7 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
         unsigned gthreads = 64;
         if (!n_dev && n > (size_t)dv.sms * 192) gthreads = (n <= (size_t)dv.sms * FAB_VERIFY_THREADS) ? FAB_VERIFY_THREADS : 256;
         const unsigned blocks = (unsigned)((n + gthreads - 1) / gthreads);
-        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(nullptr, qx, qy, e, r, s, (uint32_t)n, dv.gtab.get(), mask, off, n_dev, n_base);
+        ecdsa_verify_kernel<<<blocks, gthreads, 0, st>>>(nullptr, qx, qy, e, r, s, (uint32_t)n, dv.tab->gtab.get(), mask, off, n_dev, n_base);
         ctx->launches++;
         CK(ctx, cudaGetLastError());
     }
@@ -511,20 +534,20 @@ int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* ke
 // A key handle is (generation << 12) | slot.  A handle issued before its slot was recycled no longer matches the slot's
 // generation and silently degrades to "no table" (-1): the generic kernel then verifies against the Qx/Qy the caller
 // supplied, so a stale handle can cost speed but never correctness.
-inline int32_t make_handle(const fabgpu_ctx* ctx, int sl) { return (int32_t)(((ctx->slot_gen[sl] & 0x7ffffu) << 12) | (uint32_t)sl); }
-inline int32_t make_small_handle(const fabgpu_ctx* ctx, int sl) { return -2 - (int32_t)(((ctx->small_gen[sl] & 0x3ffu) << 20) | (uint32_t)sl); }
+inline int32_t make_handle(const fabgpu_ctx* ctx, int sl) { return (int32_t)(((ctx->kt->slot_gen[sl] & 0x7ffffu) << 12) | (uint32_t)sl); }
+inline int32_t make_small_handle(const fabgpu_ctx* ctx, int sl) { return -2 - (int32_t)(((ctx->kt->small_gen[sl] & 0x3ffu) << 20) | (uint32_t)sl); }
 // handle -> device code: >= 0 big-table slot, -2 - slot for a live small table, -1 otherwise (no table, stale handle)
 inline int32_t handle_to_slot(const fabgpu_ctx* ctx, int32_t h)
 {
     if (h <= -2) {
         const uint32_t v = (uint32_t)(-2 - h);
         const int sl = (int)(v & 0xfffffu);
-        if (sl >= ctx->small_slots || (v >> 20) != (ctx->small_gen[sl] & 0x3ffu) || !ctx->small_used[sl]) return -1;
+        if (sl >= ctx->kt->small_slots || (v >> 20) != (ctx->kt->small_gen[sl] & 0x3ffu) || !ctx->kt->small_used[sl]) return -1;
         return -2 - sl;
     }
     if (h < 0) return -1;
     const int sl = h & 0xfff;
-    if (sl >= ctx->key_slots || ((uint32_t)h >> 12) != (ctx->slot_gen[sl] & 0x7ffffu) || ctx->slot_key[sl].empty()) return -1;
+    if (sl >= ctx->kt->key_slots || ((uint32_t)h >> 12) != (ctx->kt->slot_gen[sl] & 0x7ffffu) || ctx->kt->slot_key[sl].empty()) return -1;
     return sl;
 }
 
@@ -577,7 +600,9 @@ int wait_slot(fabgpu_ctx* ctx, int slot)
     return FABGPU_OK;
 }
 
-int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batch)
+// with == nullptr: a new group -- the tables are allocated and the generator's is built; otherwise the context joins with's group
+// on with's devices and allocates only its own buffers.
+int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batch, const fabgpu_ctx* with = nullptr)
 {
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
@@ -587,7 +612,8 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
         return FABGPU_E_NO_DEVICE;
     }
     std::vector<int> ids;
-    if (device_ids == nullptr || n_dev <= 0) ids.push_back(0);
+    if (with) for (const auto& dv : with->devs) ids.push_back(dv.id);
+    else if (device_ids == nullptr || n_dev <= 0) ids.push_back(0);
     else ids.assign(device_ids, device_ids + n_dev);
     for (int id : ids)
         if (id < 0 || id >= count) { ctx->last_error = "device id out of range"; return FABGPU_E_NO_DEVICE; }
@@ -598,11 +624,21 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
         const char* ev = getenv("FABGPU_GATE_THREADS");
         int want = ev ? atoi(ev) : std::max(1, std::min(hw > 0 ? hw / 2 : 1, 32));   // gates and block parsing are latency-bound
         ctx->pool.reset(new GatePool(want));
+        const char* sth = getenv("FABGPU_SMALL_THREADS");
+        if (sth) { const int v = atoi(sth); if (v == 64 || v == 128 || v == 256 || v == 512) ctx->small_threads_env = v; }
+        const char* ck = getenv("FABGPU_CACHED_KERNEL");
+        if (ck) ctx->cached_kernel = (ck[0] == 'j' || ck[0] == '0') ? 0 : (ck[0] == 'l' ? (ck[1] == '4' ? 4 : 2) : (ck[0] == 'b' && ck[1] == 'a' && ck[2] == '2' ? 3 : 1));   // "jac" / "0": the Jacobian-chain kernel; "l2" / "l4": its lane-split variant
+    }
+    const bool fresh = with == nullptr;
+    if (!fresh) ctx->kt = with->kt;
+    else {
+        ctx->kt = std::make_shared<KeyTables>();
+        ctx->kt->devs = std::vector<DevTables>(ids.size());   // DevTables is not movable: the vector is built at its final size
         // Per-key tables are 64 MiB each (FAB_WQ = 16), per device.  The request (default 256 = 16 GiB of an H100's 80 GB) is
         // capped so that the tables never take more than half of the smallest device's free memory.
         const char* ks = getenv("FABGPU_KEY_SLOTS");
-        ctx->key_slots = ks ? std::max(1, atoi(ks)) : 256;
-        if (ctx->key_slots > 4096) ctx->key_slots = 4096;     // a handle keeps 12 bits for the slot
+        ctx->kt->key_slots = ks ? std::max(1, atoi(ks)) : 256;
+        if (ctx->kt->key_slots > 4096) ctx->kt->key_slots = 4096;     // a handle keeps 12 bits for the slot
         const size_t per_key = (size_t)FAB_Q_WINDOWS * FAB_Q_ENTRIES * sizeof(aff);
         for (int id : ids) {
             size_t free_b = 0, total_b = 0;
@@ -612,39 +648,35 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             const size_t uses = (size_t)std::count(ids.begin(), ids.end(), id);
             const size_t g_bytes = (size_t)FAB_G_WINDOWS * FAB_G_ENTRIES * sizeof(aff);
             const size_t room = free_b > 2 * g_bytes * uses ? (free_b - 2 * g_bytes * uses) / 2 / uses : 0;
-            ctx->key_slots = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->key_slots, room / per_key));
+            ctx->kt->key_slots = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->kt->key_slots, room / per_key));
         }
-        ctx->slot_key.assign(ctx->key_slots, std::string());
-        ctx->slot_tick.assign(ctx->key_slots, 0ull);
-        ctx->slot_gen.assign(ctx->key_slots, 0u);
+        ctx->kt->slot_key.assign(ctx->kt->key_slots, std::string());
+        ctx->kt->slot_tick.assign(ctx->kt->key_slots, 0ull);
+        ctx->kt->slot_gen.assign(ctx->kt->key_slots, 0u);
         // Small tables (FAB_S_POINTS * 64 bytes = 264 KiB each): default 16 384 of them (4.4 GB); FABGPU_SMALL_SLOTS = 0 turns the tier off.
         const char* ss = getenv("FABGPU_SMALL_SLOTS");
-        ctx->small_slots = ss ? std::max(0, atoi(ss)) : 16384;
-        if (ctx->small_slots > (1 << 20)) ctx->small_slots = 1 << 20;       // a handle keeps 20 bits for the slot
+        ctx->kt->small_slots = ss ? std::max(0, atoi(ss)) : 16384;
+        if (ctx->kt->small_slots > (1 << 20)) ctx->kt->small_slots = 1 << 20;       // a handle keeps 20 bits for the slot
         for (int id : ids) {
             size_t free_b = 0, total_b = 0;
             CK(ctx, cudaSetDevice(id));
             CK(ctx, cudaMemGetInfo(&free_b, &total_b));
             const size_t per_small = (size_t)FAB_S_POINTS * sizeof(aff);
             const size_t uses = (size_t)std::count(ids.begin(), ids.end(), id);
-            ctx->small_slots = (int)std::min<size_t>((size_t)ctx->small_slots, free_b / 8 / uses / per_small);
+            ctx->kt->small_slots = (int)std::min<size_t>((size_t)ctx->kt->small_slots, free_b / 8 / uses / per_small);
         }
-        ctx->small_key.assign(ctx->small_slots, fabgpu_ctx::Key64());
-        ctx->small_used.assign(ctx->small_slots, 0);
-        ctx->small_tick.assign(ctx->small_slots, 0ull);
-        ctx->small_gen.assign(ctx->small_slots, 0u);
-        ctx->small_free.clear();
-        for (int sl = ctx->small_slots - 1; sl >= 0; sl--) ctx->small_free.push_back(sl);
-        ctx->seen_tag.assign((size_t)1 << 18, 0ull); ctx->seen_cnt.assign((size_t)1 << 18, 0u);
-        const char* sth = getenv("FABGPU_SMALL_THREADS");
-        if (sth) { const int v = atoi(sth); if (v == 64 || v == 128 || v == 256 || v == 512) ctx->small_threads_env = v; }
+        ctx->kt->small_key.assign(ctx->kt->small_slots, KeyTables::Key64());
+        ctx->kt->small_used.assign(ctx->kt->small_slots, 0);
+        ctx->kt->small_tick.assign(ctx->kt->small_slots, 0ull);
+        ctx->kt->small_gen.assign(ctx->kt->small_slots, 0u);
+        ctx->kt->small_free.clear();
+        for (int sl = ctx->kt->small_slots - 1; sl >= 0; sl--) ctx->kt->small_free.push_back(sl);
+        ctx->kt->seen_tag.assign((size_t)1 << 18, 0ull); ctx->kt->seen_cnt.assign((size_t)1 << 18, 0u);
         const char* smu = getenv("FABGPU_SMALL_MIN_USES");
-        ctx->small_min_uses = smu ? atoi(smu) : 32;
-        if (ctx->small_slots == 0) ctx->small_min_uses = -1;
+        ctx->kt->small_min_uses = smu ? atoi(smu) : 32;
+        if (ctx->kt->small_slots == 0) ctx->kt->small_min_uses = -1;
         const char* mu = getenv("FABGPU_KEY_MIN_USES");
-        ctx->key_min_uses = mu ? atoi(mu) : 256;           // a table costs about 300 generic verifications to build
-        const char* ck = getenv("FABGPU_CACHED_KERNEL");
-        if (ck) ctx->cached_kernel = (ck[0] == 'j' || ck[0] == '0') ? 0 : (ck[0] == 'l' ? (ck[1] == '4' ? 4 : 2) : (ck[0] == 'b' && ck[1] == 'a' && ck[2] == '2' ? 3 : 1));   // "jac" / "0": the Jacobian-chain kernel; "l2" / "l4": its lane-split variant
+        ctx->kt->key_min_uses = mu ? atoi(mu) : 256;           // a table costs about 300 generic verifications to build
     }
     ctx->dev_cap = round_up32((max_batch + ids.size() - 1) / ids.size());
     ctx->devs = std::vector<Device>(ids.size());          // Device is not movable: the vector is built at its final size
@@ -653,6 +685,7 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
     for (size_t d = 0; d < ids.size(); d++) {
         Device& dv = ctx->devs[d];
         dv.id = ids[d];
+        dv.tab = &ctx->kt->devs[d];
         CK(ctx, cudaSetDevice(dv.id));
         CK(ctx, cudaDeviceGetAttribute(&dv.sms, cudaDevAttrMultiProcessorCount, dv.id));
         {   // Table gathers read 64-byte points at random addresses: by default the L2 fetches 128 bytes around a miss (two sectors'
@@ -663,24 +696,27 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             (void)cudaGetLastError();
         }
         Grow grow{ctx};
-        grow(dv.gtab, tab_entries * sizeof(aff));
-        grow(dv.qtab, (size_t)ctx->key_slots * FAB_Q_WINDOWS * FAB_Q_ENTRIES * sizeof(aff));
-        if (ctx->small_slots > 0) {
-            grow(dv.stab, (size_t)ctx->small_slots * FAB_S_POINTS * sizeof(aff));
-            // build scratch for up to 16 384 keys per registration, allocated once: growing it later costs a cudaFree + cudaMalloc pair in the
-            // middle of traffic (the pair waits for all work in flight)
-            const size_t c = (size_t)std::min(ctx->small_slots, 16384);
-            grow(dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff));
-            grow(dv.s_keys, 64 * c);
-            grow(dv.s_slots, 4 * c);
-        }
-        if (grow.rc) return grow.rc;
         cudaStream_t st = nullptr;
-        CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-        dv.s_stream.reset(st);
-        cudaEvent_t ev = nullptr;
-        CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        dv.s_ev.reset(ev);
+        if (fresh) {
+            dv.tab->id = dv.id;
+            grow(dv.tab->gtab, tab_entries * sizeof(aff));
+            grow(dv.tab->qtab, (size_t)ctx->kt->key_slots * FAB_Q_WINDOWS * FAB_Q_ENTRIES * sizeof(aff));
+            if (ctx->kt->small_slots > 0) {
+                grow(dv.tab->stab, (size_t)ctx->kt->small_slots * FAB_S_POINTS * sizeof(aff));
+                // build scratch for up to 16 384 keys per registration, allocated once: growing it later costs a cudaFree + cudaMalloc pair in the
+                // middle of traffic (the pair waits for all work in flight)
+                const size_t c = (size_t)std::min(ctx->kt->small_slots, 16384);
+                grow(dv.tab->s_bases, c * FAB_S_WINDOWS * sizeof(aff));
+                grow(dv.tab->s_keys, 64 * c);
+                grow(dv.tab->s_slots, 4 * c);
+            }
+            if (grow.rc) return grow.rc;
+            CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+            dv.tab->s_stream.reset(st);
+            cudaEvent_t ev = nullptr;
+            CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+            dv.tab->s_ev.reset(ev);
+        }
         for (auto& ds : dv.slot) {
             CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
             ds.stream.reset(st);
@@ -705,6 +741,7 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             int no = 0;
             CK(ctx, cudaMemPoolSetAttribute(dv.scal_pool.get(), cudaMemPoolReuseAllowInternalDependencies, &no));
         }
+        if (!fresh) continue;
 #if FAB_G_TWO_LEVEL
         {
             DevArray<u256> d_scratch; DevArray<aff> d_small;
@@ -715,13 +752,13 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
             if (grow.rc) return grow.rc;
             small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(nullptr, 1, FAB_WG, FAB_G_WINDOWS, d_small.get(), d_scratch.get(), nullptr);
             const size_t threads2 = (size_t)FAB_G_WINDOWS * ((FAB_G_ENTRIES + FAB_TAB_CHUNK - 1) / FAB_TAB_CHUNK);
-            full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), nullptr, nullptr, 1, FAB_WG, FAB_G_WINDOWS, dv.gtab.get());
+            full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), nullptr, nullptr, 1, FAB_WG, FAB_G_WINDOWS, dv.tab->gtab.get());
             ctx->launches += 2;
             CK(ctx, cudaGetLastError());
             CK(ctx, cudaStreamSynchronize(dv.slot[0].stream.get()));
         }
 #else
-        build_g_table_kernel<<<(unsigned)((tab_entries + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(dv.gtab.get());
+        build_g_table_kernel<<<(unsigned)((tab_entries + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(dv.tab->gtab.get());
         ctx->launches++;
         CK(ctx, cudaGetLastError());
 #endif
@@ -747,12 +784,10 @@ int init_impl(fabgpu_ctx* ctx, const int* device_ids, int n_dev, size_t max_batc
 
 extern "C" {
 
-int fabgpu_init(const int* device_ids, int n_dev, size_t max_batch, fabgpu_ctx** out)
+static int create(const int* device_ids, int n_dev, size_t max_batch, const fabgpu_ctx* with, fabgpu_ctx** out)
 {
-    if (!out) return FABGPU_E_ARG;
-    *out = nullptr;
     fabgpu_ctx* ctx = new fabgpu_ctx();
-    int rc = init_impl(ctx, device_ids, n_dev, max_batch);
+    int rc = init_impl(ctx, device_ids, n_dev, max_batch, with);
     if (rc != FABGPU_OK) {
         g_init_error = ctx->last_error;
         delete ctx;
@@ -760,6 +795,21 @@ int fabgpu_init(const int* device_ids, int n_dev, size_t max_batch, fabgpu_ctx**
     }
     *out = ctx;
     return FABGPU_OK;
+}
+
+int fabgpu_init(const int* device_ids, int n_dev, size_t max_batch, fabgpu_ctx** out)
+{
+    if (!out) return FABGPU_E_ARG;
+    *out = nullptr;
+    return create(device_ids, n_dev, max_batch, nullptr, out);
+}
+
+int fabgpu_init_shared(fabgpu_ctx* with, size_t max_batch, fabgpu_ctx** out)
+{
+    if (!out) return FABGPU_E_ARG;
+    *out = nullptr;
+    if (!with) { g_init_error = "fabgpu_init_shared needs a context to share tables with"; return FABGPU_E_ARG; }
+    return create(nullptr, 0, max_batch, with, out);
 }
 
 void fabgpu_destroy(fabgpu_ctx* ctx)
@@ -792,7 +842,7 @@ int fabgpu_host_buffers(fabgpu_ctx* ctx, int slot, uint8_t** qx, uint8_t** qy, u
 static int verify_async_impl(fabgpu_ctx* ctx, int slot, size_t n, bool keyed)
 {
     if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
-    std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);     // handles -> slots -> enqueue, see fabgpu_ctx::tab_mu
+    std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);     // handles -> slots -> enqueue, see KeyTables
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (n > ctx->max_batch) { ctx->last_error = "n exceeds max_batch"; return FABGPU_E_ARG; }
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
@@ -816,7 +866,7 @@ int fabgpu_host_key_slots(fabgpu_ctx* ctx, int slot, int32_t** key_slot)
     return FABGPU_OK;
 }
 
-int fabgpu_key_slot_capacity(const fabgpu_ctx* ctx) { return ctx ? ctx->key_slots : 0; }
+int fabgpu_key_slot_capacity(const fabgpu_ctx* ctx) { return ctx ? ctx->kt->key_slots : 0; }
 
 // Looks the keys up in the table cache and builds tables for the missing ones (one launch per device for the whole set).
 int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t* slots_out)
@@ -824,38 +874,39 @@ int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t
     if (!ctx || K < 0 || (K && (!keys_xy || !slots_out))) return FABGPU_E_ARG;
     // Fast path under the shared lock: every key already owns a table (the steady state of KeyImport / resolve_key_tables).
     {
-        std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);
-        std::lock_guard<std::mutex> lk(ctx->mu);
+        std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
+        std::lock_guard<std::mutex> lk(ctx->kt->mu);
         bool all = true;
-        for (int k = 0; k < K && all; k++) all = ctx->key_map.count(std::string((const char*)keys_xy + 64 * (size_t)k, 64)) != 0;
+        for (int k = 0; k < K && all; k++) all = ctx->kt->key_map.count(std::string((const char*)keys_xy + 64 * (size_t)k, 64)) != 0;
         if (all) {
-            ctx->tick++;
+            ctx->kt->tick++;
             for (int k = 0; k < K; k++) {
-                const int sl = ctx->key_map[std::string((const char*)keys_xy + 64 * (size_t)k, 64)];
-                slots_out[k] = make_handle(ctx, sl); ctx->slot_tick[sl] = ctx->tick;
+                const int sl = ctx->kt->key_map[std::string((const char*)keys_xy + 64 * (size_t)k, 64)];
+                slots_out[k] = make_handle(ctx, sl); ctx->kt->slot_tick[sl] = ctx->kt->tick;
             }
             return FABGPU_OK;
         }
     }
-    std::unique_lock<std::shared_mutex> wl(ctx->tab_mu);
+    std::unique_lock<std::shared_mutex> wl(ctx->kt->tab_mu);
     std::lock_guard<std::mutex> lk(ctx->mu);
+    std::lock_guard<std::mutex> kl(ctx->kt->mu);
     std::vector<int> fresh;                      // indices into keys_xy that need a table
     std::vector<int32_t> fresh_slot;
-    std::vector<char> slot_taken(ctx->key_slots, 0);
-    ctx->tick++;
+    std::vector<char> slot_taken(ctx->kt->key_slots, 0);
+    ctx->kt->tick++;
     for (int k = 0; k < K; k++) {
         std::string key((const char*)keys_xy + 64 * (size_t)k, 64);
-        auto it = ctx->key_map.find(key);
-        if (it != ctx->key_map.end()) { slots_out[k] = make_handle(ctx, it->second); ctx->slot_tick[it->second] = ctx->tick; slot_taken[it->second] = 1; continue; }
+        auto it = ctx->kt->key_map.find(key);
+        if (it != ctx->kt->key_map.end()) { slots_out[k] = make_handle(ctx, it->second); ctx->kt->slot_tick[it->second] = ctx->kt->tick; slot_taken[it->second] = 1; continue; }
         // least recently used slot that this call has not touched
         int best = -1;
-        for (int sl = 0; sl < ctx->key_slots; sl++)
-            if (!slot_taken[sl] && (best < 0 || ctx->slot_tick[sl] < ctx->slot_tick[best])) best = sl;
+        for (int sl = 0; sl < ctx->kt->key_slots; sl++)
+            if (!slot_taken[sl] && (best < 0 || ctx->kt->slot_tick[sl] < ctx->kt->slot_tick[best])) best = sl;
         if (best < 0) { slots_out[k] = -1; continue; }            // more distinct keys in one call than slots: stays generic
         // The slot's old owner loses it NOW (its handles die with the generation bump), but the new key is mapped only after
         // its table exists on every device: a failure below leaves the slot empty, never pointing at another key's table.
-        if (!ctx->slot_key[best].empty()) { ctx->key_map.erase(ctx->slot_key[best]); ctx->slot_key[best].clear(); ctx->slot_gen[best]++; }
-        ctx->slot_tick[best] = ctx->tick; slot_taken[best] = 1;
+        if (!ctx->kt->slot_key[best].empty()) { ctx->kt->key_map.erase(ctx->kt->slot_key[best]); ctx->kt->slot_key[best].clear(); ctx->kt->slot_gen[best]++; }
+        ctx->kt->slot_tick[best] = ctx->kt->tick; slot_taken[best] = 1;
         slots_out[k] = -1;
         fresh.push_back(k); fresh_slot.push_back(best);
     }
@@ -886,13 +937,13 @@ int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t
         if (grow.rc) return grow.rc;
         small_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(d_keys.get(), F, FAB_WQ, FAB_Q_WINDOWS, d_small.get(), d_scratch.get(), d_flags.get());
         const size_t threads2 = (size_t)F * FAB_Q_WINDOWS * ((FAB_Q_ENTRIES + FAB_TAB_CHUNK - 1) / FAB_TAB_CHUNK);
-        full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), d_slots.get(), d_flags.get(), F, FAB_WQ, FAB_Q_WINDOWS, dv.qtab.get());
+        full_tables_kernel<<<(unsigned)((threads2 + 127) / 128), 128, 0, dv.slot[0].stream.get()>>>(d_small.get(), d_slots.get(), d_flags.get(), F, FAB_WQ, FAB_Q_WINDOWS, dv.tab->qtab.get());
         ctx->launches += 2;
 #else
         const size_t threads = (size_t)F * FAB_Q_WINDOWS;
         grow(d_scratch, threads * 2 * FAB_Q_ENTRIES * sizeof(u256));
         if (grow.rc) return grow.rc;
-        build_key_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(d_keys.get(), d_slots.get(), F, dv.qtab.get(), d_scratch.get(), d_flags.get());
+        build_key_tables_kernel<<<(unsigned)((threads + 31) / 32), 32, 0, dv.slot[0].stream.get()>>>(d_keys.get(), d_slots.get(), F, dv.tab->qtab.get(), d_scratch.get(), d_flags.get());
         ctx->launches++;
 #endif
         CK(ctx, cudaGetLastError());
@@ -908,7 +959,7 @@ int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t
         if (!flags[i]) continue;                  // not a curve point: no table; the generic kernel reports it as off-curve
         const int sl = fresh_slot[i];
         std::string key((const char*)fk.data() + 64 * (size_t)i, 64);
-        ctx->slot_key[sl] = key; ctx->key_map[key] = sl;
+        ctx->kt->slot_key[sl] = key; ctx->kt->key_map[key] = sl;
         slots_out[fresh[i]] = make_handle(ctx, sl);
     }
     return FABGPU_OK;
@@ -919,19 +970,19 @@ int fabgpu_keys_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t
 // Caller holds neither tab_mu nor mu.
 static int small_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_t* handles_out)
 {
-    if (ctx->small_slots <= 0) { for (int k = 0; k < K; k++) handles_out[k] = -1; return FABGPU_OK; }
+    if (ctx->kt->small_slots <= 0) { for (int k = 0; k < K; k++) handles_out[k] = -1; return FABGPU_OK; }
     {   // fast path under the shared lock: every key already owns a small table
-        std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);
-        std::lock_guard<std::mutex> lk(ctx->mu);
+        std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
+        std::lock_guard<std::mutex> lk(ctx->kt->mu);
         bool all = true;
-        fabgpu_ctx::Key64 kk;
-        for (int k = 0; k < K && all; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); all = ctx->small_map.count(kk) != 0; }
+        KeyTables::Key64 kk;
+        for (int k = 0; k < K && all; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); all = ctx->kt->small_map.count(kk) != 0; }
         if (all) {
-            ctx->tick++;
+            ctx->kt->tick++;
             for (int k = 0; k < K; k++) {
                 memcpy(kk.b, keys_xy + 64 * (size_t)k, 64);
-                const int sl = ctx->small_map[kk];
-                handles_out[k] = make_small_handle(ctx, sl); ctx->small_tick[sl] = ctx->tick;
+                const int sl = ctx->kt->small_map[kk];
+                handles_out[k] = make_small_handle(ctx, sl); ctx->kt->small_tick[sl] = ctx->kt->tick;
             }
             return FABGPU_OK;
         }
@@ -940,72 +991,73 @@ static int small_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_
     auto tnow = [] { return std::chrono::steady_clock::now(); };
     auto tus = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
     auto tr0 = tnow();
-    std::unique_lock<std::shared_mutex> wl(ctx->tab_mu);
+    std::unique_lock<std::shared_mutex> wl(ctx->kt->tab_mu);
     std::lock_guard<std::mutex> lk(ctx->mu);
+    std::lock_guard<std::mutex> kl(ctx->kt->mu);
     auto tr1 = tnow();
-    ctx->tick++;
+    ctx->kt->tick++;
     std::vector<int> fresh; std::vector<int32_t> fresh_slot;
-    fabgpu_ctx::Key64 kk;
+    KeyTables::Key64 kk;
     int need = 0;
-    for (int k = 0; k < K; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); if (!ctx->small_map.count(kk)) need++; }
-    if (need > (int)ctx->small_free.size()) {
+    for (int k = 0; k < K; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); if (!ctx->kt->small_map.count(kk)) need++; }
+    if (need > (int)ctx->kt->small_free.size()) {
         // Out of free slots: recycle the least recently used ones in bulk (an eighth of the pool at least), after draining every device --
         // a batch in flight may still read them.  Rare by construction: the pool holds thousands of keys.
         for (auto& dv : ctx->devs) { CK(ctx, cudaSetDevice(dv.id)); CK(ctx, cudaDeviceSynchronize()); }
         std::vector<int> order;
-        for (int sl = 0; sl < ctx->small_slots; sl++) if (ctx->small_used[sl]) order.push_back(sl);
+        for (int sl = 0; sl < ctx->kt->small_slots; sl++) if (ctx->kt->small_used[sl]) order.push_back(sl);
         // keys of THIS call keep their tables
-        for (int k = 0; k < K; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); auto it = ctx->small_map.find(kk); if (it != ctx->small_map.end()) ctx->small_tick[it->second] = ctx->tick; }
-        std::sort(order.begin(), order.end(), [&](int a, int b) { return ctx->small_tick[a] < ctx->small_tick[b]; });
-        const size_t want = std::max<size_t>((size_t)need - ctx->small_free.size(), (size_t)ctx->small_slots / 8);
+        for (int k = 0; k < K; k++) { memcpy(kk.b, keys_xy + 64 * (size_t)k, 64); auto it = ctx->kt->small_map.find(kk); if (it != ctx->kt->small_map.end()) ctx->kt->small_tick[it->second] = ctx->kt->tick; }
+        std::sort(order.begin(), order.end(), [&](int a, int b) { return ctx->kt->small_tick[a] < ctx->kt->small_tick[b]; });
+        const size_t want = std::max<size_t>((size_t)need - ctx->kt->small_free.size(), (size_t)ctx->kt->small_slots / 8);
         for (size_t i = 0; i < order.size() && i < want; i++) {
             const int sl = order[i];
-            if (ctx->small_tick[sl] == ctx->tick) break;
-            ctx->small_map.erase(ctx->small_key[sl]); ctx->small_used[sl] = 0; ctx->small_gen[sl]++;
-            ctx->small_free.push_back(sl); ctx->small_recycled++;
+            if (ctx->kt->small_tick[sl] == ctx->kt->tick) break;
+            ctx->kt->small_map.erase(ctx->kt->small_key[sl]); ctx->kt->small_used[sl] = 0; ctx->kt->small_gen[sl]++;
+            ctx->kt->small_free.push_back(sl); ctx->kt->small_recycled++;
         }
     }
     for (int k = 0; k < K; k++) {
         memcpy(kk.b, keys_xy + 64 * (size_t)k, 64);
-        auto it = ctx->small_map.find(kk);
-        if (it != ctx->small_map.end()) { handles_out[k] = make_small_handle(ctx, it->second); ctx->small_tick[it->second] = ctx->tick; continue; }
+        auto it = ctx->kt->small_map.find(kk);
+        if (it != ctx->kt->small_map.end()) { handles_out[k] = make_small_handle(ctx, it->second); ctx->kt->small_tick[it->second] = ctx->kt->tick; continue; }
         handles_out[k] = -1;
-        if (ctx->small_free.empty()) continue;                      // more distinct keys in one call than the pool holds: stays generic
-        const int sl = ctx->small_free.back(); ctx->small_free.pop_back();
+        if (ctx->kt->small_free.empty()) continue;                      // more distinct keys in one call than the pool holds: stays generic
+        const int sl = ctx->kt->small_free.back(); ctx->kt->small_free.pop_back();
         // mapped at once (a duplicate later in this call finds it); un-mapped again below if the enqueue fails
-        ctx->small_map[kk] = sl; ctx->small_key[sl] = kk; ctx->small_used[sl] = 1; ctx->small_tick[sl] = ctx->tick;
+        ctx->kt->small_map[kk] = sl; ctx->kt->small_key[sl] = kk; ctx->kt->small_used[sl] = 1; ctx->kt->small_tick[sl] = ctx->kt->tick;
         fresh.push_back(k); fresh_slot.push_back(sl);
         handles_out[k] = make_small_handle(ctx, sl);
     }
     if (fresh.empty()) return FABGPU_OK;
     const int F = (int)fresh.size();
-    ctx->small_built += (unsigned long long)F;
+    ctx->kt->small_built += (unsigned long long)F;
     std::vector<uint8_t> fk(64 * (size_t)F);
     for (int i = 0; i < F; i++) memcpy(fk.data() + 64 * (size_t)i, keys_xy + 64 * (size_t)fresh[i], 64);
     auto tr2 = tnow();
     auto build_on = [&](Device& dv) -> int {
         CK(ctx, cudaSetDevice(dv.id));
         auto b0 = tnow();
-        if ((size_t)F > dv.s_cap()) {
-            CK(ctx, cudaStreamSynchronize(dv.s_stream.get()));            // an earlier build may still use the scratch
+        if ((size_t)F > dv.tab->s_cap()) {
+            CK(ctx, cudaStreamSynchronize(dv.tab->s_stream.get()));            // an earlier build may still use the scratch
             const size_t c = (size_t)F + (size_t)F / 2 + 256;
             Grow grow{ctx};
-            grow(dv.s_keys, 64 * c);
-            grow(dv.s_slots, 4 * c);
-            grow(dv.s_bases, c * FAB_S_WINDOWS * sizeof(aff));      // last: it holds s_cap()
+            grow(dv.tab->s_keys, 64 * c);
+            grow(dv.tab->s_slots, 4 * c);
+            grow(dv.tab->s_bases, c * FAB_S_WINDOWS * sizeof(aff));      // last: it holds s_cap()
             if (grow.rc) return grow.rc;
         }
         auto b1 = tnow();
-        CK(ctx, cudaMemcpyAsync(dv.s_keys.get(), fk.data(), fk.size(), cudaMemcpyHostToDevice, dv.s_stream.get()));
-        CK(ctx, cudaMemcpyAsync(dv.s_slots.get(), fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice, dv.s_stream.get()));
-        CK(ctx, cudaStreamSynchronize(dv.s_stream.get()));                // the sources are local vectors
+        CK(ctx, cudaMemcpyAsync(dv.tab->s_keys.get(), fk.data(), fk.size(), cudaMemcpyHostToDevice, dv.tab->s_stream.get()));
+        CK(ctx, cudaMemcpyAsync(dv.tab->s_slots.get(), fresh_slot.data(), 4 * (size_t)F, cudaMemcpyHostToDevice, dv.tab->s_stream.get()));
+        CK(ctx, cudaStreamSynchronize(dv.tab->s_stream.get()));                // the sources are local vectors
         auto b2 = tnow();
-        small_bases_kernel<<<(unsigned)((F + 31) / 32), 32, 0, dv.s_stream.get()>>>(dv.s_keys.get(), dv.s_slots.get(), F, dv.s_bases.get(), dv.stab.get());
-        small_windows_kernel<<<(unsigned)(((size_t)F * FAB_S_WINDOWS + 127) / 128), 128, 0, dv.s_stream.get()>>>(dv.s_bases.get(), dv.s_slots.get(), F, dv.stab.get());
+        small_bases_kernel<<<(unsigned)((F + 31) / 32), 32, 0, dv.tab->s_stream.get()>>>(dv.tab->s_keys.get(), dv.tab->s_slots.get(), F, dv.tab->s_bases.get(), dv.tab->stab.get());
+        small_windows_kernel<<<(unsigned)(((size_t)F * FAB_S_WINDOWS + 127) / 128), 128, 0, dv.tab->s_stream.get()>>>(dv.tab->s_bases.get(), dv.tab->s_slots.get(), F, dv.tab->stab.get());
         ctx->launches += 2;
         CK(ctx, cudaGetLastError());
-        CK(ctx, cudaEventRecord(dv.s_ev.get(), dv.s_stream.get()));
-        dv.s_ev_set = true;
+        CK(ctx, cudaEventRecord(dv.tab->s_ev.get(), dv.tab->s_stream.get()));
+        dv.tab->s_ev_set = true;
         if (trace) fprintf(stderr, "[fabgpu] small_register F=%d: lock %.0f us, bookkeeping %.0f us, scratch %.0f us, copies %.0f us, launches %.0f us\n", F, tus(tr0, tr1),
                            tus(tr1, tr2), tus(b0, b1), tus(b1, b2), tus(b2, tnow()));
         return FABGPU_OK;
@@ -1015,7 +1067,7 @@ static int small_register(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, int32_
         if (rc) {                                                   // nothing usable was built: give the slots back, the keys stay generic
             for (int i = 0; i < F; i++) {
                 const int sl = fresh_slot[i];
-                ctx->small_map.erase(ctx->small_key[sl]); ctx->small_used[sl] = 0; ctx->small_gen[sl]++; ctx->small_free.push_back(sl);
+                ctx->kt->small_map.erase(ctx->kt->small_key[sl]); ctx->kt->small_used[sl] = 0; ctx->kt->small_gen[sl]++; ctx->kt->small_free.push_back(sl);
                 handles_out[fresh[i]] = -1;
             }
             return rc;
@@ -1029,7 +1081,7 @@ int fabgpu_keys_register_small(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, i
     if (!ctx || K < 0 || (K && (!keys_xy || !handles_out))) return FABGPU_E_ARG;
     return small_register(ctx, keys_xy, K, handles_out);
 }
-int fabgpu_small_slot_capacity(const fabgpu_ctx* ctx) { return ctx ? ctx->small_slots : 0; }
+int fabgpu_small_slot_capacity(const fabgpu_ctx* ctx) { return ctx ? ctx->kt->small_slots : 0; }
 void fabgpu_small_table_info(int* window_bits, int* windows, size_t* table_bytes)
 {
     if (window_bits) *window_bits = FAB_WS;
@@ -1039,8 +1091,8 @@ void fabgpu_small_table_info(int* window_bits, int* windows, size_t* table_bytes
 int fabgpu_key_table_stats(fabgpu_ctx* ctx, unsigned long long out[4])
 {
     if (!ctx || !out) return FABGPU_E_ARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    out[0] = ctx->key_map.size(); out[1] = ctx->small_map.size(); out[2] = ctx->small_built; out[3] = ctx->small_recycled;
+    std::lock_guard<std::mutex> lk(ctx->kt->mu);
+    out[0] = ctx->kt->key_map.size(); out[1] = ctx->kt->small_map.size(); out[2] = ctx->kt->small_built; out[3] = ctx->kt->small_recycled;
     return FABGPU_OK;
 }
 
@@ -1264,7 +1316,7 @@ static int bccsp_device_submit(fabgpu_ctx* ctx, int slot, const uint8_t* keys_xy
     const int T = ctx->pool->size();
     bool all_slots = K > 0;
     int classes = K > 0 ? 0 : CLASS_GENERIC;                  // which non-big classes the batch holds (signatures with a bad key index are decided by the gates)
-    std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);      // held until the verify kernel is enqueued: the slots cannot be recycled in between
+    std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);      // held until the verify kernel is enqueued: the slots cannot be recycled in between
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         for (int k = 0; k < K; k++) {
@@ -1335,63 +1387,63 @@ static int bccsp_device_finish(fabgpu_ctx* ctx, int slot, uint8_t* status)
 static int resolve_key_tables(fabgpu_ctx* ctx, const uint8_t* keys_xy, int K, const int32_t* key_idx, size_t n, std::vector<int32_t>& slot_of)
 {
     slot_of.assign(K > 0 ? K : 0, -1);
-    if (!(K > 0 && keys_xy && ctx->key_min_uses >= 0)) return FABGPU_OK;
+    if (!(K > 0 && keys_xy && ctx->kt->key_min_uses >= 0)) return FABGPU_OK;
     std::vector<uint32_t> uses(K, 0);
     for (size_t i = 0; i < n; i++) if (key_idx[i] >= 0 && key_idx[i] < K) uses[key_idx[i]]++;
     std::vector<int> want_big, want_small;
     {
-        std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        fabgpu_ctx::Key64 kk;
+        std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
+        std::lock_guard<std::mutex> lk(ctx->kt->mu);
+        KeyTables::Key64 kk;
         bool touched = false;
         static thread_local std::string kbuf(64, '\0');          // lookup key without a heap allocation per key
         for (int k = 0; k < K; k++) {
             if (!uses[k]) continue;
-            if (!ctx->key_map.empty() || uses[k] >= (uint32_t)ctx->key_min_uses) {
+            if (!ctx->kt->key_map.empty() || uses[k] >= (uint32_t)ctx->kt->key_min_uses) {
                 memcpy(&kbuf[0], keys_xy + 64 * (size_t)k, 64);
-                auto it = ctx->key_map.find(kbuf);
-                if (it != ctx->key_map.end()) {
-                    if (!touched) { ctx->tick++; touched = true; }
-                    slot_of[k] = make_handle(ctx, it->second); ctx->slot_tick[it->second] = ctx->tick; continue;
+                auto it = ctx->kt->key_map.find(kbuf);
+                if (it != ctx->kt->key_map.end()) {
+                    if (!touched) { ctx->kt->tick++; touched = true; }
+                    slot_of[k] = make_handle(ctx, it->second); ctx->kt->slot_tick[it->second] = ctx->kt->tick; continue;
                 }
             }
-            if (uses[k] >= (uint32_t)ctx->key_min_uses) { want_big.push_back(k); continue; }
-            if (ctx->small_min_uses < 0) continue;
+            if (uses[k] >= (uint32_t)ctx->kt->key_min_uses) { want_big.push_back(k); continue; }
+            if (ctx->kt->small_min_uses < 0) continue;
             memcpy(kk.b, keys_xy + 64 * (size_t)k, 64);
-            auto sm = ctx->small_map.find(kk);
-            if (sm != ctx->small_map.end()) {
-                if (!touched) { ctx->tick++; touched = true; }
-                slot_of[k] = make_small_handle(ctx, sm->second); ctx->small_tick[sm->second] = ctx->tick; continue;
+            auto sm = ctx->kt->small_map.find(kk);
+            if (sm != ctx->kt->small_map.end()) {
+                if (!touched) { ctx->kt->tick++; touched = true; }
+                slot_of[k] = make_small_handle(ctx, sm->second); ctx->kt->small_tick[sm->second] = ctx->kt->tick; continue;
             }
             uint32_t total = uses[k];
-            if (total < (uint32_t)ctx->small_min_uses) {
+            if (total < (uint32_t)ctx->kt->small_min_uses) {
                 uint64_t h0, h1;
                 memcpy(&h0, kk.b + 8, 8); memcpy(&h1, kk.b + 40, 8);
                 const uint64_t tag = ((h0 * 0x9E3779B97F4A7C15ull) ^ (h1 * 0xC2B2AE3D27D4EB4Full)) | 1ull;
-                const size_t b0 = (size_t)(tag >> 20) & (ctx->seen_tag.size() - 1) & ~(size_t)3;   // bucket of four entries
+                const size_t b0 = (size_t)(tag >> 20) & (ctx->kt->seen_tag.size() - 1) & ~(size_t)3;   // bucket of four entries
                 size_t at = b0, weakest = b0;
                 bool found = false;
                 for (size_t q = b0; q < b0 + 4 && !found; q++) {
-                    if (ctx->seen_tag[q] == tag) { at = q; found = true; }
-                    else if (ctx->seen_tag[q] == 0) { if (ctx->seen_tag[weakest] != 0) weakest = q; }
-                    else if (ctx->seen_tag[weakest] != 0 && ctx->seen_cnt[q] < ctx->seen_cnt[weakest]) weakest = q;
+                    if (ctx->kt->seen_tag[q] == tag) { at = q; found = true; }
+                    else if (ctx->kt->seen_tag[q] == 0) { if (ctx->kt->seen_tag[weakest] != 0) weakest = q; }
+                    else if (ctx->kt->seen_tag[weakest] != 0 && ctx->kt->seen_cnt[q] < ctx->kt->seen_cnt[weakest]) weakest = q;
                 }
-                if (!found) { at = weakest; ctx->seen_tag[at] = tag; ctx->seen_cnt[at] = 0; }      // an empty entry, else the least used one
-                ctx->seen_cnt[at] += uses[k];
-                total = ctx->seen_cnt[at];
-                if (total >= (uint32_t)ctx->small_min_uses) { ctx->seen_tag[at] = 0; ctx->seen_cnt[at] = 0; }
+                if (!found) { at = weakest; ctx->kt->seen_tag[at] = tag; ctx->kt->seen_cnt[at] = 0; }      // an empty entry, else the least used one
+                ctx->kt->seen_cnt[at] += uses[k];
+                total = ctx->kt->seen_cnt[at];
+                if (total >= (uint32_t)ctx->kt->small_min_uses) { ctx->kt->seen_tag[at] = 0; ctx->kt->seen_cnt[at] = 0; }
             }
-            if (total >= (uint32_t)ctx->small_min_uses) want_small.push_back(k);
+            if (total >= (uint32_t)ctx->kt->small_min_uses) want_small.push_back(k);
         }
     }
-    if (!want_big.empty() && (int)want_big.size() <= ctx->key_slots) {
+    if (!want_big.empty() && (int)want_big.size() <= ctx->kt->key_slots) {
         std::vector<uint8_t> wk(64 * want_big.size());
         std::vector<int32_t> ws(want_big.size(), -1);
         for (size_t i = 0; i < want_big.size(); i++) memcpy(wk.data() + 64 * i, keys_xy + 64 * (size_t)want_big[i], 64);
         int rc = fabgpu_keys_register(ctx, wk.data(), (int)want_big.size(), ws.data());
         if (rc) return rc;
         for (size_t i = 0; i < want_big.size(); i++) slot_of[want_big[i]] = ws[i];
-    } else if (ctx->small_min_uses >= 0) {
+    } else if (ctx->kt->small_min_uses >= 0) {
         for (int k : want_big) want_small.push_back(k);              // more busy keys than big slots: the small tier takes them
     }
     if (!want_small.empty()) {
@@ -1723,6 +1775,7 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
     dm.classes = 0;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
+        std::lock_guard<std::mutex> kl(ctx->kt->mu);
         for (int i = 0; i < n_ids; i++) {
             raw_slot[i] = handle_to_slot(ctx, ctx->identity_slot[i]);
             if (raw_slot[i] < 0) { dm.all_slots = false; dm.classes |= raw_slot[i] == -1 ? CLASS_GENERIC : CLASS_SMALL; }
@@ -1752,14 +1805,14 @@ static int msp_small_tier(fabgpu_ctx* ctx, const uint8_t* keys_xy, int n_ids)
 {
     int rc = small_register(ctx, keys_xy, n_ids, ctx->identity_slot.data());
     if (rc) return rc;
-    std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);
+    std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (ctx->key_map.empty()) return FABGPU_OK;
+    if (ctx->kt->key_map.empty()) return FABGPU_OK;
     std::string kbuf(64, '\0');
     for (int i = 0; i < n_ids; i++) {
         memcpy(&kbuf[0], keys_xy + 64 * (size_t)i, 64);
-        auto it = ctx->key_map.find(kbuf);
-        if (it != ctx->key_map.end()) ctx->identity_slot[i] = make_handle(ctx, it->second);
+        auto it = ctx->kt->key_map.find(kbuf);
+        if (it != ctx->kt->key_map.end()) ctx->identity_slot[i] = make_handle(ctx, it->second);
     }
     return FABGPU_OK;
 }
@@ -1841,7 +1894,7 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
     }
     // identities are long-lived: give every key a table now (what KeyImport does when the MSP deserialises an identity)
     // An MSP with more identities than big-table slots (client certificates) puts them in the small tier instead.
-    if (n_ids > 0 && n_ids <= ctx->key_slots) {
+    if (n_ids > 0 && n_ids <= ctx->kt->key_slots) {
         int rc = fabgpu_keys_register(ctx, keys_xy, n_ids, ctx->identity_slot.data());
         if (rc) return rc;
     } else if (n_ids > 0) {
@@ -2859,10 +2912,10 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     auto& bb = ctx->bbs[slot]; auto& db = ctx->dbs[slot]; auto& dm = ctx->dm;
     db.t0 = now();
     CK(ctx, cudaSetDevice(dv.id));
-    // Identities' key tables may have been recycled by other registrations since fabgpu_msp_configure: re-issue them.  From the
-    // check to the last enqueue of this block the slot table is held shared (fabgpu_ctx::tab_mu): a concurrent
-    // fabgpu_keys_register waits, so dm.key_slot's raw slots stay the tables of these identities for the whole launch sequence.
-    std::shared_lock<std::shared_mutex> rl(ctx->tab_mu);
+    // Identities' key tables may have been recycled by other registrations since fabgpu_msp_configure, in this context or another of
+    // its group: re-issue them.  From the check to the last enqueue of this block the slot table is held shared (KeyTables::tab_mu): a
+    // concurrent fabgpu_keys_register in any context of the group waits, so dm.key_slot's raw slots stay the tables of these identities for the whole launch sequence.
+    std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
     {
         auto any_stale = [&] {
             std::lock_guard<std::mutex> lk(ctx->mu);
@@ -2873,7 +2926,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
         if (any_stale()) {
             rl.unlock();
             const int n_ids = (int)ctx->identity_slot.size();
-            const bool big = n_ids <= ctx->key_slots;
+            const bool big = n_ids <= ctx->kt->key_slots;
             int rc = big ? fabgpu_keys_register(ctx, ctx->msp.keys_xy.data(), n_ids, ctx->identity_slot.data())     // exclusive; drains every stream first
                          : msp_small_tier(ctx, ctx->msp.keys_xy.data(), n_ids);
             if (rc) return rc;
@@ -3240,8 +3293,9 @@ int fabgpu_test_couch_values(fabgpu_ctx* ctx, const uint8_t* blob, const uint32_
 
 int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* window, const uint32_t* digit, size_t n, uint8_t* out)
 {
-    if (!ctx || !window || !digit || !out || key_slot >= ctx->key_slots) return FABGPU_E_ARG;
-    std::lock_guard<std::mutex> lk(ctx->mu);            // a small slot cannot be recycled, nor a new build enqueued, until the copy-back
+    if (!ctx || !window || !digit || !out || key_slot >= ctx->kt->key_slots) return FABGPU_E_ARG;
+    std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);    // no context of the group recycles a slot, nor enqueues a build, until the copy-back
+    std::lock_guard<std::mutex> lk(ctx->mu);
     Device& dv = ctx->devs[0];
     const aff* tab;
     int windows;
@@ -3249,12 +3303,12 @@ int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* win
     if (key_slot <= -2) {
         const int32_t code = handle_to_slot(ctx, key_slot);
         if (code == -1) return FABGPU_E_ARG;            // stale handle, or the slot is no longer in use
-        tab = dv.stab.get() + (size_t)(-2 - code) * FAB_S_POINTS;
+        tab = dv.tab->stab.get() + (size_t)(-2 - code) * FAB_S_POINTS;
         windows = FAB_S_WINDOWS; stride = dmax = FAB_S_HALF;
     } else if (key_slot == -1) {
-        tab = dv.gtab.get(); windows = FAB_G_WINDOWS; stride = dmax = FAB_G_ENTRIES;
+        tab = dv.tab->gtab.get(); windows = FAB_G_WINDOWS; stride = dmax = FAB_G_ENTRIES;
     } else {
-        tab = dv.qtab.get() + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES; windows = FAB_Q_WINDOWS; stride = dmax = FAB_Q_ENTRIES;
+        tab = dv.tab->qtab.get() + (size_t)key_slot * FAB_Q_WINDOWS * FAB_Q_ENTRIES; windows = FAB_Q_WINDOWS; stride = dmax = FAB_Q_ENTRIES;
     }
     for (size_t i = 0; i < n; i++)
         if (window[i] >= (uint32_t)windows || digit[i] == 0 || digit[i] > dmax) return FABGPU_E_ARG;
@@ -3267,7 +3321,7 @@ int fabgpu_test_table_entries(fabgpu_ctx* ctx, int key_slot, const uint32_t* win
     CK(ctx, cudaMemcpy(d_w.get(), window, 4 * n, cudaMemcpyHostToDevice));
     CK(ctx, cudaMemcpy(d_d.get(), digit, 4 * n, cudaMemcpyHostToDevice));
     // small tables are built on s_stream, which the legacy stream does not wait for: read only after the last build
-    if (dv.s_ev_set) CK(ctx, cudaStreamWaitEvent(0, dv.s_ev.get(), 0));
+    if (dv.tab->s_ev_set) CK(ctx, cudaStreamWaitEvent(0, dv.tab->s_ev.get(), 0));
     table_entries_kernel<<<(unsigned)((n + 127) / 128), 128>>>(tab, stride, d_w.get(), d_d.get(), (uint32_t)n, d_out.get());
     ctx->launches++;
     CK(ctx, cudaGetLastError());

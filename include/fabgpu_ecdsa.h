@@ -63,6 +63,24 @@ enum {
  * slot (FABGPU_SLOTS slots), and builds the table on the device.  A batch given to the host-buffer entry points
  * is split into contiguous, 32-aligned ranges across the context's devices. */
 int fabgpu_init(const int* device_ids, int n_dev, size_t max_batch, fabgpu_ctx** out);
+/* Creates a context on `with`'s devices that shares `with`'s point tables and key caches: one context per channel of a peer, all in
+ * one GROUP, without a second copy of any table.  The group shares the generator's fixed-base table, the window-table pool (key -> slot
+ * map, LRU order, generations, the per-key signature counts that earn tables) and the small-table pool, with the capacities and the
+ * FABGPU_KEY_MIN_USES / FABGPU_SMALL_MIN_USES settings read when the group's first context was made; nothing is built here.  The new
+ * context owns, exactly as one from fabgpu_init does: its slots, streams, pinned and device batch buffers, gate and block buffers, the
+ * MSP view and every policy table, the capability, the tx-id set, the state table and state-database kind, the peer-exchange state,
+ * its last error, its launch count and its FABGPU_CACHED_KERNEL choice.
+ *   - handles from fabgpu_keys_register{,_small} are valid in every context of the group; a stale handle still costs speed, never
+ *     correctness.
+ *   - fabgpu_key_slot_capacity, fabgpu_small_slot_capacity and fabgpu_key_table_stats report the group's pools, and fabgpu_msp_configure
+ *     compares an MSP's size against the group's window-table capacity.
+ *   - recycling is least-recently-used across the group: a registration in one context may recycle a table another context's MSP or
+ *     batch uses, and that context registers the key again on its next block (as it does after a recycling in its own context).
+ *     Size FABGPU_KEY_SLOTS for the busy endorsers of all channels together.
+ *   - with == NULL: FABGPU_E_ARG and *out = NULL.  max_batch follows fabgpu_init's rules.  `with` may itself have been made by this
+ *     call: the new context joins the same group.  Contexts of a group may be destroyed in any order; the shared tables go with the
+ *     last of them. */
+int fabgpu_init_shared(fabgpu_ctx* with, size_t max_batch, fabgpu_ctx** out);
 void fabgpu_destroy(fabgpu_ctx* ctx);
 /* Last error text of this context (or of the failed fabgpu_init when ctx == NULL). Never NULL. */
 const char* fabgpu_last_error(const fabgpu_ctx* ctx);
