@@ -35,6 +35,7 @@ EXPORTS = [
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info", "fabgpu_committed_txids_add_block",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
+    "fabgpu_validate_pvtdata",
 ]
 
 
@@ -551,6 +552,20 @@ class Context:
         self._ck(lib().fabgpu_validate_mvcc(self._h, ctypes.c_int(slot), ctypes.c_uint64(block_num), _p(tv if tv.size else flags), _p(flags),
                                             ctypes.c_size_t(tv.shape[0])))
         return flags[: tv.shape[0]]
+
+    def validate_pvtdata(self, slot, flags, pvt):
+        """The private-data check of the block validate_wait(slot) returned (fabgpu_validate_pvtdata): flags are the block's final flags,
+        pvt maps SeqInBlock -> marshalled rwset.TxPvtReadWriteSet.  Returns (verdict, status): verdict = (code, seq, ns, coll) with code 0
+        OK, 1 mismatch, 254; status[seq] = (code, ns, coll) per entry, code 0 OK, 1 mismatch, 2 skipped, 254."""
+        fl = np.ascontiguousarray(np.asarray(flags, np.uint8))
+        seqs = sorted(pvt)
+        blob, off = _blob([bytes(pvt[k]) for k in seqs])
+        sq = np.array(seqs or [0], np.uint32)
+        st = np.zeros(3 * max(len(seqs), 1), np.int32)
+        out = np.zeros(4, np.int32)
+        self._ck(lib().fabgpu_validate_pvtdata(self._h, ctypes.c_int(slot), _p(fl if fl.size else out), ctypes.c_size_t(fl.shape[0]), _p(blob), _p(off),
+                                               _p(sq), ctypes.c_size_t(len(seqs)), _p(st), _p(out)))
+        return tuple(int(x) for x in out), {k: tuple(int(x) for x in st[3 * i:3 * i + 3]) for i, k in enumerate(seqs)}
 
     def _state_versions(self, fn, entries, height, extra):
         b = lambda x: x.encode() if isinstance(x, str) else bytes(x)

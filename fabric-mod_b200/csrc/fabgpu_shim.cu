@@ -31,6 +31,7 @@
 #include "txidset.hpp"
 #include "stateset.hpp"
 #include "couchval.cuh"
+#include "pvtdata.cuh"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -280,12 +281,21 @@ struct fabgpu_ctx {
         // the block in flight on this slot (fabgpu_validate_*_async .. fabgpu_validate_wait)
         bool busy = false, on_device = false, use_ev = false, kl_on = false, v13 = false; size_t T = 0, W_cap = 0; const uint8_t* block = nullptr;
         bool mvcc_ready = false;                 // fabgpu_validate_wait returned the block and its bytes are still on the device
+        bool pvt_ready = false;                  // the same, for fabgpu_validate_pvtdata: fabgpu_validate_mvcc leaves it set
         uint8_t txid_block = 0;                  // fabgpu_committed_txids_add_block: 0 no block submitted, 1 submitted, 2 its ids added
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
     } dbs[FABGPU_SLOTS];
     std::mutex blk_mu[FABGPU_SLOTS];
+    // fabgpu_validate_pvtdata of a slot's block (pvtdata.cuh), on the slot's stream under blk_mu[slot]: pinned staging of the private
+    // data, flags and entry tables, and the stage's arrays
+    struct PvtBufs {
+        HostArray<uint8_t> h_blob, h_flags; HostArray<uint32_t> h_off, h_seq, h_ctr; HostArray<int32_t> h_status; HostArray<unsigned long long> h_verdict;
+        DevArray<uint8_t> d_blob, d_flags, d_ent, d_dig; DevArray<uint32_t> d_off, d_seq, d_first, d_n, d_ctr; DevArray<int32_t> d_status;
+        DevArray<unsigned long long> d_verdict; DevArray<bdev::PvRec> d_rec; DevArray<bdev::ShaJobP> d_jobs;
+        uint32_t rec_hint = PV_REC_HINT;                                                 // collection records per entry the arrays are sized for
+    } pvt[FABGPU_SLOTS];
     // fabgpu_committed_txids: the ledger's tx ids on device 0 (txidset.cuh); ledger state, so fabgpu_msp_configure keeps it.  A mutation runs
     // on `stream` under slot0_mu: it first waits for every slot's last block_decide_kernel (decide_ev) -- blocks submitted before it never
     // see it -- and records `ev`, which every later block_submit makes its decide stage wait for.  The host never waits for an add (that
@@ -2886,6 +2896,94 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     return FABGPU_OK;
 }
 
+// The private-data check of the slot's block, on the slot's stream under blk_mu[slot] only (no table is read or written):
+//   H2D private data, entry tables, flags -> pv_scan_kernel (per entry: collection records, SHA-256 jobs) -> host reads the record count
+//   (grows the arrays and runs the scan again on overflow) -> sha256_segments_kernel (per record: its rwset) -> pv_check_kernel (per
+//   record: the public hash, the decode) -> pv_verdict_kernel (per entry: its outcome, atomicMin of the deciding entry) -> D2H.
+int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
+                            const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4])
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS || !out) return FABGPU_E_ARG;
+    if ((n && !flags) || (n_pvt && (!pvt_off || !seq || !status))) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    for (size_t i = 0; i < n_pvt; i++) if (pvt_off[i + 1] < pvt_off[i]) { ctx->last_error = "private-data offsets decrease"; return FABGPU_E_ARG; }
+    const size_t bytes = n_pvt ? pvt_off[n_pvt] : 0;
+    if (bytes && !pvt_blob) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    if (n_pvt > UINT32_MAX || bytes > UINT32_MAX - 64) { ctx->last_error = "too much private data for one call"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    auto& db = ctx->dbs[slot]; auto& p = ctx->pvt[slot];
+    if (db.busy || !db.pvt_ready) { ctx->last_error = "the slot holds no finished block: fabgpu_validate_wait first"; return FABGPU_E_ARG; }
+    if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
+    {
+        std::vector<uint8_t> seen(n, 0);
+        for (size_t i = 0; i < n_pvt; i++) {
+            if (seq[i] >= n) { ctx->last_error = "a seq is not below the block's transaction count"; return FABGPU_E_ARG; }
+            if (seen[seq[i]]++) { ctx->last_error = "a seq is given twice"; return FABGPU_E_ARG; }
+        }
+    }
+    out[0] = bdev::PV_OK; out[1] = out[2] = out[3] = -1;
+    if (n_pvt == 0) return FABGPU_OK;
+    const uint32_t E = (uint32_t)n_pvt, T = (uint32_t)n;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    Grow grow{ctx};
+    // slack: the SHA-256 loader reads the aligned words past a range's end
+    grow(p.h_blob, bytes + 64); grow(p.h_flags, T); grow(p.h_off, 4 * ((size_t)E + 1)); grow(p.h_seq, 4 * (size_t)E); grow(p.h_ctr, 16);
+    grow(p.h_status, 12 * (size_t)E); grow(p.h_verdict, 8);
+    grow(p.d_blob, bytes + 64); grow(p.d_flags, T); grow(p.d_off, 4 * ((size_t)E + 1)); grow(p.d_seq, 4 * (size_t)E); grow(p.d_ent, E);
+    grow(p.d_first, 4 * (size_t)E); grow(p.d_n, 4 * (size_t)E); grow(p.d_ctr, 16); grow(p.d_status, 12 * (size_t)E); grow(p.d_verdict, 8);
+    if (grow.rc) return grow.rc;
+    memcpy(p.h_blob.get(), pvt_blob, bytes); memset(p.h_blob.get() + bytes, 0, 64);
+    memcpy(p.h_flags.get(), flags, n); memcpy(p.h_off.get(), pvt_off, 4 * ((size_t)E + 1)); memcpy(p.h_seq.get(), seq, 4 * (size_t)E);
+    CK(ctx, cudaMemcpyAsync(p.d_blob.get(), p.h_blob.get(), bytes + 64, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(p.d_flags.get(), p.h_flags.get(), n, cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(p.d_off.get(), p.h_off.get(), 4 * ((size_t)E + 1), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(p.d_seq.get(), p.h_seq.get(), 4 * (size_t)E, cudaMemcpyHostToDevice, st));
+    const uint8_t* blk = ctx->bbs[slot].d_block.get();
+    bdev::PvArrays a;
+    a.pvt = p.d_blob.get(); a.off = p.d_off.get(); a.seq = p.d_seq.get(); a.n_pvt = E; a.flags = p.d_flags.get(); a.ent = p.d_ent.get();
+    a.first = p.d_first.get(); a.n_rec = p.d_n.get(); a.ctr = p.d_ctr.get(); a.status = p.d_status.get(); a.verdict = p.d_verdict.get();
+    uint32_t R = 0;
+    for (;;) {
+        const size_t R_cap = (size_t)E * p.rec_hint;
+        if (R_cap > UINT32_MAX) { ctx->last_error = "too many collections for one call"; return FABGPU_E_ARG; }
+        Grow g2{ctx};
+        g2(p.d_rec, R_cap * sizeof(bdev::PvRec)); g2(p.d_jobs, R_cap * sizeof(bdev::ShaJobP)); g2(p.d_dig, 32 * R_cap);
+        if (g2.rc) return g2.rc;
+        a.rec = p.d_rec.get(); a.R_cap = (uint32_t)R_cap; a.jobs = p.d_jobs.get(); a.dig = p.d_dig.get();
+        CK(ctx, cudaMemsetAsync(p.d_ctr.get(), 0, 16, st));
+        bdev::pv_scan_kernel<<<(E + 63) / 64, 64, 0, st>>>(blk, db.d_txs.get(), a);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(p.h_ctr.get(), p.d_ctr.get(), 4, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        R = p.h_ctr.get()[0];
+        if (R <= R_cap) break;
+        p.rec_hint = (uint32_t)((R + E - 1) / E) + 1;                   // later calls are sized for it too
+    }
+    if (R) {
+        sha256_segments_kernel<<<(R + 127) / 128, 128, 0, st>>>(p.d_blob.get(), reinterpret_cast<const ShaJob*>(p.d_jobs.get()), R, p.d_dig.get());
+        bdev::pv_check_kernel<<<(R + 127) / 128, 128, 0, st>>>(blk, db.d_txs.get(), a, R);
+        ctx->launches += 2;
+    }
+    CK(ctx, cudaMemsetAsync(p.d_verdict.get(), 0xff, 8, st));
+    bdev::pv_verdict_kernel<<<(E + 127) / 128, 128, 0, st>>>(a);
+    ctx->launches++;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpyAsync(p.h_status.get(), p.d_status.get(), 12 * (size_t)E, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(p.h_verdict.get(), p.d_verdict.get(), 8, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    memcpy(status, p.h_status.get(), 12 * (size_t)E);
+    const unsigned long long v = p.h_verdict.get()[0];
+    if (v != ~0ull) {                                          // the deciding entry: a mismatch when its flag is VALID, else 254
+        const uint32_t e = (uint32_t)v, s = (uint32_t)(v >> 32);
+        const int32_t* es = status + 3 * (size_t)e;
+        const bool mismatch = es[0] == bdev::PV_MISMATCH && flags[s] == bdev::TXC_VALID;
+        out[0] = mismatch ? bdev::PV_MISMATCH : bdev::PV_UNDET; out[1] = (int32_t)s;
+        out[2] = mismatch ? es[1] : -1; out[3] = mismatch ? es[2] : -1;
+    }
+    return FABGPU_OK;
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -3152,7 +3250,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     auto& db = ctx->dbs[slot];
     if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-    db.mvcc_ready = false; db.txid_block = 0;
+    db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 0;
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
     int rc;
     {
@@ -3178,7 +3276,7 @@ int fabgpu_validate_envelopes_async(fabgpu_ctx* ctx, int slot, const uint8_t* bl
         std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
         auto& db = ctx->dbs[slot];
         if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false; db.txid_block = 1;
+        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 1;
         return FABGPU_OK;
     }
     return validate_submit(ctx, slot, blob, env_off[n_env], env_off, n_env);
@@ -3198,7 +3296,7 @@ int fabgpu_validate_wait(fabgpu_ctx* ctx, int slot, uint8_t* flags, size_t flags
         return FABGPU_E_ARG;
     }
     const int rc = db.on_device ? block_finish(ctx, slot, flags) : FABGPU_OK;      // (an empty envelope list: nothing ran)
-    db.mvcc_ready = rc == FABGPU_OK;
+    db.mvcc_ready = db.pvt_ready = rc == FABGPU_OK;
     return rc;
 }
 

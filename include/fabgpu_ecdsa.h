@@ -473,6 +473,31 @@ int fabgpu_state_index_info(const fabgpu_ctx* ctx, unsigned long long out[3]);
  *       removing it. */
 enum { FABGPU_STATEDB_LEVELDB = 0, FABGPU_STATEDB_COUCHDB = 1 };
 int fabgpu_state_database(fabgpu_ctx* ctx, int kind);
+/* The ledger's private-data check (validateAndPreparePvtBatch, core/ledger/kvledger/txmgmt/validation/batch_preparer.go:119-188), an
+ * opt-in stage after the flags are final: every collection of the private data the caller holds is hashed and compared with the
+ * pvt_rwset_hash of the block's public read/write set, and its rwset is decoded as a KVRWSet, on the device.
+ *   The private data is one marshalled rwset.TxPvtReadWriteSet per transaction (ledger.TxPvtData.WriteSet, the rwset bytes unchanged):
+ *   entry i is pvt_blob[pvt_off[i] .. pvt_off[i+1]) with SeqInBlock seq[i].  flags are the block's n final flags (those of
+ *   TRANSACTIONS_FILTER: fabgpu_validate_mvcc's output, or the caller's once some 254s are settled).
+ *   status[3i .. 3i+2] receives entry i's outcome as if its transaction were VALID, with the namespace and collection index (in the
+ *   entry's order) where it was decided, -1 where none:
+ *     0 OK; 1 mismatch: SHA-256(rwset) differs from retrieveHash(namespace, collection) (types.go:62-78) -- the first such collection
+ *     in order, every hash of the entry being checked before any rwset is decoded; 2 skipped: no collection of the public set carries
+ *     a pvt_rwset_hash (containsPvtWrites, types.go:49-58); 254: an rwset that does not decode (a level the project's reader refuses, a
+ *     string that is not UTF-8), outer levels that do not parse, a transaction whose read/write set the walk never reached (a
+ *     non-endorser transaction included), or one whose only public hashes are present but empty while the entry holds a collection.
+ *   out = {code, seq, ns, coll}: the block's verdict from the entry with the smallest seq whose outcome is 1 or 254 and whose flag is
+ *     VALID or 254 (other flags are ignored, :133-135): 1 with its (seq, ns, coll) when its flag is VALID and it mismatches -- the
+ *     reference fails the block's commit -- else 254 with its seq (ns = coll = -1); 0 with seq = ns = coll = -1 when no entry decides.
+ *   Call it any number of times after fabgpu_validate_wait(slot) (or a blocking fabgpu_validate_block / _envelopes, slot 0) returned
+ *   the block and before the slot's next submit, whether or not fabgpu_validate_mvcc ran.  It runs on the slot's stream under the
+ *   slot's lock only, touches no table, and returns with the stream synchronised; the caller's arrays are not referenced afterwards.
+ *   FABGPU_E_ARG, with a fabgpu_last_error text and nothing enqueued, for a slot without a finished block, n other than the block's
+ *   transaction count, a seq >= n or given twice, NULL arrays with a count > 0, and decreasing offsets.
+ *   Not restated: the private update batch, incrementPvtdataVersionIfNeeded, the gossip coordinator's filtering, eligibility and
+ *   missing-data bookkeeping. */
+int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
+                            const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4]);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
