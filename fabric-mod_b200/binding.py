@@ -35,7 +35,7 @@ EXPORTS = [
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info", "fabgpu_committed_txids_add_block",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
-    "fabgpu_validate_pvtdata",
+    "fabgpu_validate_pvtdata", "fabgpu_msp_identities_add", "fabgpu_block_unknown_identities",
 ]
 
 
@@ -179,6 +179,7 @@ class Context:
         if rc != OK:
             raise FabGpuError(rc, (L.fabgpu_last_error(None) or b"").decode())
         self.max_batch = max_batch
+        self._last_block = {}               # slot -> the bytes its last block was submitted in (block_unknown_identities)
 
     def close(self):
         if self._h:
@@ -419,6 +420,7 @@ class Context:
         roots = np.array([policies[n] for n in names] or [0], np.int32)
         self._ck(lib().fabgpu_namespace_policies(self._h, _p(nb), _p(no), _p(roots), ctypes.c_int(len(names))))
         self._ns_names = names
+        self._n_principals = len(principals)
 
     def channel_capability(self, cap):
         """cap: CAP_V2_0 (the default after msp_configure) for a channel with V2_0Validation, CAP_V1_3 for a V1_3 / V1_4_2 / V1_4_3
@@ -440,6 +442,49 @@ class Context:
         words = np.ascontiguousarray(pack_principal_bits(b)).reshape(-1)
         words = words if words.size else np.zeros(1, np.uint32)
         self._ck(lib().fabgpu_msp_principal_bits(self._h, _p(words), ctypes.c_int(b.shape[0]), ctypes.c_int(b.shape[1])))
+
+    def msp_identities_add(self, identities, groups=None, bits=None):
+        """Admits identities into the table msp_configure installed, without draining the blocks in flight (fabgpu_msp_identities_add):
+        seen by every block submitted after this returns, by none submitted before.  identities: list of (serialized, mspid, key_xy,
+        valid) as for msp_configure.  groups: one de-duplication id each, required iff a group table is installed (msp_configure
+        installs one; identity_groups over the whole table gives consistent ids); bits: bool [n, n_principals], required iff
+        principal bits are installed."""
+        idb, ido = _blob([bytes(i[0]) for i in identities])
+        mb, mo = _blob([i[1].encode() for i in identities])
+        keys = np.ascontiguousarray(np.frombuffer(b"".join(bytes(i[2]) for i in identities) or b"\x00" * 64, np.uint8))
+        valid = np.array([1 if i[3] else 0 for i in identities] or [0], np.uint8)
+        g = None if groups is None else np.ascontiguousarray(np.asarray(list(groups) or [0], np.int32))
+        if g is not None and identities and g.shape[0] != len(identities):
+            raise ValueError("one group per identity")
+        w = None
+        if bits is not None:
+            # the library reads one row of the configured principals' width per identity
+            b = np.asarray(bits, dtype=bool)
+            n_pr = getattr(self, "_n_principals", 0)
+            if b.size == 0 and not identities:
+                b = np.zeros((0, n_pr), bool)
+            if b.ndim != 2 or b.shape != (len(identities), n_pr):
+                raise ValueError("bits must be a [n_identities, n_principals] array over msp_configure's %d principals" % n_pr)
+            w = np.ascontiguousarray(pack_principal_bits(b)).reshape(-1)
+            w = w if w.size else np.zeros(1, np.uint32)
+        self._ck(lib().fabgpu_msp_identities_add(self._h, _p(idb), _p(ido), _p(mb), _p(mo), _p(keys), _p(valid), _p(g), _p(w),
+                                                 ctypes.c_int(len(identities))))
+
+    def block_unknown_identities(self, slot):
+        """The identities the finished block on `slot` looked up and did not find (fabgpu_block_unknown_identities), distinct, in order
+        of first appearance: [(serialized bytes, first tx)].  Call it between validate_wait(slot) and the slot's next submit; the
+        block's bytes must still be alive (they are read back from the buffer the block was submitted in)."""
+        n, cap = ctypes.c_size_t(0), 1024
+        while True:
+            out = np.zeros(3 * cap, np.uint32)
+            self._ck(lib().fabgpu_block_unknown_identities(self._h, ctypes.c_int(slot), _p(out), ctypes.c_size_t(cap), ctypes.byref(n)))
+            if n.value <= cap:
+                break
+            cap = n.value
+        src = self._last_block.get(slot)
+        if src is None:
+            raise FabGpuError(E_ARG, "no block submitted on this slot through this binding")
+        return [(bytes(src[int(out[3 * i]): int(out[3 * i]) + int(out[3 * i + 1])]), int(out[3 * i + 2])) for i in range(n.value)]
 
     def collection_policies(self, table):
         """table: {(namespace, collection): root node index} -- the endorsement policy a write to that private-data collection is checked
@@ -590,6 +635,7 @@ class Context:
         n_env = env_off.shape[0] - 1
         self._inflight = getattr(self, "_inflight", {})
         self._inflight[slot] = (arr, env_off)
+        self._last_block[slot] = arr
         self._ck(lib().fabgpu_validate_envelopes_async(self._h, ctypes.c_int(slot), _p(arr), _p(env_off), ctypes.c_size_t(n_env)))
         return n_env
 
@@ -597,6 +643,7 @@ class Context:
         arr = np.frombuffer(block, np.uint8) if isinstance(block, (bytes, bytearray)) else block
         self._inflight = getattr(self, "_inflight", {})
         self._inflight[slot] = (arr,)
+        self._last_block[slot] = arr
         self._ck(lib().fabgpu_validate_block_async(self._h, ctypes.c_int(slot), _p(arr), ctypes.c_size_t(arr.shape[0])))
         return max(16, arr.shape[0] // 2)
 
@@ -612,6 +659,7 @@ class Context:
     def validate_block(self, block, max_tx=None):
         """block: bytes or a uint8 numpy array (e.g. a slice of block_buffer()).  Returns the TRANSACTIONS_FILTER bytes."""
         arr = np.frombuffer(block, np.uint8) if isinstance(block, (bytes, bytearray)) else block
+        self._last_block[0] = arr
         cap = max_tx or max(16, arr.shape[0] // 64)
         flags = np.full(cap, 254, np.uint8)
         n = ctypes.c_size_t(0)
@@ -623,6 +671,7 @@ class Context:
         arr = np.frombuffer(blob, np.uint8) if isinstance(blob, (bytes, bytearray)) else blob
         env_off = np.ascontiguousarray(env_off, dtype=np.uint32)
         n_env = env_off.shape[0] - 1
+        self._last_block[0] = arr
         flags = np.full(max(n_env, 1), 254, np.uint8)
         n = ctypes.c_size_t(0)
         self._ck(lib().fabgpu_validate_envelopes(self._h, _p(arr), _p(env_off), ctypes.c_size_t(n_env), _p(flags), ctypes.c_size_t(max(n_env, 1)),

@@ -114,6 +114,15 @@ kp_scatter_kernel(KpSlot* __restrict__ slots, const uint32_t* __restrict__ idx, 
     if (i < n) slots[idx[i]] = val[i];
 }
 
+// fabgpu_msp_identities_add: writes the changed slots of the MSP table's identity index (hash and identity of each)
+__global__ void __launch_bounds__(256)
+msp_scatter_kernel(uint64_t* __restrict__ ht_hash, int32_t* __restrict__ ht_idx, const uint32_t* __restrict__ pos, const uint64_t* __restrict__ hash,
+                   const int32_t* __restrict__ idx, uint32_t n)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) { ht_hash[pos[i]] = hash[i]; ht_idx[pos[i]] = idx[i]; }
+}
+
 // ---- bccsp-level batch with the gates on the device (SURVEY.md section 8f rank 3) ------------------------------------------
 // One thread per signature: sw.CSP.Verify's argument gates (bccsp/sw/impl.go:249-257), UnmarshalECDSASignature + IsLowS
 // (bccsp/utils/ecdsa.go:43-92) and hashToInt, straight from the raw DER / digest blobs.  pre[i] = 0 hands the signature to

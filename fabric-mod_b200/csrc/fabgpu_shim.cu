@@ -32,6 +32,8 @@
 #include "stateset.hpp"
 #include "couchval.cuh"
 #include "pvtdata.cuh"
+#include "msptable.hpp"
+#include "unknownids.cuh"
 #include "ecdsa_kernels.cuh"
 
 #if defined(__SSE2__)
@@ -143,6 +145,25 @@ struct HostSlot {
     HostArray<int32_t> h_key_slot;
 };
 
+// A device array of the MSP table (fabgpu_ctx::DevMsp), allocated and freed in stream order on the MSP stream (fabgpu_ctx::MspAdmit):
+// fabgpu_msp_identities_add grows it while blocks in flight still read the old one -- those keep the pointer they were launched with,
+// and the free runs after them (msp_grow).  The destructor's cudaFree runs once every reader has finished (the context is drained).
+template <typename T>
+struct MspArr {
+    T* p = nullptr; size_t cap = 0;
+    MspArr() = default;
+    MspArr(MspArr&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    MspArr& operator=(MspArr&& o) noexcept
+    {
+        if (this != &o) { if (p) cudaFree(p); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); }
+        return *this;
+    }
+    ~MspArr() { if (p) cudaFree(p); }
+    T* get() const { return p; }
+    size_t bytes() const { return cap; }
+    void drop(cudaStream_t st) { if (p) cudaFreeAsync(p, st); p = nullptr; cap = 0; }
+};
+
 }  // namespace
 
 // Minimal fork-join pool for the host gates (DER parse + packing is ~40 ns/signature single-threaded, which would
@@ -227,30 +248,52 @@ struct fabgpu_ctx {
     std::vector<std::string> principals;
     std::string channel;
     std::vector<int32_t> identity_slot;
+    // per identity: the key tier its table handle was issued in, and is re-issued in when recycled -- TIER_WINDOW (fabgpu_keys_register)
+    // or TIER_SMALL (msp_small_tier)
+    std::vector<uint8_t> identity_tier;
     struct BlockBufs {
         DevArray<uint8_t> d_block;
         HostArray<uint8_t> h_block;                               // optional pinned staging the caller may fill directly
     } bbs[FABGPU_SLOTS];
     double block_timing[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // host phases [0..4] (see fabgpu_block_timing), device stages [5..9]
     // device-side copy of the MSP view / policy (block_plan_kernel, block_decide_kernel)
+    // The identity arrays and the index are MspArr: grown by fabgpu_msp_identities_add with blocks in flight (capacity doubling).
     struct DevMsp {
-        DevArray<uint8_t> id_blob, valid, keys_xy, channel;
-        DevArray<uint32_t> id_off; DevArray<int32_t> key_slot, msp_code, ht_idx, nodes, principal_code;
-        DevArray<int32_t> group;                                      // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
+        MspArr<uint8_t> id_blob, valid, keys_xy; DevArray<uint8_t> channel;
+        MspArr<uint32_t> id_off; MspArr<int32_t> key_slot, msp_code, ht_idx; DevArray<int32_t> nodes, principal_code;
+        MspArr<int32_t> group;                                        // de-duplication groups (fabgpu_msp_identity_groups), null = identity index
+        bool configured = false;                                      // fabgpu_msp_configure installed this table
+        msptab::Mirror mirror;                                        // host copy of id_blob / id_off / ht_hash / ht_idx
+        std::unordered_map<std::string, int32_t> codes;               // MSP id -> msp_code, identities and principals alike
         DevArray<uint8_t> ns_blob; DevArray<uint32_t> ns_off; DevArray<int32_t> ns_root; int32_t n_ns = 0;    // fabgpu_namespace_policies
         std::vector<int32_t> ns_root_host;                            // the same roots, for the v1.3 mode's ImplicitMeta check
         uint8_t mode = BD_MODE_V20;                       // fabgpu_channel_capability
         DevArray<uint8_t> ver_blob; DevArray<uint32_t> ver_off;       // fabgpu_namespace_versions, null = none
-        DevArray<uint32_t> pbits; int32_t pbits_words = 0;            // fabgpu_msp_principal_bits, null = MSP-id member matching
+        MspArr<uint32_t> pbits; int32_t pbits_words = 0;              // fabgpu_msp_principal_bits, null = MSP-id member matching
         DevArray<uint8_t> cp_ns_blob, cp_name_blob; DevArray<uint32_t> cp_ns_off, cp_name_off;   // fabgpu_collection_policies, cp_size = 0: none
         DevArray<int32_t> cp_root, cp_idx; DevArray<uint64_t> cp_hash; uint32_t cp_size = 0;
         // fabgpu_key_policies: slots, entry bytes, and the table's nodes after the configured ones in `nodes`; kp_size = 0: none.
         // kp_idx / kp_val stage the changed slots of an update.
         DevArray<bdev::KpSlot> kp_slots, kp_val; DevArray<uint8_t> kp_blob; DevArray<uint32_t> kp_idx; uint32_t kp_size = 0; int32_t kp_n_nodes = 0;
         bool nodes_lost = false;                                      // a failed key-table call lost the configured nodes: no blocks
-        DevArray<uint64_t> ht_hash; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
+        MspArr<uint64_t> ht_hash; uint32_t ht_size = 0; int32_t n_ids = 0, n_nodes = 0, n_principals = 0; uint32_t channel_len = 0;
         bool all_slots = true; int classes = 0;                    // which non-big classes the identities' keys fall in (CLASS_*)
     } dm;
+    // fabgpu_msp_identities_add: the MSP stream (every DevMsp identity array is allocated, copied and freed on it) and the ordering of
+    // admissions, as for the committed tx-id set.  An add runs on `stream` under slot0_mu: it first waits for every slot's last
+    // block_decide_kernel (TxidSet::decide_ev, shared) -- blocks submitted before it never see it -- and records `ev`, which every later
+    // block_submit makes its first block_resolve_kernel wait for.  The pinned staging buffers rotate, each guarded by its own event, so the
+    // host never waits for an add.  `admitted`: an identity was added since the last fabgpu_msp_configure (submits then record decide_ev).
+    struct MspAdmit {
+        static constexpr int RING = 4;
+        Stream stream; Event ev; bool ev_set = false, admitted = false;
+        HostArray<uint8_t> h_stage[RING]; Event stage_ev[RING]; bool stage_set[RING] = {}; unsigned seq = 0;
+    } adm;
+    // fabgpu_block_unknown_identities of a slot's block (unknownids.cuh), on the slot's stream under blk_mu[slot]
+    struct UkBufs {
+        DevArray<uint64_t> d_hash; DevArray<uint32_t> d_index, d_rep, d_cnt, d_out; DevArray<unsigned long long> d_first;
+        HostArray<uint32_t> h_cnt, h_out;
+    } uk[FABGPU_SLOTS];
     bdev::KeyPolicyTable kpt;                                      // host mirror of the key policy table
     std::atomic<uint32_t> kl_hint{BD_WRITES_HINT};                 // write records per transaction the block slots are sized for; grows on overflow
     struct GateBufs {                          // fabgpu_bccsp_verify_batch with device-side gates
@@ -372,6 +415,28 @@ struct Grow {
     template <typename A> void operator()(A& a, size_t bytes) { if (rc == FABGPU_OK) rc = a.reserve(ctx, bytes); else a = A(); }
 };
 
+// Makes `a` hold at least `need` bytes (plus 8 of slack: word-wise readers may touch the aligned word past the end), keeping its first
+// `keep` bytes: a larger array (at least twice the old capacity) is allocated and copied in stream order on st.  The old array is freed
+// there too, or, with `retire`, handed over to be freed later (after the stream has waited for the blocks that still read it).
+// fresh: reallocate even when the array is large enough.
+template <typename T>
+static int msp_grow(fabgpu_ctx* ctx, MspArr<T>& a, cudaStream_t st, size_t need, size_t keep, std::vector<void*>* retire = nullptr,
+                    bool fresh = false)
+{
+    need += 8;
+    if (need <= a.cap && !fresh) return FABGPU_OK;
+    const size_t cap = std::max(need, 2 * a.cap);
+    void* p = nullptr;
+    CK(ctx, cudaMallocAsync(&p, cap, st));
+    if (keep && cudaMemcpyAsync(p, a.p, keep, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
+        cudaFreeAsync(p, st); ctx->last_error = "MSP table copy failed"; return FABGPU_E_CUDA;
+    }
+    if (retire) { if (a.p) retire->push_back(a.p); a.p = nullptr; a.cap = 0; }
+    else a.drop(st);
+    a.p = static_cast<T*>(p); a.cap = cap;
+    return FABGPU_OK;
+}
+
 bool fault_injected()
 {
     const char* v = getenv("FABGPU_FAULT_INJECT");
@@ -439,6 +504,7 @@ unsigned small_threads(const fabgpu_ctx* ctx, const Device& dv, size_t n, bool b
 }
 // classes (mode 2 with scratch): which of the non-big classes the batch may contain -- a class the caller knows to be absent is not launched.
 enum { CLASS_SMALL = 1, CLASS_GENERIC = 2 };
+enum : uint8_t { TIER_WINDOW = 0, TIER_SMALL = 1 };    // fabgpu_ctx::identity_tier
 // n_dev / n_base (block path): the batch is [0, min(n, n_base + *n_dev)) with *n_dev written by an earlier kernel of the stream.
 int launch_verify(fabgpu_ctx* ctx, const Device& dv, int mode, const int32_t* key_slot, const uint8_t* qx, const uint8_t* qy,
                   const uint8_t* e, const uint8_t* r, const uint8_t* s, size_t n, uint32_t* mask, uint32_t* off, cudaStream_t st,
@@ -1755,6 +1821,42 @@ int fabgpu_bccsp_verify(fabgpu_ctx* ctx, const uint8_t* key_xy, const uint8_t* s
 
 // ---- block-level pre-pass -------------------------------------------------------------------------------------------
 
+// The MSP stream (fabgpu_ctx::MspAdmit), created on first use on device 0 of the context
+static int msp_stream(fabgpu_ctx* ctx, cudaStream_t* out)
+{
+    auto& a = ctx->adm;
+    if (!a.stream) {
+        cudaStream_t st = nullptr; cudaEvent_t ev = nullptr;
+        CK(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); a.stream.reset(st);
+        CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); a.ev.reset(ev);
+        for (auto& e : a.stage_ev) { cudaEvent_t x = nullptr; CK(ctx, cudaEventCreateWithFlags(&x, cudaEventDisableTiming)); e.reset(x); }
+    }
+    *out = a.stream.get();
+    return FABGPU_OK;
+}
+
+// Raw table slots of identities [i0, i1) from their handles, and the classes they add (DevMsp::all_slots / classes)
+static void msp_raw_slots(fabgpu_ctx* ctx, int i0, int i1, int32_t* raw)
+{
+    auto& dm = ctx->dm;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::lock_guard<std::mutex> kl(ctx->kt->mu);
+    for (int i = i0; i < i1; i++) {
+        raw[i - i0] = handle_to_slot(ctx, ctx->identity_slot[i]);
+        if (raw[i - i0] < 0) { dm.all_slots = false; dm.classes |= raw[i - i0] == -1 ? CLASS_GENERIC : CLASS_SMALL; }
+    }
+}
+
+static int32_t msp_code_of(fabgpu_ctx* ctx, const std::string& mspid)
+{
+    auto& codes = ctx->dm.codes;
+    auto it = codes.find(mspid);
+    if (it != codes.end()) return it->second;
+    const int32_t c = (int32_t)codes.size();
+    codes[mspid] = c;
+    return c;
+}
+
 // Device copy of the MSP view and the policy for block_plan_kernel / block_decide_kernel (device 0 of the context).
 static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* keys_xy, const uint8_t* valid, int n_ids,
                       const int32_t* policy_nodes, int n_nodes)
@@ -1762,58 +1864,57 @@ static int upload_msp(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* i
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& dm = ctx->dm;
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
-    // blocks already enqueued on a slot were launched with the OLD tables (passed by value): let them finish before those go away
+    cudaStream_t ms = nullptr;
+    if (int rc = msp_stream(ctx, &ms)) return rc;
+    // blocks already enqueued on a slot were launched with the OLD tables (passed by value), and admissions may still be copying into
+    // them: let both finish before those go away
     for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
+    CK(ctx, cudaStreamSynchronize(ms));
     dm = fabgpu_ctx::DevMsp();
+    ctx->adm.admitted = ctx->adm.ev_set = false;
     ctx->kpt = bdev::KeyPolicyTable();                       // its SignedBy nodes index the principals being replaced
-    // MSP-id codes: equal strings <=> equal codes, shared between identities and policy principals
-    std::unordered_map<std::string, int32_t> codes;
-    auto code_of = [&](const std::string& sname) { auto it = codes.find(sname); if (it != codes.end()) return it->second; int32_t c = (int32_t)codes.size(); codes[sname] = c; return c; };
+    // MSP-id codes: equal strings <=> equal codes, shared between identities and policy principals; kept for later admissions
     std::vector<int32_t> msp_code(n_ids > 0 ? n_ids : 1, -1), pcode(ctx->principals.size() ? ctx->principals.size() : 1, -1);
-    for (int i = 0; i < n_ids; i++) msp_code[i] = code_of(ctx->msp.mspid[i]);
-    for (size_t i = 0; i < ctx->principals.size(); i++) pcode[i] = code_of(ctx->principals[i]);
-    uint32_t hsz = 8; while (hsz < (uint32_t)(4 * n_ids + 8)) hsz <<= 1;
-    std::vector<uint64_t> hh(hsz, 0); std::vector<int32_t> hi(hsz, -1);
-    for (int i = 0; i < n_ids; i++) {
-        const uint64_t hv = bdev::sample_hash(id_blob + id_off[i], id_off[i + 1] - id_off[i]);
-        uint32_t pos = (uint32_t)hv & (hsz - 1);
-        while (hh[pos] != 0) pos = (pos + 1) & (hsz - 1);
-        hh[pos] = hv; hi[pos] = i;
-    }
+    for (int i = 0; i < n_ids; i++) msp_code[i] = msp_code_of(ctx, ctx->msp.mspid[i]);
+    for (size_t i = 0; i < ctx->principals.size(); i++) pcode[i] = msp_code_of(ctx, ctx->principals[i]);
+    dm.mirror.configure(id_blob, id_off, n_ids);
+    const uint32_t hsz = dm.mirror.size();
     dm.all_slots = true;
     std::vector<int32_t> raw_slot(n_ids > 0 ? n_ids : 1, -1);
     dm.classes = 0;
-    {
-        std::lock_guard<std::mutex> lk(ctx->mu);
-        std::lock_guard<std::mutex> kl(ctx->kt->mu);
-        for (int i = 0; i < n_ids; i++) {
-            raw_slot[i] = handle_to_slot(ctx, ctx->identity_slot[i]);
-            if (raw_slot[i] < 0) { dm.all_slots = false; dm.classes |= raw_slot[i] == -1 ? CLASS_GENERIC : CLASS_SMALL; }
-        }
-    }
+    msp_raw_slots(ctx, 0, n_ids, raw_slot.data());
     auto up = [&](auto& dst, const void* src, size_t bytes) -> int {
         if (int rc = dst.reserve(ctx, bytes + 8)) return rc;   // slack: word-wise readers may touch the aligned word past the end
         if (bytes) CK(ctx, cudaMemcpy(dst.get(), src, bytes, cudaMemcpyHostToDevice));
         return FABGPU_OK;
     };
+    auto up_ms = [&](auto& dst, const void* src, size_t bytes) -> int {
+        if (int rc = msp_grow(ctx, dst, ms, bytes, 0)) return rc;
+        if (bytes) CK(ctx, cudaMemcpyAsync(dst.get(), src, bytes, cudaMemcpyHostToDevice, ms));
+        return FABGPU_OK;
+    };
     const size_t blob_len = n_ids ? id_off[n_ids] : 0;
-    if (up(dm.id_blob, id_blob, blob_len) || up(dm.id_off, id_off, 4 * (size_t)(n_ids + 1) * (n_ids ? 1 : 0)) || up(dm.valid, valid, (size_t)n_ids) ||
-        up(dm.keys_xy, keys_xy, 64 * (size_t)n_ids) || up(dm.key_slot, raw_slot.data(), 4 * (size_t)n_ids) ||
-        up(dm.msp_code, msp_code.data(), 4 * (size_t)n_ids) || up(dm.ht_hash, hh.data(), 8 * (size_t)hsz) || up(dm.ht_idx, hi.data(), 4 * (size_t)hsz) ||
+    if (up_ms(dm.id_blob, id_blob, blob_len) || up_ms(dm.id_off, id_off, 4 * (size_t)(n_ids + 1) * (n_ids ? 1 : 0)) || up_ms(dm.valid, valid, (size_t)n_ids) ||
+        up_ms(dm.keys_xy, keys_xy, 64 * (size_t)n_ids) || up_ms(dm.key_slot, raw_slot.data(), 4 * (size_t)n_ids) ||
+        up_ms(dm.msp_code, msp_code.data(), 4 * (size_t)n_ids) || up_ms(dm.ht_hash, dm.mirror.ht_hash.data(), 8 * (size_t)hsz) ||
+        up_ms(dm.ht_idx, dm.mirror.ht_idx.data(), 4 * (size_t)hsz) ||
         up(dm.nodes, policy_nodes, 16 * (size_t)n_nodes) || up(dm.principal_code, pcode.data(), 4 * ctx->principals.size()) ||
         up(dm.channel, ctx->channel.data(), ctx->channel.size()))
         return FABGPU_E_CUDA;
+    CK(ctx, cudaStreamSynchronize(ms));                      // the sources are the caller's and local vectors
     dm.ht_size = n_ids ? hsz : 0; dm.n_ids = n_ids; dm.n_nodes = n_nodes; dm.n_principals = (int32_t)ctx->principals.size();
     dm.channel_len = (uint32_t)ctx->channel.size();
+    dm.configured = true;
     return FABGPU_OK;
 }
 
 
-// An MSP with more identities than window-table slots: every identity gets a small table; the ones whose key ALREADY owns a window table --
-// the integrator registered the few busy ones (the endorsing peers) with fabgpu_keys_register beforehand -- keep using that.
-static int msp_small_tier(fabgpu_ctx* ctx, const uint8_t* keys_xy, int n_ids)
+// Small tables for identities: every identity gets a small table; the ones whose key ALREADY owns a window table -- the integrator
+// registered the few busy ones (the endorsing peers) with fabgpu_keys_register beforehand -- keep using that.  The tier of an MSP with more
+// identities than window-table slots, and of every admitted identity.
+static int msp_small_tier(fabgpu_ctx* ctx, const uint8_t* keys_xy, int n_ids, int32_t* handles)
 {
-    int rc = small_register(ctx, keys_xy, n_ids, ctx->identity_slot.data());
+    int rc = small_register(ctx, keys_xy, n_ids, handles);
     if (rc) return rc;
     std::shared_lock<std::shared_mutex> rl(ctx->kt->tab_mu);
     std::lock_guard<std::mutex> lk(ctx->mu);
@@ -1822,7 +1923,7 @@ static int msp_small_tier(fabgpu_ctx* ctx, const uint8_t* keys_xy, int n_ids)
     for (int i = 0; i < n_ids; i++) {
         memcpy(&kbuf[0], keys_xy + 64 * (size_t)i, 64);
         auto it = ctx->kt->key_map.find(kbuf);
-        if (it != ctx->kt->key_map.end()) ctx->identity_slot[i] = make_handle(ctx, it->second);
+        if (it != ctx->kt->key_map.end()) handles[i] = make_handle(ctx, it->second);
     }
     return FABGPU_OK;
 }
@@ -1901,6 +2002,7 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
             ctx->principals.emplace_back((const char*)principal_blob + principal_off[i], principal_off[i + 1] - principal_off[i]);
         ctx->channel = channel_id;
         ctx->identity_slot.assign(n_ids, -1);
+        ctx->identity_tier.assign(n_ids, n_ids <= ctx->kt->key_slots ? TIER_WINDOW : TIER_SMALL);
     }
     // identities are long-lived: give every key a table now (what KeyImport does when the MSP deserialises an identity)
     // An MSP with more identities than big-table slots (client certificates) puts them in the small tier instead.
@@ -1908,17 +2010,18 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
         int rc = fabgpu_keys_register(ctx, keys_xy, n_ids, ctx->identity_slot.data());
         if (rc) return rc;
     } else if (n_ids > 0) {
-        int rc = msp_small_tier(ctx, keys_xy, n_ids);             // also with the small tier off or too small: pre-registered window tables are still picked up
+        int rc = msp_small_tier(ctx, keys_xy, n_ids, ctx->identity_slot.data());      // also with the small tier off or too small: pre-registered window tables are still picked up
         if (rc) return rc;
     }
     return upload_msp(ctx, id_blob, id_off, keys_xy, valid, n_ids, policy_nodes, n_nodes);
 }
 
-// drains the block slots' streams: kernels already enqueued keep reading the tables they were launched with
+// drains the block slots' streams and the MSP stream: kernels already enqueued keep reading the tables they were launched with
 static int drain_block_streams(fabgpu_ctx* ctx)
 {
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
     for (auto& ds : ctx->devs[0].slot) CK(ctx, cudaStreamSynchronize(ds.stream.get()));
+    if (ctx->adm.stream) CK(ctx, cudaStreamSynchronize(ctx->adm.stream.get()));
     return FABGPU_OK;
 }
 
@@ -1927,12 +2030,14 @@ int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids)
     if (!ctx || n_ids < 0 || (n_ids && !group)) return FABGPU_E_ARG;
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& dm = ctx->dm;
-    if (n_ids != dm.n_ids) { ctx->last_error = "group table does not match the identities given to fabgpu_msp_configure"; return FABGPU_E_ARG; }
+    if (n_ids != dm.n_ids) { ctx->last_error = "group table does not match the identities the MSP table holds"; return FABGPU_E_ARG; }
     int rc = drain_block_streams(ctx); if (rc) return rc;
     dm.group = {};
     if (n_ids == 0) return FABGPU_OK;
-    if ((rc = dm.group.reserve(ctx, 4 * (size_t)n_ids))) return rc;
-    CK(ctx, cudaMemcpy(dm.group.get(), group, 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
+    cudaStream_t ms = nullptr;
+    if ((rc = msp_stream(ctx, &ms)) || (rc = msp_grow(ctx, dm.group, ms, 4 * (size_t)n_ids, 0))) return rc;
+    CK(ctx, cudaMemcpyAsync(dm.group.get(), group, 4 * (size_t)n_ids, cudaMemcpyHostToDevice, ms));
+    CK(ctx, cudaStreamSynchronize(ms));
     return FABGPU_OK;
 }
 
@@ -1942,7 +2047,7 @@ int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, 
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& dm = ctx->dm;
     if (n_ids && (n_ids != dm.n_ids || n_principals != dm.n_principals)) {
-        ctx->last_error = "principal bits do not match the identities and principals given to fabgpu_msp_configure";
+        ctx->last_error = "principal bits do not match the identities the MSP table holds and the principals given to fabgpu_msp_configure";
         return FABGPU_E_ARG;
     }
     int rc = drain_block_streams(ctx); if (rc) return rc;
@@ -1950,9 +2055,149 @@ int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, 
     if (n_ids == 0) return FABGPU_OK;
     const int W = (n_principals + 31) / 32;
     const size_t bytes = 4 * (size_t)n_ids * W;
-    if ((rc = dm.pbits.reserve(ctx, bytes + 8))) return rc;     // non-null even with no principals: it selects the bit test
-    if (bytes) CK(ctx, cudaMemcpy(dm.pbits.get(), bits, bytes, cudaMemcpyHostToDevice));
+    cudaStream_t ms = nullptr;
+    if ((rc = msp_stream(ctx, &ms)) || (rc = msp_grow(ctx, dm.pbits, ms, bytes, 0))) return rc;     // non-null even with no principals: it selects the bit test
+    if (bytes) CK(ctx, cudaMemcpyAsync(dm.pbits.get(), bits, bytes, cudaMemcpyHostToDevice, ms));
+    CK(ctx, cudaStreamSynchronize(ms));
     dm.pbits_words = W;
+    return FABGPU_OK;
+}
+
+// A failed admission may have left the device table half written: from here on no lookup finds an identity (every transaction is 254)
+// until fabgpu_msp_configure installs a table again.  The host's per-identity state goes back to the n0 identities the device arrays
+// are known to hold, so that the stale-handle re-issue in block_submit never writes past them.
+static int msp_admit_fail(fabgpu_ctx* ctx, int rc, int n0)
+{
+    ctx->dm.ht_size = 0; ctx->dm.configured = false;
+    ctx->identity_slot.resize(n0); ctx->identity_tier.resize(n0);
+    ctx->msp.serialized.resize(n0); ctx->msp.mspid.resize(n0); ctx->msp.keys_xy.resize(64 * (size_t)n0); ctx->msp.valid.resize(n0);
+    ctx->last_error += " (the MSP table is lost until fabgpu_msp_configure installs one)";
+    return rc;
+}
+
+int fabgpu_msp_identities_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* mspid_blob, const uint32_t* mspid_off,
+                              const uint8_t* keys_xy, const uint8_t* valid, const int32_t* group, const uint32_t* bits, int n)
+{
+    if (!ctx) return FABGPU_E_ARG;
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& dm = ctx->dm; auto& a = ctx->adm;
+    if (!dm.configured) { ctx->last_error = "no MSP table: call fabgpu_msp_configure first"; return FABGPU_E_ARG; }
+    if (const char* err = dm.mirror.check_add(id_blob, id_off, mspid_blob, mspid_off, keys_xy, valid, group, bits, n, dm.group.get() != nullptr,
+                                              dm.pbits.get() != nullptr)) {
+        ctx->last_error = err; return FABGPU_E_ARG;
+    }
+    if (n > INT32_MAX - dm.n_ids) { ctx->last_error = "too many identities"; return FABGPU_E_ARG; }
+    if (n == 0) return FABGPU_OK;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t ms = nullptr;
+    if (int rc = msp_stream(ctx, &ms)) return rc;
+    // key tables first: nothing of the table has changed if this fails
+    std::vector<int32_t> handles(n, -1);
+    if (int rc = msp_small_tier(ctx, keys_xy, n, handles.data())) return rc;
+    const int n0 = dm.n_ids, n1 = n0 + n;
+    const size_t W = (size_t)dm.pbits_words;
+    // host side: the mirrors, the MSP-id codes and the new index slots
+    ctx->identity_slot.insert(ctx->identity_slot.end(), handles.begin(), handles.end());
+    ctx->identity_tier.resize(n1, TIER_SMALL);
+    std::vector<int32_t> raw(n), code(n);
+    msp_raw_slots(ctx, n0, n1, raw.data());
+    for (int i = 0; i < n; i++) {
+        std::string mspid((const char*)mspid_blob + mspid_off[i], mspid_off[i + 1] - mspid_off[i]);
+        code[i] = msp_code_of(ctx, mspid);
+        ctx->msp.add(id_blob + id_off[i], id_off[i + 1] - id_off[i]);
+        ctx->msp.mspid.push_back(std::move(mspid));
+    }
+    ctx->msp.keys_xy.insert(ctx->msp.keys_xy.end(), keys_xy, keys_xy + 64 * (size_t)n);
+    ctx->msp.valid.insert(ctx->msp.valid.end(), valid, valid + n);
+    const size_t blob0 = dm.mirror.blob.size();
+    std::vector<uint32_t> dirty;
+    const bool full = dm.mirror.add(id_blob, id_off, n, dirty);
+    const uint32_t hsz = dm.mirror.size();
+    // One pinned staging buffer: the appended rows, then the index (whole, or the changed slots: position, hash, identity).  Offsets
+    // from n0 + 1 (from 0 for an empty table, whose array holds no offset yet).
+    const size_t D = full ? hsz : dirty.size(), B = dm.mirror.blob.size() - blob0, f0 = n0 ? (size_t)n0 + 1 : 0, F = (size_t)n1 + 1 - f0;
+    size_t at = 0;
+    auto sec = [&](size_t bytes) { const size_t o = at; at += (bytes + 7) & ~(size_t)7; return o; };
+    const size_t o_blob = sec(B), o_off = sec(4 * F), o_valid = sec(n), o_keys = sec(64 * (size_t)n), o_slot = sec(4 * (size_t)n),
+                 o_code = sec(4 * (size_t)n), o_group = sec(group ? 4 * (size_t)n : 0), o_bits = sec(bits ? 4 * W * n : 0),
+                 o_idx = sec(4 * D), o_hash = sec(8 * D), o_pos = sec(full ? 0 : 4 * D);
+    const size_t o_scatter = o_idx;                                  // the scatter's values, copied to the device as one range
+    const int r = (int)(a.seq++ % fabgpu_ctx::MspAdmit::RING);
+    auto& hs = a.h_stage[r];
+    if (a.stage_set[r]) CK(ctx, cudaEventSynchronize(a.stage_ev[r].get()));         // its copies, RING admissions ago
+    if (at > hs.bytes())
+        if (int rc = hs.reserve(ctx, std::max(at, 2 * hs.bytes()))) return msp_admit_fail(ctx, rc, n0);
+    uint8_t* h = hs.get();
+    memcpy(h + o_blob, dm.mirror.blob.data() + blob0, B);
+    memcpy(h + o_off, dm.mirror.off.data() + f0, 4 * F);
+    memcpy(h + o_valid, valid, n);
+    memcpy(h + o_keys, keys_xy, 64 * (size_t)n);
+    memcpy(h + o_slot, raw.data(), 4 * (size_t)n);
+    memcpy(h + o_code, code.data(), 4 * (size_t)n);
+    if (group) memcpy(h + o_group, group, 4 * (size_t)n);
+    if (bits) memcpy(h + o_bits, bits, 4 * W * n);
+    for (size_t d = 0; d < D; d++) {
+        const uint32_t pos = full ? (uint32_t)d : dirty[d];
+        if (!full) memcpy(h + o_pos + 4 * d, &pos, 4);
+        memcpy(h + o_hash + 8 * d, &dm.mirror.ht_hash[pos], 8);
+        memcpy(h + o_idx + 4 * d, &dm.mirror.ht_idx[pos], 4);
+    }
+    // 1. before the waits, what no block in flight reads: grown arrays (the old ones retired until after the waits), the appended rows
+    //    past n0, a new index after growth, and the scatter's values.  The staging buffer's event follows these copies only.
+    std::vector<void*> retired;
+    uint8_t* d = nullptr;
+    auto retire_all = [&] { for (void* q : retired) cudaFreeAsync(q, ms); retired.clear(); if (d) cudaFreeAsync(d, ms); d = nullptr; };
+    auto fail = [&](int rc, const char* what) {
+        if (what) ctx->last_error = what;
+        for (auto& ds : ctx->devs[0].slot) cudaStreamSynchronize(ds.stream.get());     // the retired arrays' readers, before their free
+        retire_all();
+        return msp_admit_fail(ctx, rc, n0);
+    };
+    int rc = FABGPU_OK;
+    if ((rc = msp_grow(ctx, dm.id_blob, ms, blob0 + B, blob0, &retired)) ||
+        (rc = msp_grow(ctx, dm.id_off, ms, 4 * ((size_t)n1 + 1), 4 * f0, &retired)) ||
+        (rc = msp_grow(ctx, dm.valid, ms, n1, n0, &retired)) || (rc = msp_grow(ctx, dm.keys_xy, ms, 64 * (size_t)n1, 64 * (size_t)n0, &retired)) ||
+        (rc = msp_grow(ctx, dm.key_slot, ms, 4 * (size_t)n1, 4 * (size_t)n0, &retired)) ||
+        (rc = msp_grow(ctx, dm.msp_code, ms, 4 * (size_t)n1, 4 * (size_t)n0, &retired)) ||
+        (group && (rc = msp_grow(ctx, dm.group, ms, 4 * (size_t)n1, 4 * (size_t)n0, &retired))) ||
+        (bits && (rc = msp_grow(ctx, dm.pbits, ms, 4 * W * n1, 4 * W * n0, &retired))) ||
+        (full && ((rc = msp_grow(ctx, dm.ht_hash, ms, 8 * (size_t)hsz, 0, &retired, true)) ||
+                  (rc = msp_grow(ctx, dm.ht_idx, ms, 4 * (size_t)hsz, 0, &retired, true)))))
+        return fail(rc, nullptr);
+    auto up = [&](void* dst, size_t o, size_t bytes) { return !bytes || cudaMemcpyAsync(dst, h + o, bytes, cudaMemcpyHostToDevice, ms) == cudaSuccess; };
+    bool ok = up(dm.id_blob.get() + blob0, o_blob, B) && up(dm.id_off.get() + f0, o_off, 4 * F) && up(dm.valid.get() + n0, o_valid, n) &&
+              up(dm.keys_xy.get() + 64 * (size_t)n0, o_keys, 64 * (size_t)n) && up(dm.key_slot.get() + n0, o_slot, 4 * (size_t)n) &&
+              up(dm.msp_code.get() + n0, o_code, 4 * (size_t)n) && (!group || up(dm.group.get() + n0, o_group, 4 * (size_t)n)) &&
+              (!bits || up(dm.pbits.get() + W * n0, o_bits, 4 * W * n));
+    if (ok && full) ok = up(dm.ht_hash.get(), o_hash, 8 * D) && up(dm.ht_idx.get(), o_idx, 4 * D);
+    if (ok && !full && D) {
+        ok = cudaMallocAsync(reinterpret_cast<void**>(&d), at - o_scatter, ms) == cudaSuccess;
+        if (!ok) d = nullptr;
+        ok = ok && up(d, o_scatter, at - o_scatter);
+    }
+    ok = ok && cudaEventRecord(a.stage_ev[r].get(), ms) == cudaSuccess;
+    if (!ok) return fail(FABGPU_E_CUDA, "MSP table admission copy failed");
+    a.stage_set[r] = true;
+    // 2. the MSP stream waits for every slot's last decide stage: a slot whose last block recorded none waits for all its stream holds
+    auto& tx = ctx->txid;
+    for (int k = 0; k < FABGPU_SLOTS && ok; k++) {
+        if (!tx.decide_ev[k]) { cudaEvent_t ev = nullptr; ok = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess; tx.decide_ev[k].reset(ev); }
+        if (ok && !tx.decide_set[k]) ok = cudaEventRecord(tx.decide_ev[k].get(), ctx->devs[0].slot[k].stream.get()) == cudaSuccess;
+        ok = ok && cudaStreamWaitEvent(ms, tx.decide_ev[k].get(), 0) == cudaSuccess;
+    }
+    // 3. after them: the index slots blocks in flight read, in place, and the frees of what they were launched with
+    if (ok && !full && D) {
+        bdev::msp_scatter_kernel<<<(unsigned)((D + 255) / 256), 256, 0, ms>>>(dm.ht_hash.get(), dm.ht_idx.get(), reinterpret_cast<const uint32_t*>(d + (o_pos - o_scatter)),
+                                                                               reinterpret_cast<const uint64_t*>(d + (o_hash - o_scatter)),
+                                                                               reinterpret_cast<const int32_t*>(d), (uint32_t)D);
+        ctx->launches++;
+        ok = cudaGetLastError() == cudaSuccess;
+    }
+    if (!ok) return fail(FABGPU_E_CUDA, "MSP table admission enqueue failed");
+    retire_all();
+    CK(ctx, cudaEventRecord(a.ev.get(), ms));
+    a.ev_set = a.admitted = true;
+    dm.n_ids = n1; dm.ht_size = hsz;
     return FABGPU_OK;
 }
 
@@ -2984,6 +3229,48 @@ int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, siz
     return FABGPU_OK;
 }
 
+int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, size_t cap, size_t* n_out)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    if (!n_out || (cap && !out)) { ctx->last_error = "output arrays missing"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    auto& db = ctx->dbs[slot]; auto& u = ctx->uk[slot];
+    if (db.busy || !db.pvt_ready) { ctx->last_error = "the slot holds no finished block: fabgpu_validate_wait first"; return FABGPU_E_ARG; }
+    *n_out = 0;
+    if (db.T == 0) return FABGPU_OK;
+    const uint32_t T = (uint32_t)db.T, J = (uint32_t)(db.T * (1 + BD_ENDS_HINT));
+    uint32_t slots = 16; while (slots < 2 * J) slots <<= 1;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    Grow grow{ctx};
+    grow(u.d_hash, 8 * (size_t)J); grow(u.d_index, 4 * (size_t)slots); grow(u.d_rep, 4 * (size_t)J); grow(u.d_first, 8 * (size_t)J);
+    grow(u.d_cnt, 4 * ((size_t)T + 1)); grow(u.d_out, 12 * (size_t)J); grow(u.h_cnt, 4); grow(u.h_out, 12 * (size_t)J);
+    if (grow.rc) return grow.rc;
+    bdev::UkArrays a;
+    a.raw = db.d_raw.get(); a.ident = db.d_ident.get(); a.txs = db.d_txs.get(); a.T = T; a.E_cap = J - T; a.n_end = db.d_counter.get();
+    a.hash = u.d_hash.get(); a.index = u.d_index.get(); a.index_mask = slots - 1; a.rep = u.d_rep.get(); a.first = u.d_first.get();
+    a.cnt = u.d_cnt.get(); a.out = u.d_out.get();
+    const uint8_t* blk = ctx->bbs[slot].d_block.get();
+    CK(ctx, cudaMemsetAsync(u.d_index.get(), 0xff, 4 * (size_t)slots, st));
+    bdev::uk_hash_kernel<<<(J + 127) / 128, 128, 0, st>>>(blk, a);
+    bdev::uk_insert_kernel<<<(J + 127) / 128, 128, 0, st>>>(blk, a);
+    bdev::uk_count_kernel<<<(T + 127) / 128, 128, 0, st>>>(a);
+    bdev::uk_scan_kernel<<<1, 1024, 0, st>>>(a);
+    bdev::uk_emit_kernel<<<(T + 127) / 128, 128, 0, st>>>(a);
+    ctx->launches += 5;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpyAsync(u.h_cnt.get(), u.d_cnt.get() + T, 4, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    const size_t total = u.h_cnt.get()[0], w = std::min(total, cap);
+    if (w) {
+        CK(ctx, cudaMemcpyAsync(u.h_out.get(), u.d_out.get(), 12 * w, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        memcpy(out, u.h_out.get(), 12 * w);
+    }
+    *n_out = total;
+    return FABGPU_OK;
+}
+
 int fabgpu_block_buffer_slot(fabgpu_ctx* ctx, int slot, size_t bytes, uint8_t** out)
 {
     if (!ctx || !out || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
@@ -3023,23 +3310,29 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
         };
         if (any_stale()) {
             rl.unlock();
+            // every identity in its own tier (fabgpu_ctx::identity_tier): configured ones as fabgpu_msp_configure issued them, admitted ones small
             const int n_ids = (int)ctx->identity_slot.size();
-            const bool big = n_ids <= ctx->kt->key_slots;
-            int rc = big ? fabgpu_keys_register(ctx, ctx->msp.keys_xy.data(), n_ids, ctx->identity_slot.data())     // exclusive; drains every stream first
-                         : msp_small_tier(ctx, ctx->msp.keys_xy.data(), n_ids);
-            if (rc) return rc;
-            rl.lock();
-            std::vector<int32_t> raw(n_ids, -1);
-            dm.all_slots = true; dm.classes = 0;
-            {
-                std::lock_guard<std::mutex> lk(ctx->mu);      // a handle recycled again in the gap resolves to -1: that identity goes through the generic kernel
-                for (int i = 0; i < n_ids; i++) {
-                    raw[i] = handle_to_slot(ctx, ctx->identity_slot[i]);
-                    if (raw[i] < 0) { dm.all_slots = false; dm.classes |= raw[i] == -1 ? CLASS_GENERIC : CLASS_SMALL; }
-                }
+            for (uint8_t tier : {TIER_WINDOW, TIER_SMALL}) {
+                std::vector<int> which;
+                for (int i = 0; i < n_ids; i++) if (ctx->identity_tier[i] == tier) which.push_back(i);
+                if (which.empty()) continue;
+                const int m = (int)which.size();
+                std::vector<uint8_t> keys(64 * (size_t)m);
+                std::vector<int32_t> hd(m);
+                for (int q = 0; q < m; q++) { memcpy(keys.data() + 64 * (size_t)q, ctx->msp.keys_xy.data() + 64 * (size_t)which[q], 64); hd[q] = ctx->identity_slot[which[q]]; }
+                int rc = tier == TIER_WINDOW ? fabgpu_keys_register(ctx, keys.data(), m, hd.data())     // exclusive; drains every stream first
+                                             : msp_small_tier(ctx, keys.data(), m, hd.data());
+                if (rc) return rc;
+                for (int q = 0; q < m; q++) ctx->identity_slot[which[q]] = hd[q];
             }
-            // submitters are serialised by slot0_mu; blocks in flight on the other slots still read dm.key_slot: let them finish first
+            rl.lock();
+            std::vector<int32_t> raw(n_ids > 0 ? n_ids : 1, -1);
+            dm.all_slots = true; dm.classes = 0;
+            msp_raw_slots(ctx, 0, n_ids, raw.data());         // a handle recycled again in the gap resolves to -1: that identity goes through the generic kernel
+            // submitters are serialised by slot0_mu; blocks in flight on the other slots still read dm.key_slot, and admissions write it:
+            // let them finish first
             for (auto& dsx : dv.slot) CK(ctx, cudaStreamSynchronize(dsx.stream.get()));
+            if (ctx->adm.stream) CK(ctx, cudaStreamSynchronize(ctx->adm.stream.get()));
             CK(ctx, cudaMemcpy(dm.key_slot.get(), raw.data(), 4 * (size_t)n_ids, cudaMemcpyHostToDevice));
         }
     }
@@ -3137,6 +3430,7 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     // under this block's kernels: the slots.)
     CK(ctx, cudaMemcpyAsync(bb.d_block.get(), block, block_len, cudaMemcpyHostToDevice, st));
     bdev::block_walk_kernel<<<(cnt + 31) / 32, 32, 0, st>>>(bb.d_block.get(), db.d_env_off.get(), 0u, cnt, cnt, dm.channel.get(), dm.channel_len, db.d_txs.get(), db.d_raw.get(), ja, db.d_counter.get());
+    if (ctx->adm.ev_set) CK(ctx, cudaStreamWaitEvent(st, ctx->adm.ev.get(), 0));      // the MSP table as the admissions returned so far left it
     bdev::block_resolve_kernel<<<(cnt + 63) / 64, 64, 0, st>>>(bb.d_block.get(), db.d_raw.get(), 0u, cnt, m, ja, db.d_txs.get());                      // creator jobs
     sha256_segments_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), reinterpret_cast<const ShaJob*>(db.d_sha.get()), cnt, db.d_dig.get());
     sha256_segments_kernel<<<(2 * cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), reinterpret_cast<const ShaJob*>(db.d_sha.get() + J_cap), 2 * cnt, db.d_dig.get() + 32 * J_cap);
@@ -3163,10 +3457,12 @@ static int block_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size_t 
     bdev::block_decide_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(bb.d_block.get(), db.d_txs.get(), cnt, m, pol, db.d_mask.get(), db.d_gate.get(), db.d_ident.get(), db.d_dig.get(), (uint32_t)J_cap, db.d_flags.get(),
                                                                db.d_hash.get(), db.d_seg.get(), kl, db.v13 ? db.d_counter.get() + 1 : nullptr, tsd);
     ctx->launches++;
-    if (tx_set.installed) {                                   // a later mutation of the set waits for this decide stage
+    if (tx_set.installed || ctx->adm.admitted) {              // a later mutation of the set or the MSP table waits for this decide stage
         if (!tx_set.decide_ev[slot]) { cudaEvent_t ev = nullptr; CK(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); tx_set.decide_ev[slot].reset(ev); }
         CK(ctx, cudaEventRecord(tx_set.decide_ev[slot].get(), st));
         tx_set.decide_set[slot] = true;
+    } else {
+        tx_set.decide_set[slot] = false;                      // this block recorded none: a mutation waits for the slot's whole stream
     }
     if (db.kl_on) {
         bdev::block_kl_resolve_kernel<<<1, 256, 0, st>>>(db.d_txs.get(), cnt, kl, db.d_flags.get());

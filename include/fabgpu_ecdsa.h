@@ -271,6 +271,8 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
  *       identity satisfies ADMIN without it, mspimpl.go:506-513); the creator's Validate() is still checked.  n_ids and
  *       n_principals must equal fabgpu_msp_configure's, else FABGPU_E_ARG and nothing changes; n_ids = 0 removes the bits
  *       and restores MSP-id member matching.
+ *   (_identity_groups and _principal_bits take the identities the table holds now: those fabgpu_msp_configure installed, then those
+ *       fabgpu_msp_identities_add admitted, in that order.)
  *   _collection_policies: the endorsement policy of private-data collections.  Entry i says that a write to collection coll[i]
  *       (coll_blob + (n+1) offsets) of namespace ns[i] (ns_blob + (n+1) offsets) is checked against the tree at node coll_root[i] of
  *       fabgpu_msp_configure's array instead of the chaincode's (core/common/validation/statebased/v20.go:105-147).  The caller
@@ -285,6 +287,19 @@ int fabgpu_msp_configure(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t
  *       n = 0 removes the table: every write falls under its namespace's chaincode policy, as without this call. */
 int fabgpu_msp_identity_groups(fabgpu_ctx* ctx, const int32_t* group, int n_ids);
 int fabgpu_msp_principal_bits(fabgpu_ctx* ctx, const uint32_t* bits, int n_ids, int n_principals);
+/* Identity admission: appends n identities to the table fabgpu_msp_configure installed, in its encoding (serialized bytes, MSP id,
+ * X||Y, Validate() outcome), without draining the block slots -- the table the device reads while blocks are in flight.  A new MSP id
+ * gets a code of its own, which matches no principal of the policies.  group: one de-duplication id per identity (it may name an
+ * existing group, e.g. another serialization of a held certificate), given iff a group table is installed; bits: W words per identity
+ * (W of fabgpu_msp_principal_bits), given iff principal bits are installed.  Ordering as for fabgpu_committed_txids_add: blocks submitted
+ * before the call returns never see the new identities, every block submitted after it does; the host never waits for blocks in
+ * flight.  Each admitted key gets a small table (or keeps the window table it owns); with no small slot free it goes through the
+ * generic kernel.  FABGPU_E_ARG, with nothing enqueued and the table unchanged, for: no configured table, n < 0, NULL arrays with
+ * n > 0, decreasing offsets, an empty identity, an identity the table holds (equal bytes) or one given twice, group or bits present
+ * when it must be absent or absent when it must be present, a negative group.  fabgpu_msp_configure replaces admitted identities
+ * too.  Contexts of one table group (fabgpu_init_shared) admit independently. */
+int fabgpu_msp_identities_add(fabgpu_ctx* ctx, const uint8_t* id_blob, const uint32_t* id_off, const uint8_t* mspid_blob, const uint32_t* mspid_off,
+                              const uint8_t* keys_xy, const uint8_t* valid, const int32_t* group, const uint32_t* bits, int n);
 int fabgpu_namespace_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const int32_t* ns_root, int n_ns);
 int fabgpu_collection_policies(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* ns_off, const uint8_t* coll_blob,
                                const uint32_t* coll_off, const int32_t* coll_root, int n);
@@ -498,6 +513,14 @@ int fabgpu_state_database(fabgpu_ctx* ctx, int kind);
  *   missing-data bookkeeping. */
 int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
                             const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4]);
+/* The identities the slot's finished block looked up in the MSP table and did not find (creators and endorsers with a signature
+ * job), listed on the device: distinct serialized identities, ordered by first appearance -- transaction, then the creator before its
+ * endorsers in endorsement order -- as triples (offset, length, first tx), the offset and length in the bytes the slot's block was
+ * submitted in.  At most cap triples go to out; *n_out gets the full count.  These are what the peer runs through its MSP
+ * (DeserializeIdentity, Validate, SatisfiesPrincipal) and hands to fabgpu_msp_identities_add.  Any number of calls between the slot's
+ * fabgpu_validate_wait and its next submit, on the slot's stream; returns synchronised.  FABGPU_E_ARG, with nothing enqueued, for a
+ * slot with no finished block and for NULL outputs. */
+int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, size_t cap, size_t* n_out);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
