@@ -12,6 +12,9 @@ SLOTS = 3
 CAP_V2_0, CAP_V1_3 = 0, 1      # fabgpu_channel_capability
 STATEDB_LEVELDB, STATEDB_COUCHDB = 0, 1             # fabgpu_state_database
 STATE_REMOVE = (2 ** 64 - 1, 2 ** 64 - 1)   # fabgpu_state_versions_update: a version that removes the key
+UPDATE_WORDS, UPDATE_PUT, UPDATE_DELETE = 14, 1, 2       # fabgpu_block_updates: words per record, its ops
+SRC_NONE, SRC_BLOCK, SRC_COMMITTED = 0, 1, 2            # ... and its value and metadata sources
+COMMITTED = "committed"                                 # block_updates: a value or metadata the peer reads from its state database
 
 OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
 (ST_VALID, ST_INVALID, ST_ERR_NIL_KEY, ST_ERR_EMPTY_SIG, ST_ERR_EMPTY_DIGEST, ST_ERR_UNMARSHAL, ST_ERR_R_NOT_POSITIVE,
@@ -35,7 +38,7 @@ EXPORTS = [
     "fabgpu_committed_txids", "fabgpu_committed_txids_add", "fabgpu_committed_txids_info", "fabgpu_committed_txids_add_block",
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
-    "fabgpu_validate_pvtdata", "fabgpu_msp_identities_add", "fabgpu_block_unknown_identities",
+    "fabgpu_validate_pvtdata", "fabgpu_msp_identities_add", "fabgpu_block_unknown_identities", "fabgpu_block_updates",
 ]
 
 
@@ -485,6 +488,34 @@ class Context:
         if src is None:
             raise FabGpuError(E_ARG, "no block submitted on this slot through this binding")
         return [(bytes(src[int(out[3 * i]): int(out[3 * i]) + int(out[3 * i + 1])]), int(out[3 * i + 2])) for i in range(n.value)]
+
+    def block_updates(self, slot, block_num):
+        """The update batch of the block validate_mvcc(slot, block_num) last ran on (fabgpu_block_updates): [(tx, op, ns, coll, key, value,
+        metadata)] in the library's order -- op "put" or "del"; ns, coll (b"" for a public key) and key as bytes; value the bytes (read back
+        from the buffer the block was submitted in), COMMITTED (the peer's GetState supplies it) or None for a delete; metadata the
+        Serialize bytes, None (nil) or COMMITTED.  None when the batch is incomplete and the peer builds it itself."""
+        n = (ctypes.c_size_t * 2)()
+        complete = ctypes.c_int(0)
+        rec_cap, meta_cap = 1024, 1 << 16
+        while True:
+            rec = np.zeros(UPDATE_WORDS * rec_cap, np.uint32)
+            meta = np.zeros(meta_cap, np.uint8)
+            self._ck(lib().fabgpu_block_updates(self._h, ctypes.c_int(slot), ctypes.c_uint64(block_num), _p(rec), ctypes.c_size_t(rec_cap), _p(meta),
+                                                ctypes.c_size_t(meta_cap), n, ctypes.byref(complete)))
+            if n[0] <= rec_cap and n[1] <= meta_cap:
+                break
+            rec_cap, meta_cap = max(rec_cap, n[0]), max(meta_cap, n[1])
+        if not complete.value:
+            return None
+        src = memoryview(self._last_block[slot]).cast("B")
+        meta = meta.tobytes()
+        out = []
+        for w in rec[: UPDATE_WORDS * n[0]].reshape(-1, UPDATE_WORDS).tolist():
+            value = None if w[2] == SRC_NONE else bytes(src[w[10]:w[10] + w[11]]) if w[2] == SRC_BLOCK else COMMITTED
+            md = None if w[3] == SRC_NONE else meta[w[12]:w[12] + w[13]] if w[3] == SRC_BLOCK else COMMITTED
+            out.append((w[0], "put" if w[1] == UPDATE_PUT else "del", bytes(src[w[4]:w[4] + w[5]]), bytes(src[w[6]:w[6] + w[7]]),
+                        bytes(src[w[8]:w[8] + w[9]]), value, md))
+        return out
 
     def collection_policies(self, table):
         """table: {(namespace, collection): root node index} -- the endorsement policy a write to that private-data collection is checked

@@ -31,6 +31,7 @@
 #include "txidset.hpp"
 #include "stateset.hpp"
 #include "couchval.cuh"
+#include "updates.cuh"
 #include "pvtdata.cuh"
 #include "msptable.hpp"
 #include "unknownids.cuh"
@@ -326,6 +327,7 @@ struct fabgpu_ctx {
         bool mvcc_ready = false;                 // fabgpu_validate_wait returned the block and its bytes are still on the device
         bool pvt_ready = false;                  // the same, for fabgpu_validate_pvtdata: fabgpu_validate_mvcc leaves it set
         uint8_t txid_block = 0;                  // fabgpu_committed_txids_add_block: 0 no block submitted, 1 submitted, 2 its ids added
+        bool upd_ready = false;                  // fabgpu_validate_mvcc ran on this block (fabgpu_block_updates): cleared by the next submit
         std::vector<uint64_t> dup_keys; std::vector<uint32_t> dup_idx;   // scratch of the duplicate-tx-id pass (per slot: waits may run concurrently)
         std::chrono::steady_clock::time_point t0, t1;
         Event ev[6];                             // created on the first block timed with FABGPU_BLOCK_EVENTS=1
@@ -387,6 +389,13 @@ struct fabgpu_ctx {
         bool couch = false;
         DevArray<bdev::CvWrite> d_cvw; DevArray<uint32_t> d_cv_first, d_cv_n; DevArray<uint8_t> d_cv_undet, d_cv_code; DevArray<uint32_t> d_cv_long;
         uint32_t cv_hint = 4;                                                            // public writes per transaction
+        // fabgpu_block_updates of the block the stage last ran on (updates.cuh), built by the first call from the stage's arrays, which
+        // stay untouched until the next stage.  upd_slot -1: none (the next stage or state call clears it).  upd_incomplete: open, broken
+        // or aliased as the stage left it, or found so by the build.
+        int upd_slot = -1; uint64_t upd_block = 0; uint32_t upd_R = 0, upd_K = 0, upd_T = 0; bool upd_incomplete = false, upd_built = false;
+        size_t upd_n[2] = {0, 0};
+        DevArray<bdev::UdPair> d_upair; DevArray<bdev::UdKey> d_ukey; DevArray<bdev::UdSeg> d_useg; DevArray<uint8_t> d_uneed, d_utxneed, d_umeta;
+        DevArray<uint32_t> d_ubase, d_umark, d_uokey, d_uomoff, d_uout, d_uctr; HostArray<uint32_t> h_uctr;
         ~StateSet() { if (table) cudaFree(table); }
     } sv;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, then devices, then the group's tables if
@@ -2860,6 +2869,7 @@ static int sv_replace(fabgpu_ctx* ctx, const uint8_t* ns_blob, const uint32_t* n
     if (const char* err = stateset::prepare(ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, ctx->sv.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& s = ctx->sv;
+    s.upd_slot = -1;
     if (s.couch && !cv_keys_ok(ctx, coll_off, key_blob, key_off, ver, n)) return FABGPU_E_ARG;
     int rc = drain_block_streams(ctx);                         // the stage of a slot's block may still be running: let it finish
     if (!rc) rc = sv_begin(ctx);
@@ -2900,6 +2910,7 @@ int fabgpu_state_versions_update(fabgpu_ctx* ctx, const uint8_t* ns_blob, const 
     if (const char* err = stateset::prepare(ns_blob, ns_off, coll_blob, coll_off, key_blob, key_off, ver, n, ctx->sv.seed, recs)) { ctx->last_error = err; return FABGPU_E_ARG; }
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& s = ctx->sv;
+    s.upd_slot = -1;
     if (!s.installed) { ctx->last_error = "no state version table installed: call fabgpu_state_versions first"; return FABGPU_E_ARG; }
     if (s.broken) { ctx->last_error = "the state version table is broken by a failed call: replace it with fabgpu_state_versions"; return FABGPU_E_ARG; }
     if (s.couch && !cv_keys_ok(ctx, coll_off, key_blob, key_off, ver, n)) return FABGPU_E_ARG;
@@ -3011,6 +3022,15 @@ static int cv_prepass(fabgpu_ctx* ctx, cudaStream_t st, const uint8_t* blk, cons
     return FABGPU_OK;
 }
 
+// The stage ran on the slot's block: fabgpu_block_updates may build its batch from the stage's arrays (R records, K key-table entries)
+static void upd_mark(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t R, uint32_t K, uint32_t T, bool incomplete)
+{
+    auto& s = ctx->sv;
+    s.upd_slot = slot; s.upd_block = block_num; s.upd_R = R; s.upd_K = K; s.upd_T = T;
+    s.upd_incomplete = incomplete; s.upd_built = false; s.upd_n[0] = s.upd_n[1] = 0;
+    ctx->dbs[slot].upd_ready = true;
+}
+
 // The MVCC stage of the slot's block, on the slot's stream after its last kernel:
 //   mv_scan_kernel (per transaction: read / write records with key digests) -> host reads the record count (grows the arrays and runs
 //   the scan again on overflow) -> mv_key_kernel (per record: the block's key table, the committed table's answer) -> mv_check_kernel
@@ -3027,6 +3047,7 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
     auto& s = ctx->sv; auto& db = ctx->dbs[slot];
+    s.upd_slot = -1;
     if (!s.installed) { ctx->last_error = "no state version table installed: call fabgpu_state_versions first"; return FABGPU_E_ARG; }
     if (s.open) { ctx->last_error = "the previous block is open: fabgpu_state_versions_update(..., height = block_num + 1) first"; return FABGPU_E_ARG; }
     if (block_num != s.height) { ctx->last_error = "block_num is not the table's height"; return FABGPU_E_ARG; }
@@ -3034,12 +3055,13 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
     if (s.broken) {                                            // nothing can be decided or applied
         for (size_t t = 0; t < n; t++) flags[t] = tv_flags[t] == bdev::TXC_VALID ? bdev::TXC_NOT_VALIDATED : tv_flags[t];
+        upd_mark(ctx, slot, block_num, 0, 0, 0, true);
         return FABGPU_OK;
     }
     int rc = sv_begin(ctx);
     if (rc) return rc;
     const uint32_t T = (uint32_t)n;
-    if (T == 0) { db.mvcc_ready = false; s.height = block_num + 1; return FABGPU_OK; }
+    if (T == 0) { db.mvcc_ready = false; s.height = block_num + 1; upd_mark(ctx, slot, block_num, 0, 0, 0, false); return FABGPU_OK; }
     cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
     Grow grow{ctx};
     grow(s.d_first, 4 * (size_t)T); grow(s.d_n, 4 * (size_t)T); grow(s.d_mlist, 4 * (size_t)T); grow(s.d_info, T); grow(s.d_tv, T); grow(s.d_flags, T);
@@ -3138,6 +3160,7 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     db.mvcc_ready = false;
     if (hc[1] || hc[2] != UINT32_MAX) s.open = true;           // two keys shared a tag, or a write set could not be enumerated
     else s.height = block_num + 1;
+    upd_mark(ctx, slot, block_num, R, K, T, s.open);
     return FABGPU_OK;
 }
 
@@ -3268,6 +3291,97 @@ int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, si
         memcpy(out, u.h_out.get(), 12 * w);
     }
     *n_out = total;
+    return FABGPU_OK;
+}
+
+// Builds the update batch of the block the stage last ran on (on `slot`'s stream; returns synchronised):
+//   ud_pair_kernel (per record: (tx, key) pairs of VALID writes) -> ud_class_kernel (per pair) -> ud_walk_kernel (per pair: the nearest
+//   earlier writers) -> ud_base_kernel (one CTA: transaction-order positions) -> ud_resolve_kernel (per key) -> ud_seg_kernel (per
+//   transaction holding a wanted record: one re-scan) -> ud_compact_kernel (one CTA: order, metadata offsets, totals) -> host reads the
+//   totals -> ud_emit_kernel (per record).
+static int upd_build(fabgpu_ctx* ctx, int slot)
+{
+    auto& s = ctx->sv; auto& db = ctx->dbs[slot];
+    const uint32_t R = s.upd_R, T = s.upd_T, K = s.upd_K;
+    if (!s.upd_incomplete && T && memchr(s.h_flags.get(), bdev::TXC_NOT_VALIDATED, T)) s.upd_incomplete = true;    // a 254 is left
+    if (s.upd_incomplete || R == 0) return FABGPU_OK;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    uint32_t P = 64;
+    while (P < 2 * (uint64_t)R) P <<= 1;
+    Grow g{ctx};
+    g(s.d_upair, (size_t)P * sizeof(bdev::UdPair)); g(s.d_ukey, (size_t)K * sizeof(bdev::UdKey)); g(s.d_useg, (size_t)R * sizeof(bdev::UdSeg));
+    g(s.d_uneed, R); g(s.d_utxneed, T); g(s.d_ubase, 4 * (size_t)T); g(s.d_umark, 4 * (size_t)R); g(s.d_uokey, 4 * (size_t)R);
+    g(s.d_uomoff, 4 * (size_t)R); g(s.d_uctr, 16); g(s.h_uctr, 16);
+    if (g.rc) return g.rc;
+    CK(ctx, cudaMemsetAsync(s.d_upair.get(), 0, (size_t)P * sizeof(bdev::UdPair), st));
+    CK(ctx, cudaMemsetAsync(s.d_ukey.get(), 0, (size_t)K * sizeof(bdev::UdKey), st));
+    CK(ctx, cudaMemsetAsync(s.d_uneed.get(), 0, R, st));
+    CK(ctx, cudaMemsetAsync(s.d_utxneed.get(), 0, T, st));
+    CK(ctx, cudaMemsetAsync(s.d_umark.get(), 0, 4 * (size_t)R, st));
+    CK(ctx, cudaMemsetAsync(s.d_uctr.get(), 0, 16, st));
+    bdev::UdArrays a;
+    a.rec = s.d_rec.get(); a.first_rec = s.d_first.get(); a.n_rec = s.d_n.get(); a.flags = s.d_flags.get(); a.R = R; a.T = T; a.K = K;
+    a.pair = s.d_upair.get(); a.P_size = P; a.key = s.d_ukey.get(); a.base = s.d_ubase.get(); a.mark = s.d_umark.get();
+    a.need = s.d_uneed.get(); a.txneed = s.d_utxneed.get(); a.seg = s.d_useg.get(); a.out_key = s.d_uokey.get(); a.out_moff = s.d_uomoff.get();
+    a.out = nullptr; a.meta = nullptr; a.ctr = s.d_uctr.get();
+    const uint8_t* blk = ctx->bbs[slot].d_block.get();
+    bdev::ud_pair_kernel<<<(R + 255) / 256, 256, 0, st>>>(a);
+    bdev::ud_class_kernel<<<P / 256 + 1, 256, 0, st>>>(a);
+    bdev::ud_walk_kernel<<<P / 256 + 1, 256, 0, st>>>(a);
+    bdev::ud_base_kernel<<<1, 1024, 0, st>>>(a);
+    bdev::ud_resolve_kernel<<<(K + 255) / 256, 256, 0, st>>>(a);
+    bdev::ud_seg_kernel<<<(T + 63) / 64, 64, 0, st>>>(blk, db.d_txs.get(), a);
+    bdev::ud_compact_kernel<<<1, 1024, 0, st>>>(a);
+    ctx->launches += 7;
+    CK(ctx, cudaGetLastError());
+    uint32_t* hc = s.h_uctr.get();
+    CK(ctx, cudaMemcpyAsync(hc, s.d_uctr.get(), 12, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    if (hc[0]) { s.upd_incomplete = true; return FABGPU_OK; }
+    const uint32_t n = hc[1], mb = hc[2];
+    if (n) {
+        Grow g2{ctx};
+        g2(s.d_uout, (size_t)n * bdev::UD_WORDS * 4); g2(s.d_umeta, std::max<size_t>(mb, 1));
+        if (g2.rc) return g2.rc;
+        a.out = s.d_uout.get(); a.meta = s.d_umeta.get();
+        bdev::ud_emit_kernel<<<(n + 127) / 128, 128, 0, st>>>(blk, a);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaStreamSynchronize(st));
+    }
+    s.upd_n[0] = n; s.upd_n[1] = mb;
+    return FABGPU_OK;
+}
+
+int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t* rec, size_t rec_cap, uint8_t* meta, size_t meta_cap,
+                         size_t n_out[2], int* complete)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    if (!n_out || !complete || (rec_cap && !rec) || (meta_cap && !meta)) { ctx->last_error = "output arrays missing"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    if (s.upd_slot != slot || s.upd_block != block_num || !ctx->dbs[slot].upd_ready) {
+        ctx->last_error = "no update batch for this slot and block: fabgpu_validate_mvcc(slot, block_num) last ran on another, or a stage, a "
+                          "state version call or the slot's next submit came after it";
+        return FABGPU_E_ARG;
+    }
+    if (!s.upd_built) {
+        if (int rc = upd_build(ctx, slot)) return rc;
+        s.upd_built = true;
+    }
+    n_out[0] = n_out[1] = 0; *complete = 0;
+    if (s.upd_incomplete) return FABGPU_OK;
+    *complete = 1; n_out[0] = s.upd_n[0]; n_out[1] = s.upd_n[1];
+    const size_t w = std::min(s.upd_n[0], rec_cap), m = std::min(s.upd_n[1], meta_cap);
+    if (w || m) {
+        CK(ctx, cudaSetDevice(ctx->devs[0].id));
+        cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+        if (w) CK(ctx, cudaMemcpyAsync(rec, s.d_uout.get(), w * bdev::UD_WORDS * 4, cudaMemcpyDeviceToHost, st));
+        if (m) CK(ctx, cudaMemcpyAsync(meta, s.d_umeta.get(), m, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+    }
     return FABGPU_OK;
 }
 
@@ -3546,7 +3660,7 @@ static int validate_submit(fabgpu_ctx* ctx, int slot, const uint8_t* block, size
     std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
     auto& db = ctx->dbs[slot];
     if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-    db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 0;
+    db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 0; db.upd_ready = false;
     if (fault_injected()) { ctx->last_error = "fault injected (FABGPU_FAULT_INJECT=1)"; return FABGPU_E_INJECTED; }
     int rc;
     {
@@ -3572,7 +3686,7 @@ int fabgpu_validate_envelopes_async(fabgpu_ctx* ctx, int slot, const uint8_t* bl
         std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
         auto& db = ctx->dbs[slot];
         if (db.busy) { ctx->last_error = "slot already holds a block: call fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 1;
+        db.T = 0; db.on_device = false; db.busy = true; db.mvcc_ready = false; db.pvt_ready = false; db.txid_block = 1; db.upd_ready = false;
         return FABGPU_OK;
     }
     return validate_submit(ctx, slot, blob, env_off[n_env], env_off, n_env);

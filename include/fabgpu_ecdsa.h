@@ -521,6 +521,35 @@ int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, siz
  * fabgpu_validate_wait and its next submit, on the slot's stream; returns synchronised.  FABGPU_E_ARG, with nothing enqueued, for a
  * slot with no finished block and for NULL outputs. */
 int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, size_t cap, size_t* n_out);
+/* The block's public and hashed update batch, as applyWriteSet leaves it in publicUpdates and hashUpdates for the transactions the
+ * MVCC stage left VALID (validation/types.go:81-111, tx_ops.go:18-232): each key a VALID transaction wrote, at most once, with its final
+ * operation in the block at version (block_num, tx).  Records of FABGPU_UPDATE_WORDS uint32 words go to rec, at most rec_cap of them:
+ *   [0] tx (the version's tx_num)   [1] op: FABGPU_UPDATE_PUT or FABGPU_UPDATE_DELETE
+ *   [2] value source: FABGPU_SRC_NONE (a DELETE), FABGPU_SRC_BLOCK (the KVWrite.value or KVWriteHash.value_hash at [10], [11] -- possibly
+ *       an earlier VALID transaction's, which a metadata-only write inherits) or FABGPU_SRC_COMMITTED (the peer reads it with GetState /
+ *       GetValueHash: no writer of the block put the key before)
+ *   [3] metadata source: FABGPU_SRC_NONE (nil), FABGPU_SRC_BLOCK (statemetadata.Serialize of the deciding metadata write's entries, at
+ *       meta[[12] .. [12] + [13])) or FABGPU_SRC_COMMITTED (GetStateMetadata / GetPrivateDataMetadataByHash)
+ *   [4], [5] namespace; [6], [7] collection (length 0 for a public key); [8], [9] key (the 32-byte key hash for a hashed key): offsets and
+ *       lengths in the bytes the slot's block was submitted in
+ *   [10], [11] the value (FABGPU_SRC_BLOCK), [12], [13] the metadata bytes (FABGPU_SRC_BLOCK); 0 otherwise.
+ * Records come ordered by tx, then by the wire position of that transaction's first write of the key.  n_out[0] gets the full record
+ * count and n_out[1] the metadata bytes; at most meta_cap bytes go to meta.  *complete = 1 when the batch is the block's; 0 with no
+ * records (the peer builds the batch itself) when a flag is 254 after the stage, the stage left the block open, two digests shared a
+ * tag, the table was broken, a record's metadata entries are not canonical (name = 1 then value = 2, each at most once and non-empty,
+ * minimal lengths, nothing else), or a record depends on a key the table marks unknown.  The private update batch is not built.
+ * Call it any number of times after fabgpu_validate_mvcc(slot, block_num) returned, until the next fabgpu_validate_mvcc, the next
+ * fabgpu_state_versions* call or the slot's next submit; the first call builds the batch on the slot's stream, later ones copy it.
+ * Returns synchronised.  FABGPU_E_ARG, with nothing enqueued, when slot and block_num are not those the stage last ran on, after one of
+ * those events, and for NULL outputs. */
+#define FABGPU_UPDATE_WORDS 14
+#define FABGPU_UPDATE_PUT 1
+#define FABGPU_UPDATE_DELETE 2
+#define FABGPU_SRC_NONE 0
+#define FABGPU_SRC_BLOCK 1
+#define FABGPU_SRC_COMMITTED 2
+int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t* rec, size_t rec_cap, uint8_t* meta, size_t meta_cap,
+                         size_t n_out[2], int* complete);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
