@@ -15,6 +15,7 @@ STATE_REMOVE = (2 ** 64 - 1, 2 ** 64 - 1)   # fabgpu_state_versions_update: a ve
 UPDATE_WORDS, UPDATE_PUT, UPDATE_DELETE = 14, 1, 2       # fabgpu_block_updates: words per record, its ops
 SRC_NONE, SRC_BLOCK, SRC_COMMITTED = 0, 1, 2            # ... and its value and metadata sources
 COMMITTED = "committed"                                 # block_updates: a value or metadata the peer reads from its state database
+PVT_UPDATE_WORDS, UPDATE_RENEW = 11, 3                  # fabgpu_block_pvt_updates: words per record, the op the peer resolves
 
 OK, E_NO_DEVICE, E_CUDA, E_ARG, E_INJECTED = 0, -1, -2, -3, -4
 (ST_VALID, ST_INVALID, ST_ERR_NIL_KEY, ST_ERR_EMPTY_SIG, ST_ERR_EMPTY_DIGEST, ST_ERR_UNMARSHAL, ST_ERR_R_NOT_POSITIVE,
@@ -39,6 +40,7 @@ EXPORTS = [
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
     "fabgpu_validate_pvtdata", "fabgpu_msp_identities_add", "fabgpu_block_unknown_identities", "fabgpu_block_updates",
+    "fabgpu_block_pvt_updates",
 ]
 
 
@@ -516,6 +518,41 @@ class Context:
             out.append((w[0], "put" if w[1] == UPDATE_PUT else "del", bytes(src[w[4]:w[4] + w[5]]), bytes(src[w[6]:w[6] + w[7]]),
                         bytes(src[w[8]:w[8] + w[9]]), value, md))
         return out
+
+    def block_pvt_updates(self, slot, block_num, pvt):
+        """The private update batch of the block validate_mvcc(slot, block_num) last ran on (fabgpu_block_pvt_updates); pvt maps SeqInBlock
+        -> marshalled rwset.TxPvtReadWriteSet, as validate_pvtdata takes it.  Returns (verdict, status, records): verdict and status as
+        validate_pvtdata gives them with the stage's flags; records None when the batch is incomplete (the peer builds it itself), else
+        [(tx, op, ns, coll, key, value, hashed_index)] in the library's order -- op "put", "del" or "renew"; ns, coll, key and value (a put's;
+        None otherwise) as bytes; hashed_index the index of the hashed PUT record in block_updates' list for a "renew", else None."""
+        seqs = sorted(pvt)
+        items = [bytes(pvt[k]) for k in seqs]
+        blob, off = _blob(items)
+        sq = np.array(seqs or [0], np.uint32)
+        st = np.zeros(3 * max(len(seqs), 1), np.int32)
+        out = np.zeros(4, np.int32)
+        n = ctypes.c_size_t(0)
+        complete = ctypes.c_int(0)
+        cap = 1024
+        while True:
+            rec = np.zeros(PVT_UPDATE_WORDS * cap, np.uint32)
+            self._ck(lib().fabgpu_block_pvt_updates(self._h, ctypes.c_int(slot), ctypes.c_uint64(block_num), _p(blob), _p(off), _p(sq),
+                                                    ctypes.c_size_t(len(seqs)), _p(st), _p(out), _p(rec), ctypes.c_size_t(cap), ctypes.byref(n),
+                                                    ctypes.byref(complete)))
+            if n.value <= cap:
+                break
+            cap = n.value
+        verdict = tuple(int(x) for x in out)
+        status = {k: tuple(int(x) for x in st[3 * i:3 * i + 3]) for i, k in enumerate(seqs)}
+        if not complete.value:
+            return verdict, status, None
+        src = bytes(blob)
+        ops = {UPDATE_PUT: "put", UPDATE_DELETE: "del", UPDATE_RENEW: "renew"}
+        records = []
+        for w in rec[: PVT_UPDATE_WORDS * n.value].reshape(-1, PVT_UPDATE_WORDS).tolist():
+            records.append((w[0], ops[w[1]], src[w[2]:w[2] + w[3]], src[w[4]:w[4] + w[5]], src[w[6]:w[6] + w[7]],
+                            src[w[8]:w[8] + w[9]] if w[1] == UPDATE_PUT else None, w[10] if w[1] == UPDATE_RENEW else None))
+        return verdict, status, records
 
     def collection_policies(self, table):
         """table: {(namespace, collection): root node index} -- the endorsement policy a write to that private-data collection is checked

@@ -33,6 +33,7 @@
 #include "couchval.cuh"
 #include "updates.cuh"
 #include "pvtdata.cuh"
+#include "pvtupdates.cuh"
 #include "msptable.hpp"
 #include "unknownids.cuh"
 #include "ecdsa_kernels.cuh"
@@ -340,6 +341,10 @@ struct fabgpu_ctx {
         DevArray<uint8_t> d_blob, d_flags, d_ent, d_dig; DevArray<uint32_t> d_off, d_seq, d_first, d_n, d_ctr; DevArray<int32_t> d_status;
         DevArray<unsigned long long> d_verdict; DevArray<bdev::PvRec> d_rec; DevArray<bdev::ShaJobP> d_jobs;
         uint32_t rec_hint = PV_REC_HINT;                                                 // collection records per entry the arrays are sized for
+        // fabgpu_block_pvt_updates (pvtupdates.cuh): the private batch, rebuilt by every call after the check above
+        DevArray<uint32_t> d_wfirst, d_mfirst, d_tbase, d_pctr, d_rmark, d_mark, d_okey, d_out; DevArray<bdev::PuItem> d_item, d_meta;
+        DevArray<bdev::ShaJobP> d_mjobs; DevArray<uint8_t> d_mdig; DevArray<bdev::PuKey> d_key; HostArray<uint32_t> h_pctr, h_out;
+        uint32_t w_hint = PU_W_HINT, m_hint = PU_M_HINT;                                // writes / metadata writes per entry
     } pvt[FABGPU_SLOTS];
     // fabgpu_committed_txids: the ledger's tx ids on device 0 (txidset.cuh); ledger state, so fabgpu_msp_configure keeps it.  A mutation runs
     // on `stream` under slot0_mu: it first waits for every slot's last block_decide_kernel (decide_ev) -- blocks submitted before it never
@@ -394,6 +399,7 @@ struct fabgpu_ctx {
         // or aliased as the stage left it, or found so by the build.
         int upd_slot = -1; uint64_t upd_block = 0; uint32_t upd_R = 0, upd_K = 0, upd_T = 0; bool upd_incomplete = false, upd_built = false;
         size_t upd_n[2] = {0, 0};
+        std::vector<uint8_t> upd_flags;                                                  // the final flags the stage returned (fabgpu_block_pvt_updates)
         DevArray<bdev::UdPair> d_upair; DevArray<bdev::UdKey> d_ukey; DevArray<bdev::UdSeg> d_useg; DevArray<uint8_t> d_uneed, d_utxneed, d_umeta;
         DevArray<uint32_t> d_ubase, d_umark, d_uokey, d_uomoff, d_uout, d_uctr; HostArray<uint32_t> h_uctr;
         ~StateSet() { if (table) cudaFree(table); }
@@ -3023,9 +3029,10 @@ static int cv_prepass(fabgpu_ctx* ctx, cudaStream_t st, const uint8_t* blk, cons
 }
 
 // The stage ran on the slot's block: fabgpu_block_updates may build its batch from the stage's arrays (R records, K key-table entries)
-static void upd_mark(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t R, uint32_t K, uint32_t T, bool incomplete)
+static void upd_mark(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t R, uint32_t K, uint32_t T, bool incomplete, const uint8_t* flags, size_t n)
 {
     auto& s = ctx->sv;
+    s.upd_flags.assign(flags, flags + n);
     s.upd_slot = slot; s.upd_block = block_num; s.upd_R = R; s.upd_K = K; s.upd_T = T;
     s.upd_incomplete = incomplete; s.upd_built = false; s.upd_n[0] = s.upd_n[1] = 0;
     ctx->dbs[slot].upd_ready = true;
@@ -3055,13 +3062,13 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
     if (s.broken) {                                            // nothing can be decided or applied
         for (size_t t = 0; t < n; t++) flags[t] = tv_flags[t] == bdev::TXC_VALID ? bdev::TXC_NOT_VALIDATED : tv_flags[t];
-        upd_mark(ctx, slot, block_num, 0, 0, 0, true);
+        upd_mark(ctx, slot, block_num, 0, 0, 0, true, flags, n);
         return FABGPU_OK;
     }
     int rc = sv_begin(ctx);
     if (rc) return rc;
     const uint32_t T = (uint32_t)n;
-    if (T == 0) { db.mvcc_ready = false; s.height = block_num + 1; upd_mark(ctx, slot, block_num, 0, 0, 0, false); return FABGPU_OK; }
+    if (T == 0) { db.mvcc_ready = false; s.height = block_num + 1; upd_mark(ctx, slot, block_num, 0, 0, 0, false, flags, 0); return FABGPU_OK; }
     cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
     Grow grow{ctx};
     grow(s.d_first, 4 * (size_t)T); grow(s.d_n, 4 * (size_t)T); grow(s.d_mlist, 4 * (size_t)T); grow(s.d_info, T); grow(s.d_tv, T); grow(s.d_flags, T);
@@ -3160,36 +3167,44 @@ int fabgpu_validate_mvcc(fabgpu_ctx* ctx, int slot, uint64_t block_num, const ui
     db.mvcc_ready = false;
     if (hc[1] || hc[2] != UINT32_MAX) s.open = true;           // two keys shared a tag, or a write set could not be enumerated
     else s.height = block_num + 1;
-    upd_mark(ctx, slot, block_num, R, K, T, s.open);
+    upd_mark(ctx, slot, block_num, R, K, T, s.open, flags, n);
     return FABGPU_OK;
 }
 
-// The private-data check of the slot's block, on the slot's stream under blk_mu[slot] only (no table is read or written):
-//   H2D private data, entry tables, flags -> pv_scan_kernel (per entry: collection records, SHA-256 jobs) -> host reads the record count
-//   (grows the arrays and runs the scan again on overflow) -> sha256_segments_kernel (per record: its rwset) -> pv_check_kernel (per
-//   record: the public hash, the decode) -> pv_verdict_kernel (per entry: its outcome, atomicMin of the deciding entry) -> D2H.
-int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
-                            const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4])
+// The private-data arrays' refusals that need no lock: decreasing offsets, a missing blob, sizes past 32 bits
+static int pvt_args(fabgpu_ctx* ctx, const uint8_t* pvt_blob, const uint32_t* pvt_off, size_t n_pvt)
 {
-    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS || !out) return FABGPU_E_ARG;
-    if ((n && !flags) || (n_pvt && (!pvt_off || !seq || !status))) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
     for (size_t i = 0; i < n_pvt; i++) if (pvt_off[i + 1] < pvt_off[i]) { ctx->last_error = "private-data offsets decrease"; return FABGPU_E_ARG; }
     const size_t bytes = n_pvt ? pvt_off[n_pvt] : 0;
     if (bytes && !pvt_blob) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
     if (n_pvt > UINT32_MAX || bytes > UINT32_MAX - 64) { ctx->last_error = "too much private data for one call"; return FABGPU_E_ARG; }
-    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
-    auto& db = ctx->dbs[slot]; auto& p = ctx->pvt[slot];
-    if (db.busy || !db.pvt_ready) { ctx->last_error = "the slot holds no finished block: fabgpu_validate_wait first"; return FABGPU_E_ARG; }
-    if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
-    {
-        std::vector<uint8_t> seen(n, 0);
-        for (size_t i = 0; i < n_pvt; i++) {
-            if (seq[i] >= n) { ctx->last_error = "a seq is not below the block's transaction count"; return FABGPU_E_ARG; }
-            if (seen[seq[i]]++) { ctx->last_error = "a seq is given twice"; return FABGPU_E_ARG; }
-        }
+    return FABGPU_OK;
+}
+
+// Every seq below the block's transaction count n, none given twice
+static int pvt_seqs(fabgpu_ctx* ctx, const uint32_t* seq, size_t n_pvt, size_t n)
+{
+    std::vector<uint8_t> seen(n, 0);
+    for (size_t i = 0; i < n_pvt; i++) {
+        if (seq[i] >= n) { ctx->last_error = "a seq is not below the block's transaction count"; return FABGPU_E_ARG; }
+        if (seen[seq[i]]++) { ctx->last_error = "a seq is given twice"; return FABGPU_E_ARG; }
     }
+    return FABGPU_OK;
+}
+
+// The private-data check of the slot's block, on the slot's stream under blk_mu[slot] (arguments already checked; returns synchronised):
+//   H2D private data, entry tables, flags -> pv_scan_kernel (per entry: collection records, SHA-256 jobs) -> host reads the record count
+//   (grows the arrays and runs the scan again on overflow) -> sha256_segments_kernel (per record: its rwset) -> pv_check_kernel (per
+//   record: the public hash, the decode) -> pv_verdict_kernel (per entry: its outcome, atomicMin of the deciding entry) -> D2H.
+// The records, the flags and the private data stay on the device for fabgpu_block_pvt_updates; R_out: the record count.
+static int pvt_check(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
+                     const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4], uint32_t& R_out)
+{
+    auto& db = ctx->dbs[slot]; auto& p = ctx->pvt[slot];
+    R_out = 0;
     out[0] = bdev::PV_OK; out[1] = out[2] = out[3] = -1;
     if (n_pvt == 0) return FABGPU_OK;
+    const size_t bytes = pvt_off[n_pvt];
     const uint32_t E = (uint32_t)n_pvt, T = (uint32_t)n;
     CK(ctx, cudaSetDevice(ctx->devs[0].id));
     cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
@@ -3249,7 +3264,23 @@ int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, siz
         out[0] = mismatch ? bdev::PV_MISMATCH : bdev::PV_UNDET; out[1] = (int32_t)s;
         out[2] = mismatch ? es[1] : -1; out[3] = mismatch ? es[2] : -1;
     }
+    R_out = R;
     return FABGPU_OK;
+}
+
+int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
+                            const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4])
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS || !out) return FABGPU_E_ARG;
+    if ((n && !flags) || (n_pvt && (!pvt_off || !seq || !status))) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    if (int rc = pvt_args(ctx, pvt_blob, pvt_off, n_pvt)) return rc;
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    auto& db = ctx->dbs[slot];
+    if (db.busy || !db.pvt_ready) { ctx->last_error = "the slot holds no finished block: fabgpu_validate_wait first"; return FABGPU_E_ARG; }
+    if (n != db.T) { ctx->last_error = "n is not the block's transaction count"; return FABGPU_E_ARG; }
+    if (int rc = pvt_seqs(ctx, seq, n_pvt, n)) return rc;
+    uint32_t R;
+    return pvt_check(ctx, slot, flags, n, pvt_blob, pvt_off, seq, n_pvt, status, out, R);
 }
 
 int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, size_t cap, size_t* n_out)
@@ -3382,6 +3413,135 @@ int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t
         if (m) CK(ctx, cudaMemcpyAsync(meta, s.d_umeta.get(), m, cudaMemcpyDeviceToHost, st));
         CK(ctx, cudaStreamSynchronize(st));
     }
+    return FABGPU_OK;
+}
+
+// Builds the private update batch after pvt_check left its records on the device (on `slot`'s stream; returns synchronised).  complete:
+// 0 when the peer builds it itself; n_rec: the records, whose words are in p.h_out.
+//   pu_list_kernel (per entry: writes and metadata writes of a VALID entry that passed; the host reads the counts, grows the arrays and
+//   runs it again on overflow) -> sha256_segments_kernel (per metadata write: its key) -> pu_base_kernel (one CTA: transaction-order
+//   positions) -> pu_key_kernel (per item: the key table, the last writer) -> pu_first_kernel (per item) -> pu_renew_kernel (per
+//   metadata write: the hashed record, the value to compare) -> sha256_segments_kernel (per metadata write: that value) -> pu_mark_kernel
+//   (per key) -> pu_compact_kernel (one CTA: order, totals) -> host reads the totals -> pu_emit_kernel (per record).
+static int pvu_build(fabgpu_ctx* ctx, int slot, uint32_t E, uint32_t T, int& complete, size_t& n_rec)
+{
+    auto& s = ctx->sv; auto& p = ctx->pvt[slot];
+    complete = 0; n_rec = 0;
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    const uint32_t K = s.upd_n[0] ? s.upd_K : 0, H = (uint32_t)s.upd_n[0];
+    Grow grow{ctx};
+    grow(p.d_wfirst, 4 * (size_t)E); grow(p.d_mfirst, 4 * (size_t)E); grow(p.d_tbase, 4 * (size_t)T); grow(p.d_pctr, 32); grow(p.h_pctr, 32);
+    grow(p.d_rmark, 4 * (size_t)std::max(K, 1u));
+    if (grow.rc) return grow.rc;
+    bdev::PuArrays a;
+    a.pvt = p.d_blob.get(); a.seq = p.d_seq.get(); a.n_pvt = E; a.T = T; a.flags = p.d_flags.get(); a.status = p.d_status.get();
+    a.rec = p.d_rec.get(); a.first = p.d_first.get(); a.n_rec = p.d_n.get(); a.wfirst = p.d_wfirst.get(); a.mfirst = p.d_mfirst.get();
+    a.tbase = p.d_tbase.get(); a.ctr = p.d_pctr.get(); a.seed = s.seed; a.stage_seed = s.seed; a.blk = ctx->bbs[slot].d_block.get();
+    a.stage.key = K ? s.d_key.get() : nullptr; a.stage.K_size = K;
+    a.ukey = K ? s.d_ukey.get() : nullptr; a.useg = K ? s.d_useg.get() : nullptr; a.uokey = K ? s.d_uokey.get() : nullptr; a.n_h = H;
+    a.rmark = p.d_rmark.get();
+    uint32_t* hc = p.h_pctr.get();
+    uint32_t W = 0, M = 0;
+    for (;;) {
+        const size_t W_cap = (size_t)E * p.w_hint, M_cap = (size_t)E * p.m_hint;
+        if (W_cap > UINT32_MAX || M_cap > UINT32_MAX) { ctx->last_error = "too many private writes for one call"; return FABGPU_E_ARG; }
+        Grow g2{ctx};
+        g2(p.d_item, W_cap * sizeof(bdev::PuItem)); g2(p.d_meta, M_cap * sizeof(bdev::PuItem)); g2(p.d_mjobs, M_cap * sizeof(bdev::ShaJobP));
+        g2(p.d_mdig, 32 * M_cap);
+        if (g2.rc) return g2.rc;
+        a.item = p.d_item.get(); a.W_cap = (uint32_t)W_cap; a.meta = p.d_meta.get(); a.M_cap = (uint32_t)M_cap; a.jobs = p.d_mjobs.get();
+        a.dig = p.d_mdig.get();
+        CK(ctx, cudaMemsetAsync(p.d_tbase.get(), 0, 4 * (size_t)T, st));
+        CK(ctx, cudaMemsetAsync(p.d_pctr.get(), 0, 32, st));
+        bdev::pu_list_kernel<<<(E + 63) / 64, 64, 0, st>>>(a);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(hc, p.d_pctr.get(), 12, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+        W = hc[0]; M = hc[1];
+        if (W <= W_cap && M <= M_cap) break;
+        if (W > W_cap) p.w_hint = (uint32_t)((W + E - 1) / E) + 1;        // later calls are sized for it too
+        if (M > M_cap) p.m_hint = (uint32_t)((M + E - 1) / E) + 1;
+    }
+    if (hc[2]) return FABGPU_OK;                                         // a Put of a nil value
+    uint32_t P = 64;
+    while (P < 2 * ((uint64_t)W + M)) P <<= 1;
+    Grow g3{ctx};
+    g3(p.d_key, (size_t)P * sizeof(bdev::PuKey)); g3(p.d_mark, 4 * (size_t)std::max(W, 1u)); g3(p.d_okey, 4 * ((size_t)W + H + 1));
+    if (g3.rc) return g3.rc;
+    a.key = p.d_key.get(); a.P_size = P; a.mark = p.d_mark.get(); a.out_key = p.d_okey.get();
+    CK(ctx, cudaMemsetAsync(p.d_key.get(), 0, (size_t)P * sizeof(bdev::PuKey), st));
+    CK(ctx, cudaMemsetAsync(p.d_mark.get(), 0, 4 * (size_t)std::max(W, 1u), st));
+    if (K) CK(ctx, cudaMemsetAsync(p.d_rmark.get(), 0, 4 * (size_t)K, st));
+    const ShaJob* jobs = reinterpret_cast<const ShaJob*>(p.d_mjobs.get());
+    if (M) { sha256_segments_kernel<<<(M + 127) / 128, 128, 0, st>>>(p.d_blob.get(), jobs, M, p.d_mdig.get()); ctx->launches++; }
+    bdev::pu_base_kernel<<<1, 1024, 0, st>>>(a);
+    ctx->launches++;
+    if (W + M) {
+        bdev::pu_key_kernel<<<(W + M + 255) / 256, 256, 0, st>>>(a, W, W + M);
+        bdev::pu_first_kernel<<<(W + M + 255) / 256, 256, 0, st>>>(a, W, W + M);
+        ctx->launches += 2;
+    }
+    if (M) {
+        bdev::pu_renew_kernel<<<(M + 127) / 128, 128, 0, st>>>(a, M);
+        sha256_segments_kernel<<<(M + 127) / 128, 128, 0, st>>>(p.d_blob.get(), jobs, M, p.d_mdig.get());
+        ctx->launches += 2;
+    }
+    bdev::pu_mark_kernel<<<P / 256 + 1, 256, 0, st>>>(a);
+    bdev::pu_compact_kernel<<<1, 1024, 0, st>>>(a, W);
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpyAsync(hc, p.d_pctr.get(), 20, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    if (hc[2]) return FABGPU_OK;
+    const size_t n = (size_t)hc[3] + hc[4];
+    if (n) {
+        Grow g4{ctx};
+        g4(p.d_out, n * bdev::PU_WORDS * 4); g4(p.h_out, n * bdev::PU_WORDS * 4);
+        if (g4.rc) return g4.rc;
+        a.out = p.d_out.get();
+        bdev::pu_emit_kernel<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>(a);
+        ctx->launches++;
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(p.h_out.get(), p.d_out.get(), n * bdev::PU_WORDS * 4, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+    }
+    complete = 1; n_rec = n;
+    return FABGPU_OK;
+}
+
+int fabgpu_block_pvt_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* pvt_blob, const uint32_t* pvt_off, const uint32_t* seq,
+                             size_t n_pvt, int32_t* status, int32_t out[4], uint32_t* rec, size_t rec_cap, size_t* n_out, int* complete)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    if (!out || !n_out || !complete || (rec_cap && !rec)) { ctx->last_error = "output arrays missing"; return FABGPU_E_ARG; }
+    if (n_pvt && (!pvt_off || !seq || !status)) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    if (int rc = pvt_args(ctx, pvt_blob, pvt_off, n_pvt)) return rc;
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv; auto& db = ctx->dbs[slot];
+    if (s.upd_slot != slot || s.upd_block != block_num || !db.upd_ready) {
+        ctx->last_error = "no update batch for this slot and block: fabgpu_validate_mvcc(slot, block_num) last ran on another, or a stage, a "
+                          "state version call or the slot's next submit came after it";
+        return FABGPU_E_ARG;
+    }
+    const size_t n = db.T;
+    if (int rc = pvt_seqs(ctx, seq, n_pvt, n)) return rc;
+    if (!s.upd_built) {
+        if (int rc = upd_build(ctx, slot)) return rc;
+        s.upd_built = true;
+    }
+    *n_out = 0; *complete = 0;
+    uint32_t R;
+    if (int rc = pvt_check(ctx, slot, s.upd_flags.data(), n, pvt_blob, pvt_off, seq, n_pvt, status, out, R)) return rc;
+    if (s.upd_incomplete || out[0] != bdev::PV_OK) return FABGPU_OK;
+    if (n_pvt == 0) { *complete = 1; return FABGPU_OK; }
+    int c = 0; size_t nr = 0;
+    if (int rc = pvu_build(ctx, slot, (uint32_t)n_pvt, (uint32_t)n, c, nr)) return rc;
+    if (!c) return FABGPU_OK;
+    *complete = 1; *n_out = nr;
+    const size_t w = std::min(nr, rec_cap);
+    if (w) memcpy(rec, ctx->pvt[slot].h_out.get(), w * bdev::PU_WORDS * 4);
     return FABGPU_OK;
 }
 

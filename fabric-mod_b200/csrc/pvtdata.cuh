@@ -116,7 +116,11 @@ BD_HD bool pv_read(const uint8_t* base, Seg r)
 // RangeQueryInfo{start_key = 1, end_key = 2, itr_exhausted = 3, raw_reads = 4, reads_merkle_hashes = 5}, QueryReads{kv_reads = 1},
 // QueryReadsMerkleSummary{max_degree = 1, max_level = 2, max_level_hashes = 3}, KVWrite{key = 1, is_delete = 2, value = 3},
 // KVMetadataWrite{key = 1, entries = 2}, KVMetadataEntry{name = 1, value = 2}.  false: a level does not parse, or a string is not UTF-8.
-BD_HD bool pv_decode(const uint8_t* base, Seg rw)
+// on_write(field, body) is handed each KVWrite (field 3) and KVMetadataWrite (field 4) in wire order once its level has been read -- the
+// private update batch (pvtupdates.cuh) walks the writes of rwsets the check found decodable; the check itself passes none.
+struct PvNoWrites { BD_HD void operator()(uint32_t, Seg) const {} };
+template <typename W = PvNoWrites>
+BD_HD bool pv_decode(const uint8_t* base, Seg rw, W on_write = W())
 {
     bool ok = true;
     auto none = [](uint32_t, Seg) {};
@@ -130,13 +134,16 @@ BD_HD bool pv_decode(const uint8_t* base, Seg rw)
                     else if (h == 4) ok = scan_msg(base, c, BD_F(1), 0, [&](uint32_t, Seg kv) { ok = ok && pv_read(base, kv); }) && ok;
                     else ok = scan_msg(base, c, BD_F(3), BD_F(1) | BD_F(2), none);
                 }) && ok;
-            else if (g == 3)
+            else if (g == 3) {
                 ok = scan_msg(base, b, BD_F(1) | BD_F(3), BD_F(2), [&](uint32_t h, Seg c) { if (h == 1) ok = ok && pv_str(base, c); }) && ok;
-            else
+                if (ok) on_write(g, b);
+            } else {
                 ok = scan_msg(base, b, BD_F(1) | BD_F(2), 0, [&](uint32_t h, Seg c) {
                     if (h == 1) ok = ok && pv_str(base, c);
                     else ok = ok && scan_msg(base, c, BD_F(1) | BD_F(2), 0, [&](uint32_t q, Seg d) { if (q == 1) ok = ok && pv_str(base, d); });
                 }) && ok;
+                if (ok) on_write(g, b);
+            }
         })) return false;
     return ok;
 }

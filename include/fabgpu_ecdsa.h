@@ -509,8 +509,8 @@ int fabgpu_state_database(fabgpu_ctx* ctx, int kind);
  *   slot's lock only, touches no table, and returns with the stream synchronised; the caller's arrays are not referenced afterwards.
  *   FABGPU_E_ARG, with a fabgpu_last_error text and nothing enqueued, for a slot without a finished block, n other than the block's
  *   transaction count, a seq >= n or given twice, NULL arrays with a count > 0, and decreasing offsets.
- *   Not restated: the private update batch, incrementPvtdataVersionIfNeeded, the gossip coordinator's filtering, eligibility and
- *   missing-data bookkeeping. */
+ *   The private update batch and incrementPvtdataVersionIfNeeded are built by fabgpu_block_pvt_updates, which runs this check itself
+ *   with the MVCC stage's flags.  Not restated: the gossip coordinator's filtering, eligibility and missing-data bookkeeping. */
 int fabgpu_validate_pvtdata(fabgpu_ctx* ctx, int slot, const uint8_t* flags, size_t n, const uint8_t* pvt_blob, const uint32_t* pvt_off,
                             const uint32_t* seq, size_t n_pvt, int32_t* status, int32_t out[4]);
 /* The identities the slot's finished block looked up in the MSP table and did not find (creators and endorsers with a signature
@@ -537,7 +537,8 @@ int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, si
  * count and n_out[1] the metadata bytes; at most meta_cap bytes go to meta.  *complete = 1 when the batch is the block's; 0 with no
  * records (the peer builds the batch itself) when a flag is 254 after the stage, the stage left the block open, two digests shared a
  * tag, the table was broken, a record's metadata entries are not canonical (name = 1 then value = 2, each at most once and non-empty,
- * minimal lengths, nothing else), or a record depends on a key the table marks unknown.  The private update batch is not built.
+ * minimal lengths, nothing else), or a record depends on a key the table marks unknown.  The private update batch is
+ * fabgpu_block_pvt_updates'.
  * Call it any number of times after fabgpu_validate_mvcc(slot, block_num) returned, until the next fabgpu_validate_mvcc, the next
  * fabgpu_state_versions* call or the slot's next submit; the first call builds the batch on the slot's stream, later ones copy it.
  * Returns synchronised.  FABGPU_E_ARG, with nothing enqueued, when slot and block_num are not those the stage last ran on, after one of
@@ -550,6 +551,44 @@ int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, si
 #define FABGPU_SRC_COMMITTED 2
 int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t* rec, size_t rec_cap, uint8_t* meta, size_t meta_cap,
                          size_t n_out[2], int* complete);
+/* The block's private update batch, as validateAndPreparePvtBatch leaves it in PvtUpdates (validation/batch_preparer.go:119-160,
+ * 341-410), for the block fabgpu_validate_mvcc(slot, block_num) last ran on.  The private data is passed as fabgpu_validate_pvtdata takes
+ * it; the call runs that check itself with the stage's own final flags and fills status and out exactly as fabgpu_validate_pvtdata would
+ * with them (a peer that runs the MVCC stage calls this instead).  The batch is defined over those flags only: for each transaction left
+ * VALID whose entry the check passed (not skipped), in transaction order,
+ *   every KVWrite of its KVRWSets, through namespaces, collections and writes in wire order, is a Put of its value (a Delete when
+ *     is_delete) at (block_num, tx); a later write of the same (namespace, collection, key) replaces an earlier one, within one
+ *     transaction too;
+ *   every KVMetadataWrite's (namespace, collection, key) is collected; for each one whose hashed key (SHA-256 of the key) the hashed
+ *     batch of fabgpu_block_updates PUTs at (block_num, h), incrementPvtdataVersionIfNeeded (:360-393) renews the latest private value
+ *     -- the batch's, else the committed one -- to version (block_num, h) when its version differs and SHA-256 of it equals that PUT's
+ *     value hash.  A hashed DELETE, or no hashed record, never renews.
+ * Records of FABGPU_PVT_UPDATE_WORDS uint32 words go to rec, at most rec_cap of them; *n_out gets the full count:
+ *   [0] tx (the version's tx_num: the deciding write's, or for a renewal the hashed PUT's)
+ *   [1] op: FABGPU_UPDATE_PUT, FABGPU_UPDATE_DELETE or FABGPU_UPDATE_RENEW
+ *   [2], [3] namespace; [4], [5] collection; [6], [7] key; [8], [9] the value (PUT; 0 otherwise): offsets and lengths in pvt_blob
+ *   [10] RENEW: the index of the hashed PUT record in fabgpu_block_updates' records; UINT32_MAX otherwise.
+ * PUT and DELETE records are the batch: each key at most once, ordered by the tx of the write that decides it, then by the position of
+ * that transaction's first write of the key among its entry's writes.  A renewal the device decided (the latest value is in the batch)
+ * is such a PUT with [0] = the hashed record's tx, in the same place.  RENEW records follow, in the order of their hashed records: a
+ * metadata-written key not in the private batch whose hashed key the hashed batch PUTs.  The peer resolves each with one
+ * GetPrivateData(ns, coll, key): when a value is present, its version is not (block_num, [0]), and SHA-256(value) equals the hashed
+ * record's value hash (its bytes in the block, or GetValueHash for FABGPU_SRC_COMMITTED), it puts that value at (block_num, [0]);
+ * otherwise nothing.  So the block's commit batch is fabgpu_block_updates' records, these records and one GetPrivateData per RENEW.
+ * *complete = 1 when the batch is the block's; 0 with no records (the peer builds it itself; status and out are still filled) when the
+ * public and hashed batch is incomplete (fabgpu_block_updates' reasons), out[0] != 0 (the reference fails the commit), a VALID entry
+ * has a KVWrite that is not a delete and has no value field (PutValAndMetadata panics on a nil value; a present but empty value is
+ * []byte{} and commits), two key digests shared a tag, a renewal the device decides needs a hashed value hash from the committed state,
+ * or a renewal would put a private DELETE's nil value (the hashed value hash is SHA-256 of the empty string: the reference panics).
+ * Call window and locks as fabgpu_block_updates: after fabgpu_validate_mvcc(slot, block_num), until the next stage, state version call
+ * or submit of the slot; it builds the public and hashed batch first if no call did (a later fabgpu_block_updates only copies it).  The
+ * private batch is rebuilt on every call, on the slot's stream; returns synchronised, and the caller's arrays are not referenced
+ * afterwards.  FABGPU_E_ARG, with a fabgpu_last_error text and nothing enqueued, for fabgpu_block_updates' refusals, a seq >= the
+ * block's transaction count or given twice, decreasing offsets, NULL outputs, and NULL inputs with a count > 0. */
+#define FABGPU_PVT_UPDATE_WORDS 11
+#define FABGPU_UPDATE_RENEW 3
+int fabgpu_block_pvt_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* pvt_blob, const uint32_t* pvt_off, const uint32_t* seq,
+                             size_t n_pvt, int32_t* status, int32_t out[4], uint32_t* rec, size_t rec_cap, size_t* n_out, int* complete);
 /* flags[i] receives the validation code of transaction i; *n_tx_out the number of transactions. */
 int fabgpu_validate_block(fabgpu_ctx* ctx, const uint8_t* block, size_t block_len, uint8_t* flags, size_t flags_cap, size_t* n_tx_out);
 /* Same for a caller that already holds Block.Data.Data as separate byte strings (the Go validator does): `blob` is their
