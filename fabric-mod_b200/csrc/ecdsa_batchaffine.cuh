@@ -1,6 +1,6 @@
 // Batch-affine accumulation for the key-table verification path: the GPU restatement of the sum
 //   R = sum_j T_G[j][u1_j] + sum_j T_Q[j][u2_j]
-// that ecdsa_verify_one_cached (ecdsa_verify.cuh) computes with 28 Jacobian mixed additions of 11 field multiplications each.
+// that ecdsa_verify_one_cached (ecdsa_verify.cuh) computes with 28 XYZZ mixed additions of 10 field multiplications each.
 // (What it replaces in the reference: the CombinedMult behind Go's ecdsa.Verify at bccsp/sw/ecdsa.go:56.)
 //
 // Every operand is an AFFINE table entry, so the additions can be affine too -- lambda = (y2 - y1)/(x2 - x1), 1M + 1S + 1M -- if the

@@ -286,6 +286,17 @@ ecdsa_prep_kernel(const int32_t* __restrict__ key_slot, const uint8_t* __restric
     scal[3 * (size_t)stride + idx] = make_uint4(u2.v[4], u2.v[5], u2.v[6], u2.v[7]);
 }
 
+// The scalars ecdsa_prep_kernel wrote for signature idx, read where the chain uses them: u2 is not held in registers through u1's windows.
+struct ScalRows {
+    const uint4* scal;
+    uint32_t stride, idx;
+    __device__ u256 operator()(int t) const
+    {
+        const uint4 a = __ldg(scal + (size_t)(2 * t) * stride + idx), b = __ldg(scal + (size_t)(2 * t + 1) * stride + idx);
+        return u256_const(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w);
+    }
+};
+
 #ifndef FAB_CACHED_THREADS
 #define FAB_CACHED_THREADS 512        // largest CTA the kernel may be launched with (launch_verify picks 128 / 256 / 512)
 #endif
@@ -308,10 +319,11 @@ ecdsa_verify_cached_kernel(const int32_t* __restrict__ key_slot, const uint4* __
     if (idx < n) {
         const int32_t slot = key_slot[idx];
         if (slot >= 0) {
-            const uint4 a = scal[idx], b = scal[stride + idx], c = scal[2 * (size_t)stride + idx], d = scal[3 * (size_t)stride + idx];
-            const u256 u1 = u256_const(a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w), u2 = u256_const(c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w);
-            if (!u256_is_zero(u2))                                  // u2 = 0: r or s outside [1, n-1]
-                res = ecdsa_chain_cached(qtab + (size_t)slot * (FAB_Q_WINDOWS * FAB_Q_ENTRIES), u1, u2, load_be32(r + (size_t)idx * 32), gtab);
+            const ScalRows sc = {scal, stride, idx};
+            if (!u256_is_zero(sc(1))) {                             // u2 = 0: r or s outside [1, n-1]
+                const xyzz acc = ecdsa_chain_cached(qtab + (size_t)slot * (FAB_Q_WINDOWS * FAB_Q_ENTRIES), sc, gtab);
+                res = final_check(acc, load_be32(r + (size_t)idx * 32));     // r loaded after the chain: no registers held through it
+            }
         }
     }
     const uint32_t vmask = __ballot_sync(0xffffffffu, res == V_VALID);

@@ -11,7 +11,8 @@
 //          (ceil(256/FAB_WG) mixed additions, no doublings);
 //   u2*Q : keys with a table (ecdsa_verify_one_cached): FAB_WQ-bit unsigned windows over the key's own table;
 //          keys without (ecdsa_verify_one): signed 5-bit Booth windows, 16-entry Jacobian table of 1Q..16Q per signature.
-// The final comparison avoids the field inversion: R.x == r' * R.Z^2 for r' in {r, r+n (if < p)}.
+// The window chains accumulate in XYZZ coordinates (p256_point.cuh), the generic kernel in Jacobian ones.
+// The final comparison avoids the field inversion: R.x == r' * R.ZZ (Jacobian: r' * R.Z^2) for r' in {r, r+n (if < p)}.
 #pragma once
 #include "p256_point.cuh"
 #include "p256_modinv.cuh"
@@ -134,14 +135,11 @@ FAB_HD jac add_fixed_base(jac r, const u256& k, const aff* gtab)
     return r;
 }
 
-// Accept iff acc != infinity and acc.x mod n == r, without leaving Jacobian coordinates:
-// X == r' * Z^2 for r' in {r, r + n (only when r + n < p)}.
-FAB_HD uint32_t final_check(const jac& acc, const u256& r)
+// x = X / zz of a finite point: valid iff x mod n == r, i.e. X == r' * zz for r' in {r, r + n (only when r + n < p)}.
+FAB_HD uint32_t x_check(const u256& X, const u256& zz, const u256& r)
 {
-    if (jac_is_infinity(acc)) return V_INVALID;       // Go: x == 0 && y == 0 -> false
     const u256 n = sc_n();
-    const u256 z2 = fe_sqr(acc.Z);
-    if (u256_eq(fe_mul(fe_to_mont(r), z2), acc.X)) return V_VALID;
+    if (u256_eq(fe_mul(fe_to_mont(r), zz), X)) return V_VALID;
     if (u256_lt(r, p_minus_n())) {                    // x mod n == r also when x = r + n < p
         u256 rn; uint32_t c = 0;
 #pragma unroll
@@ -151,9 +149,21 @@ FAB_HD uint32_t final_check(const jac& acc, const u256& r)
             const uint32_t t2 = t + c; const uint32_t c2 = t2 < t;
             rn.v[i] = t2; c = c1 | c2;
         }
-        if (u256_eq(fe_mul(fe_to_mont(rn), z2), acc.X)) return V_VALID;
+        if (u256_eq(fe_mul(fe_to_mont(rn), zz), X)) return V_VALID;
     }
     return V_INVALID;
+}
+
+// Accept iff acc != infinity (Go: x == 0 && y == 0 -> false) and acc.x mod n == r, without leaving the projective coordinates.
+FAB_HD uint32_t final_check(const jac& acc, const u256& r)
+{
+    if (jac_is_infinity(acc)) return V_INVALID;
+    return x_check(acc.X, fe_sqr(acc.Z), r);
+}
+FAB_HD uint32_t final_check(const xyzz& acc, const u256& r)
+{
+    if (u256_is_zero(acc.ZZ)) return V_INVALID;
+    return x_check(acc.X, acc.ZZ, r);
 }
 
 // All five inputs are plain 256-bit integers (e already formed by hashToInt: leftmost 32 digest bytes, left-padded).
@@ -191,23 +201,30 @@ FAB_HD void ecdsa_u1u2(const u256& e, const u256& r, const u256& w, u256& u1, u2
     u2 = sc_mul(r, w);
 }
 
-// The second half of a verification when the public key has a precomputed window table (fabgpu_keys_register): from the
-// scalars u1, u2, R = u1*G + u2*Q with u2*Q fixed-base too -- FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions in total, no
-// doublings, no per-signature table -- and the final check against r.  The key was checked to be a curve point when its table
-// was built.  ecdsa_verify_cached_kernel runs this on the scalars ecdsa_prep_kernel computed; ecdsa_verify_one_cached below is
-// the whole verification for one signature.
-FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& u2, const u256& r, const aff* gtab)
+// The two scalars of a chain held in registers: scalar(0) = u1, scalar(1) = u2.
+struct ChainScalars {
+    u256 u1, u2;
+    FAB_HD u256 operator()(int t) const { return t ? u2 : u1; }
+};
+
+// The point of a verification when the public key has a precomputed window table (fabgpu_keys_register): from the scalars u1, u2,
+// R = u1*G + u2*Q with u2*Q fixed-base too -- FAB_G_WINDOWS + FAB_Q_WINDOWS mixed additions in total, no doublings, no per-signature
+// table.  The caller checks R against r (final_check).  The key was checked to be a curve point when its table was built.
+// ecdsa_verify_cached_kernel runs this on the scalars ecdsa_prep_kernel computed, read from memory where the chain needs them
+// (Scalars: a functor, scalar(t) for t = 0, 1); ecdsa_verify_one_cached below is the whole verification for one signature.
+template <class Scalars> FAB_HD xyzz ecdsa_chain_cached(const aff* qtab, const Scalars& scalar, const aff* gtab)
 {
     // One loop over both tables -- 12 windows of u1 in the generator's table, then 16 windows of u2 in the key's table -- so that
     // the kernel holds a single copy of the point addition (expanded in place when FAB_CACHED_INLINE).
-    jac acc = jac_infinity();
+    xyzz acc = xyzz_infinity();
 #if defined(__CUDA_ARCH__) && FAB_JAC_L2PREFETCH
     // every table entry this signature will gather, requested from the L2 up front (the tables are HBM-resident: 3.2 GB + 64 MiB per key)
 #pragma unroll 1
     for (int t = 0; t < 2; t++) {
         uint32_t kk[8];
+        const u256 k = scalar(t);
 #pragma unroll
-        for (int i = 0; i < 8; i++) kk[i] = t ? u2.v[i] : u1.v[i];
+        for (int i = 0; i < 8; i++) kk[i] = k.v[i];
         const aff* tab = t ? qtab : gtab;
         const uint32_t wbits = t ? FAB_WQ : FAB_WG, entries = (1u << wbits) - 1u;
         const int windows = t ? FAB_Q_WINDOWS : FAB_G_WINDOWS;
@@ -223,13 +240,14 @@ FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& 
 #endif
     // cur: this window's entry (nullptr for a zero digit).  Each pass forms the NEXT window's entry address once, for its prefetch and
     // as the next pass's gather address.
-    const uint32_t d0 = u1.v[0] & (uint32_t)FAB_G_ENTRIES;
+    const uint32_t d0 = scalar(0).v[0] & (uint32_t)FAB_G_ENTRIES, dq0 = scalar(1).v[0] & (uint32_t)FAB_Q_ENTRIES;
     const aff* cur = d0 ? gtab + (d0 - 1) : nullptr;
 #pragma unroll 1
     for (int t = 0; t < 2; t++) {
         uint32_t kk[8];
+        const u256 k = scalar(t);
 #pragma unroll
-        for (int i = 0; i < 8; i++) kk[i] = t ? u2.v[i] : u1.v[i];
+        for (int i = 0; i < 8; i++) kk[i] = k.v[i];
         const aff* tab = t ? qtab : gtab;
         const uint32_t wbits = t ? FAB_WQ : FAB_WG, entries = (1u << wbits) - 1u;
         const int windows = t ? FAB_Q_WINDOWS : FAB_G_WINDOWS;
@@ -241,17 +259,17 @@ FAB_HD uint32_t ecdsa_chain_cached(const aff* qtab, const u256& u1, const u256& 
             // the entry of the next window (or the first window of the key's table)
             const aff* nx = nullptr;
             if (j + 1 < windows) { const uint32_t dn = kk[0] & entries; if (dn) nx = tab + (size_t)(j + 1) * entries + (dn - 1); }
-            else if (t == 0) { const uint32_t dn = u2.v[0] & ((1u << FAB_WQ) - 1u); if (dn) nx = qtab + (dn - 1); }
+            else if (t == 0 && dq0) nx = qtab + (dq0 - 1);
 #if defined(__CUDA_ARCH__) && FAB_JAC_NEXT_PREFETCH
             // requested from the L2 while this addition runs: the tables are HBM-resident, so without it one DRAM round trip per
             // addition is exposed
             if (nx) asm volatile("prefetch.global.L2 [%0];" :: "l"(nx));
 #endif
-            if (cur) acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, load_aff_nc(cur));
+            if (cur) acc = xyzz_add_aff_t<FAB_CACHED_INLINE != 0>(acc, load_aff_nc(cur));
             cur = nx;
         }
     }
-    return final_check(acc, r);
+    return acc;
 }
 
 // One signature through a key's window table, scalars included (one inversion of its own).
@@ -264,9 +282,9 @@ FAB_HD uint32_t ecdsa_verify_one_cached(const aff* qtab, const u256& e, const u2
 #else
     const u256 w = sc_inv_to_mont(s);
 #endif
-    u256 u1, u2;
-    ecdsa_u1u2(e, r, w, u1, u2);
-    return ecdsa_chain_cached(qtab, u1, u2, r, gtab);
+    ChainScalars sc;
+    ecdsa_u1u2(e, r, w, sc.u1, sc.u2);
+    return final_check(ecdsa_chain_cached(qtab, sc, gtab), r);
 }
 
 // ---- small key tables: the tier between "never seen" and a 64 MiB window table --------------------------------------------------
@@ -333,7 +351,7 @@ FAB_HD uint32_t ecdsa_verify_one_small(const aff* stab, const u256& e, const u25
 #endif
     const u256 u1 = sc_mul(sc_reduce_once(e), w);
     const u256 u2 = sc_mul(r, w);
-    jac acc = jac_infinity();
+    xyzz acc = xyzz_infinity();
 #pragma unroll 1
     for (int t = 0; t < 2; t++) {
         uint32_t kk[8];
@@ -357,7 +375,7 @@ FAB_HD uint32_t ecdsa_verify_one_small(const aff* stab, const u256& e, const u25
             if (d) {
                 aff pt = load_aff_nc(tab + (size_t)j * stride + (d - 1));
                 if (neg) pt.y = fe_neg(pt.y);
-                acc = jac_add_aff_t<FAB_CACHED_INLINE != 0>(acc, pt);
+                acc = xyzz_add_aff_t<FAB_CACHED_INLINE != 0>(acc, pt);
             }
         }
     }

@@ -1,5 +1,5 @@
-// P-256 group law in Jacobian coordinates over the Montgomery field of p256_fe.cuh.
-// Infinity is Z == 0.  All routines are complete: P = Q, P = -Q and infinity operands are handled, because
+// P-256 group law in Jacobian coordinates over the Montgomery field of p256_fe.cuh, and the XYZZ mixed addition of the window chains.
+// Infinity is Z == 0 (XYZZ: ZZ == 0).  All routines are complete: P = Q, P = -Q and infinity operands are handled, because
 // the reference's verifier (Go crypto/elliptic CombinedMult behind bccsp/sw/ecdsa.go:56) is complete and the
 // bitmask must match it on adversarial inputs too (SURVEY.md A.5 items 6-7).
 #pragma once
@@ -102,6 +102,53 @@ template <bool INL> FAB_HD jac jac_add_aff_t(const jac& p, const aff& q)
     return r;
 }
 FAB_HD jac jac_add_aff(const jac& p, const aff& q) { return jac_add_aff_t<false>(p, q); }
+
+// XYZZ coordinates for the window chains, which only ever add affine table points into one accumulator: x = X / ZZ, y = Y / ZZZ,
+// ZZ^3 = ZZZ^2.  Infinity is ZZ == 0.  A mixed addition needs no Z1^2, and its products sit four levels deep instead of seven.
+struct xyzz { u256 X, Y, ZZ, ZZZ; };     // Montgomery form
+
+FAB_HD xyzz xyzz_infinity() { xyzz r; r.X = fe_one(); r.Y = fe_one(); r.ZZ = u256_zero(); r.ZZZ = u256_zero(); return r; }
+
+// The P = 0 cases of xyzz_add_aff_t: the accumulator is q itself (R = 0) -> 2q, or -q -> infinity.  Out of line and by value for
+// the reasons given at jac_add_h_zero; it needs only q, so the accumulator is not copied out at all.
+#if defined(__CUDA_ARCH__)
+__device__ __noinline__
+#else
+inline
+#endif
+xyzz xyzz_add_p_zero(aff q, u256 rr)
+{
+    if (!u256_is_zero(rr)) return xyzz_infinity();
+    const jac d = jac_double(jac_from_aff(q));
+    xyzz r;
+    r.X = d.X; r.Y = d.Y;
+    r.ZZ = fe_sqr(d.Z);
+    r.ZZZ = fe_mul(r.ZZ, d.Z);
+    return r;
+}
+
+// Mixed addition (madd-2008-s, Z2 = 1): 8M + 2S + 7 additive ops.  INL: field multiplications expanded in place (fe_mul_t).
+// The ZZ3 / ZZZ3 pair goes last: issued before the Y3 pair, it cost the key-table kernel a local frame and 1 % of its time.
+template <bool INL> FAB_HD xyzz xyzz_add_aff_t(const xyzz& p, const aff& q)
+{
+    if (u256_is_zero(p.ZZ)) { xyzz r; r.X = q.x; r.Y = q.y; r.ZZ = fe_one(); r.ZZZ = fe_one(); return r; }
+    u256 u2, s2;
+    fe_mul2_t<INL>(q.x, p.ZZ, q.y, p.ZZZ, u2, s2);          // U2 = x2 ZZ1 ; S2 = y2 ZZZ1
+    const u256 pe = fe_sub(u2, p.X);
+    const u256 rr = fe_sub(s2, p.Y);
+    if (u256_is_zero(pe)) return xyzz_add_p_zero(q, rr);
+    const u256 pp = fe_sqr_t<INL>(pe);
+    const u256 r2 = fe_sqr_t<INL>(rr);
+    u256 ppp, qq;
+    fe_mul2_t<INL>(pe, pp, p.X, pp, ppp, qq);               // PPP = P PP ; Q = X1 PP
+    xyzz r;
+    r.X = fe_sub(fe_sub(r2, ppp), fe_dbl(qq));
+    u256 t, yp;
+    fe_mul2_t<INL>(rr, fe_sub(qq, r.X), p.Y, ppp, t, yp);   // R (Q - X3) ; Y1 PPP
+    r.Y = fe_sub(t, yp);
+    fe_mul2_t<INL>(p.ZZ, pp, p.ZZZ, ppp, r.ZZ, r.ZZZ);      // ZZ3 = ZZ1 PP ; ZZZ3 = ZZZ1 PPP
+    return r;
+}
 
 // y^2 == x^3 - 3x + b  (x, y already in Montgomery form and < p)
 FAB_HD bool aff_on_curve(const aff& a)
