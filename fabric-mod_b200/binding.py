@@ -40,7 +40,7 @@ EXPORTS = [
     "fabgpu_state_versions", "fabgpu_state_versions_update", "fabgpu_state_versions_info", "fabgpu_validate_mvcc",
     "fabgpu_state_versions_indexed", "fabgpu_state_index_info", "fabgpu_state_database", "fabgpu_test_couch_values",
     "fabgpu_validate_pvtdata", "fabgpu_msp_identities_add", "fabgpu_block_unknown_identities", "fabgpu_block_updates",
-    "fabgpu_block_pvt_updates",
+    "fabgpu_block_pvt_updates", "fabgpu_block_update_bytes",
 ]
 
 
@@ -518,6 +518,25 @@ class Context:
             out.append((w[0], "put" if w[1] == UPDATE_PUT else "del", bytes(src[w[4]:w[4] + w[5]]), bytes(src[w[6]:w[6] + w[7]]),
                         bytes(src[w[8]:w[8] + w[9]]), value, md))
         return out
+
+    def block_update_bytes(self, slot, block_num, committed=()):
+        """The bytes deterministicBytesForPubAndHashUpdates returns for the update batch of the block validate_mvcc(slot, block_num) last
+        ran on (fabgpu_block_update_bytes): the input of the block's commit hash.  committed: the values of block_updates' COMMITTED-value
+        records, in record order (GetState / GetValueHash).  bytes, or None when incomplete and the peer builds them itself."""
+        committed = [bytes(v) for v in committed]
+        blob, off = _blob(committed)
+        n = ctypes.c_size_t(0)
+        complete = ctypes.c_int(0)
+        cap = 1 << 16
+        while True:
+            out = np.zeros(cap, np.uint8)
+            self._ck(lib().fabgpu_block_update_bytes(self._h, ctypes.c_int(slot), ctypes.c_uint64(block_num), _p(blob), _p(off),
+                                                     ctypes.c_size_t(len(committed)), _p(out), ctypes.c_size_t(cap), ctypes.byref(n),
+                                                     ctypes.byref(complete)))
+            if n.value <= cap:
+                break
+            cap = n.value
+        return out[: n.value].tobytes() if complete.value else None
 
     def block_pvt_updates(self, slot, block_num, pvt):
         """The private update batch of the block validate_mvcc(slot, block_num) last ran on (fabgpu_block_pvt_updates); pvt maps SeqInBlock

@@ -34,6 +34,7 @@
 #include "updates.cuh"
 #include "pvtdata.cuh"
 #include "pvtupdates.cuh"
+#include "updatebytes.cuh"
 #include "msptable.hpp"
 #include "unknownids.cuh"
 #include "ecdsa_kernels.cuh"
@@ -402,6 +403,12 @@ struct fabgpu_ctx {
         std::vector<uint8_t> upd_flags;                                                  // the final flags the stage returned (fabgpu_block_pvt_updates)
         DevArray<bdev::UdPair> d_upair; DevArray<bdev::UdKey> d_ukey; DevArray<bdev::UdSeg> d_useg; DevArray<uint8_t> d_uneed, d_utxneed, d_umeta;
         DevArray<uint32_t> d_ubase, d_umark, d_uokey, d_uomoff, d_uout, d_uctr; HostArray<uint32_t> h_uctr;
+        // fabgpu_block_update_bytes (updatebytes.cuh): the batch's records sorted by (namespace, collection, key) -- in d_bitem or, when
+        // upd_sorted, d_bitem2 -- and each record's index among the COMMITTED-value records (upd_ncom of them), built by the first call
+        // for the batch; then per call the committed values, the KVWrites' offsets and chunks, and the bytes
+        bool upd_ordered = false; int upd_sorted = 0; uint32_t upd_ncom = 0;
+        DevArray<bdev::UbItem> d_bitem, d_bitem2; DevArray<uint32_t> d_bcidx, d_bchunk, d_bvoff, d_bctr; DevArray<unsigned long long> d_boff;
+        DevArray<uint8_t> d_bval, d_bout; HostArray<uint32_t> h_bctr; HostArray<unsigned long long> h_btot;
         ~StateSet() { if (table) cudaFree(table); }
     } sv;
     // The members above go in reverse order of declaration -- block slots and MSP copy first, then devices, then the group's tables if
@@ -3034,7 +3041,7 @@ static void upd_mark(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t R, 
     auto& s = ctx->sv;
     s.upd_flags.assign(flags, flags + n);
     s.upd_slot = slot; s.upd_block = block_num; s.upd_R = R; s.upd_K = K; s.upd_T = T;
-    s.upd_incomplete = incomplete; s.upd_built = false; s.upd_n[0] = s.upd_n[1] = 0;
+    s.upd_incomplete = incomplete; s.upd_built = false; s.upd_ordered = false; s.upd_n[0] = s.upd_n[1] = 0;
     ctx->dbs[slot].upd_ready = true;
 }
 
@@ -3413,6 +3420,128 @@ int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t
         if (m) CK(ctx, cudaMemcpyAsync(meta, s.d_umeta.get(), m, cudaMemcpyDeviceToHost, st));
         CK(ctx, cudaStreamSynchronize(st));
     }
+    return FABGPU_OK;
+}
+
+static bdev::UbArrays ubytes_arrays(fabgpu_ctx* ctx, int slot)
+{
+    auto& s = ctx->sv;
+    bdev::UbArrays a;
+    a.rec = s.d_uout.get(); a.n = (uint32_t)s.upd_n[0]; a.blk = ctx->bbs[slot].d_block.get();
+    a.item = s.upd_sorted ? s.d_bitem2.get() : s.d_bitem.get(); a.cidx = s.d_bcidx.get(); a.cval = nullptr; a.coff = nullptr;
+    a.block_num = s.upd_block; a.off = nullptr; a.chunk = nullptr; a.out = nullptr; a.ctr = s.d_bctr.get();
+    return a;
+}
+
+// The order of a complete batch's records for fabgpu_block_update_bytes, built once per batch (on `slot`'s stream; returns
+// synchronised): ub_item_kernel (per record: its sort item, whether its value is COMMITTED) -> ub_sort_kernel (one launch per merge
+// pass) -> ub_cscan_kernel (one CTA: each record's index among the COMMITTED-value records) -> host reads their count.
+static int ubytes_order(fabgpu_ctx* ctx, int slot)
+{
+    auto& s = ctx->sv;
+    const uint32_t n = (uint32_t)s.upd_n[0];
+    s.upd_sorted = 0; s.upd_ncom = 0;
+    if (s.upd_incomplete || n == 0) return FABGPU_OK;
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    Grow g{ctx};
+    g(s.d_bitem, (size_t)n * sizeof(bdev::UbItem)); g(s.d_bitem2, (size_t)n * sizeof(bdev::UbItem)); g(s.d_bcidx, 4 * (size_t)n);
+    g(s.d_bctr, 16); g(s.h_bctr, 16);
+    if (g.rc) return g.rc;
+    CK(ctx, cudaMemsetAsync(s.d_bctr.get(), 0, 16, st));
+    bdev::UbArrays a = ubytes_arrays(ctx, slot);
+    bdev::ub_item_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+    ctx->launches++;
+    bdev::UbItem* in = s.d_bitem.get(); bdev::UbItem* out = s.d_bitem2.get();
+    for (uint32_t width = 1; width < n; width <<= 1) {
+        bdev::ub_sort_kernel<<<(n + 255) / 256, 256, 0, st>>>(in, out, n, width, a.blk);
+        ctx->launches++;
+        std::swap(in, out);
+    }
+    s.upd_sorted = in == s.d_bitem2.get();
+    bdev::ub_cscan_kernel<<<1, 1024, 0, st>>>(a);
+    ctx->launches++;
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpyAsync(s.h_bctr.get(), s.d_bctr.get(), 8, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    s.upd_ncom = s.h_bctr.get()[1];
+    return FABGPU_OK;
+}
+
+// The batch's deterministic bytes (on `slot`'s stream; returns synchronised), after ubytes_order:
+//   H2D committed values -> ub_size_kernel (per sorted position: framed length, long-value chunks, UTF-8 of the names) -> ub_scan_kernel
+//   (one CTA: offsets, chunk indices, totals) -> host reads the totals -> ub_emit_kernel (one warp per position) -> ub_long_kernel (one
+//   CTA per chunk of the values over UB_SHORT bytes) -> D2H at most out_cap bytes.
+int fabgpu_block_update_bytes(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* val_blob, const uint32_t* val_off, size_t n_val,
+                              uint8_t* out, size_t out_cap, size_t* n_out, int* complete)
+{
+    if (!ctx || slot < 0 || slot >= FABGPU_SLOTS) return FABGPU_E_ARG;
+    if (!n_out || !complete || (out_cap && !out)) { ctx->last_error = "output arrays missing"; return FABGPU_E_ARG; }
+    if (n_val && !val_off) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    if (n_val >= UINT32_MAX) { ctx->last_error = "too many committed values for one call"; return FABGPU_E_ARG; }
+    for (size_t j = 0; j < n_val; j++) if (val_off[j + 1] < val_off[j]) { ctx->last_error = "committed-value offsets decrease"; return FABGPU_E_ARG; }
+    const size_t vbytes = n_val ? val_off[n_val] : 0;
+    if (vbytes && !val_blob) { ctx->last_error = "arrays missing"; return FABGPU_E_ARG; }
+    std::lock_guard<std::mutex> lk(ctx->blk_mu[slot]);
+    std::lock_guard<std::mutex> lk0(ctx->slot0_mu);
+    auto& s = ctx->sv;
+    if (s.upd_slot != slot || s.upd_block != block_num || !ctx->dbs[slot].upd_ready) {
+        ctx->last_error = "no update batch for this slot and block: fabgpu_validate_mvcc(slot, block_num) last ran on another, or a stage, a "
+                          "state version call or the slot's next submit came after it";
+        return FABGPU_E_ARG;
+    }
+    if (!s.upd_built) {
+        if (int rc = upd_build(ctx, slot)) return rc;
+        s.upd_built = true;
+    }
+    if (!s.upd_ordered) {
+        if (int rc = ubytes_order(ctx, slot)) return rc;
+        s.upd_ordered = true;
+    }
+    if (!s.upd_incomplete && n_val != s.upd_ncom) {
+        ctx->last_error = "n_val is not the number of the batch's records whose value source is FABGPU_SRC_COMMITTED";
+        return FABGPU_E_ARG;
+    }
+    *n_out = 0; *complete = 0;
+    if (s.upd_incomplete) return FABGPU_OK;
+    const uint32_t n = (uint32_t)s.upd_n[0];
+    if (n == 0) { *complete = 1; return FABGPU_OK; }
+    CK(ctx, cudaSetDevice(ctx->devs[0].id));
+    cudaStream_t st = ctx->devs[0].slot[slot].stream.get();
+    Grow g{ctx};
+    g(s.d_boff, 8 * ((size_t)n + 1)); g(s.d_bchunk, 4 * ((size_t)n + 1)); g(s.d_bval, std::max<size_t>(vbytes, 1));
+    g(s.d_bvoff, 4 * (n_val + 1)); g(s.h_btot, 16);
+    if (g.rc) return g.rc;
+    if (vbytes) CK(ctx, cudaMemcpyAsync(s.d_bval.get(), val_blob, vbytes, cudaMemcpyHostToDevice, st));
+    if (n_val) CK(ctx, cudaMemcpyAsync(s.d_bvoff.get(), val_off, 4 * (n_val + 1), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemsetAsync(s.d_bctr.get(), 0, 4, st));
+    bdev::UbArrays a = ubytes_arrays(ctx, slot);
+    a.cval = s.d_bval.get(); a.coff = s.d_bvoff.get(); a.off = s.d_boff.get(); a.chunk = s.d_bchunk.get();
+    bdev::ub_size_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+    bdev::ub_scan_kernel<<<1, 1024, 0, st>>>(a);
+    ctx->launches += 2;
+    CK(ctx, cudaGetLastError());
+    unsigned long long* ht = s.h_btot.get();
+    CK(ctx, cudaMemcpyAsync(ht, a.off + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(s.h_bctr.get(), a.chunk + n, 4, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(s.h_bctr.get() + 1, a.ctr, 4, cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    const size_t total = (size_t)ht[0]; const uint32_t chunks = s.h_bctr.get()[0];
+    if (s.h_bctr.get()[1]) return FABGPU_OK;                       // a name is not UTF-8: proto.Marshal fails
+    if (total) {
+        Grow g2{ctx};
+        g2(s.d_bout, total);
+        if (g2.rc) return g2.rc;
+        a.out = s.d_bout.get();
+        bdev::ub_emit_kernel<<<(uint32_t)(((size_t)n * 32 + 255) / 256), 256, 0, st>>>(a);
+        ctx->launches++;
+        if (chunks) { bdev::ub_long_kernel<<<chunks, 256, 0, st>>>(a); ctx->launches++; }
+        CK(ctx, cudaGetLastError());
+        const size_t w = std::min(total, out_cap);
+        if (w) CK(ctx, cudaMemcpyAsync(out, s.d_bout.get(), w, cudaMemcpyDeviceToHost, st));
+        CK(ctx, cudaStreamSynchronize(st));
+    }
+    *n_out = total; *complete = 1;
     return FABGPU_OK;
 }
 

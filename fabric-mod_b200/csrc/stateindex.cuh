@@ -41,9 +41,10 @@ BD_HD int key_cmp(const KeyRef& a, const KeyRef& b)
     return c ? c : bytes_cmp(a.key, a.kl, b.key, b.kl);
 }
 
-// The first position of arr[lo, hi) whose key is not below k (keys sorted)
-template <typename T>
-BD_HD uint64_t ri_lower(const T* arr, uint64_t lo, uint64_t hi, const uint8_t* src, const KeyRef& k)
+// The first position of arr[lo, hi) whose key is not below k (keys sorted).  R: the reference type key_ref(src, T) gives and key_cmp
+// orders -- KeyRef here, the three-part UbRef of updatebytes.cuh
+template <typename T, typename R>
+BD_HD uint64_t ri_lower(const T* arr, uint64_t lo, uint64_t hi, const uint8_t* src, const R& k)
 {
     while (lo < hi) {
         const uint64_t mid = lo + (hi - lo) / 2;
@@ -76,8 +77,9 @@ BD_HD void ri_merge_one(const T* own, uint64_t i, const T* other, uint64_t n_oth
     out[out_base + i + ri_lower(other, 0, n_other, src, key_ref(src, own[i]))] = own[i];
 }
 
-// One pass of the merge sort of n written keys: runs of `width` merge pairwise into runs of 2 width
-BD_HD void ri_sort_one(const WrittenKey* in, uint32_t i, uint32_t n, uint32_t width, const uint8_t* src, WrittenKey* out)
+// One pass of the merge sort of n distinct keys (written keys; update_bytes' records): runs of `width` merge pairwise into runs of 2 width
+template <typename T>
+BD_HD void ri_sort_one(const T* in, uint32_t i, uint32_t n, uint32_t width, const uint8_t* src, T* out)
 {
     const uint32_t r = i / width, pair = (r & ~1u) * width, partner = (r ^ 1u) * width;
     if (partner >= n) { out[i] = in[i]; return; }

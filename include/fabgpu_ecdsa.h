@@ -551,6 +551,32 @@ int fabgpu_block_unknown_identities(fabgpu_ctx* ctx, int slot, uint32_t* out, si
 #define FABGPU_SRC_COMMITTED 2
 int fabgpu_block_updates(fabgpu_ctx* ctx, int slot, uint64_t block_num, uint32_t* rec, size_t rec_cap, uint8_t* meta, size_t meta_cap,
                          size_t n_out[2], int* complete);
+/* The bytes deterministicBytesForPubAndHashUpdates (txmgr/update_batch_bytes.go:29-105) returns for the batch fabgpu_block_updates
+ * hands back for the same slot and block: the updateBatchBytes of LockBasedTxMgr.ValidateAndPrepare (lockbased_txmgr.go:220-221).
+ * The peer passes out[0 .. *n_out) to kvLedger.addBlockCommitHash (kv_ledger.go:621-632) in place of that function's result, and the
+ * block's commit hash is SHA-256(varint(len(flags)) || flags || out[0 .. *n_out) || previous commit hash) as before.  The bytes are
+ * proto.Marshal(Updates{kvwrites = 1}) of one KVWrite{namespace = 1 string, collection = 2 string, key = 3, isDelete = 4, value = 5,
+ * version_bytes = 6} per record (txmgr/updates.proto; proto3, so empty fields and a false isDelete are left out):
+ *   order: namespaces bytewise, namespace "" (the channel config) left out; within a namespace its public keys, then its collections
+ *     by name; keys bytewise (a hashed key as its 32 raw bytes);
+ *   namespace on the first KVWrite of each namespace only, collection on the first of each collection only (never on a public one);
+ *   key the record's key; isDelete for a DELETE; value the PUT's value -- the block's, or for a FABGPU_SRC_COMMITTED record the caller's
+ *     (an empty value is left out, with isDelete false); version_bytes EncodeOrderPreservingVarUint64(block_num) followed by that of the
+ *     record's tx.  Metadata is not part of the bytes.
+ * Committed values: value j is val_blob[val_off[j] .. val_off[j + 1]) and belongs to the j-th record, in fabgpu_block_updates' record
+ * order, whose value source is FABGPU_SRC_COMMITTED: what the peer reads to commit it anyway (GetState for a public key, GetValueHash
+ * for a hashed one).  n_val must be the number of such records.
+ * *n_out gets the full length; at most out_cap bytes go to out.  *complete = 1 when the bytes are the block's (an empty batch, or one
+ * of namespace "" only, gives 0 bytes); 0 with *n_out = 0 when the batch is incomplete (fabgpu_block_updates' reasons; n_val is then
+ * not checked) or an emitted namespace or collection name is not valid UTF-8 (proto.Marshal fails, and with it the reference's commit):
+ * the peer builds the bytes itself.
+ * Call window and locks as fabgpu_block_updates: after fabgpu_validate_mvcc(slot, block_num), until the next stage, state version call
+ * or submit of the slot; it builds the batch first if no call did, and the batch's order once (later calls reuse both).  Returns
+ * synchronised, and the caller's arrays are not referenced afterwards.  FABGPU_E_ARG, with a fabgpu_last_error text and nothing of its
+ * own enqueued, for fabgpu_block_updates' refusals, an n_val other than the number of FABGPU_SRC_COMMITTED records, decreasing offsets,
+ * NULL outputs, and NULL inputs with n_val > 0. */
+int fabgpu_block_update_bytes(fabgpu_ctx* ctx, int slot, uint64_t block_num, const uint8_t* val_blob, const uint32_t* val_off, size_t n_val,
+                              uint8_t* out, size_t out_cap, size_t* n_out, int* complete);
 /* The block's private update batch, as validateAndPreparePvtBatch leaves it in PvtUpdates (validation/batch_preparer.go:119-160,
  * 341-410), for the block fabgpu_validate_mvcc(slot, block_num) last ran on.  The private data is passed as fabgpu_validate_pvtdata takes
  * it; the call runs that check itself with the stage's own final flags and fills status and out exactly as fabgpu_validate_pvtdata would
